@@ -20,7 +20,9 @@
 //                             dQ_partial = dS K                      (wgmma; dS^T through shared memory)
 //                           Everything is computed TRANSPOSED (rows = keys) so that P^T and dS^T come out of the
 //                           accumulators in the register layout of a wgmma A operand.  The dQ partial tile of the
-//                           warpgroup's 64 keys is added to an fp32 accumulator in global memory (vector reductions).
+//                           warpgroup's 64 keys is added to an fp32 accumulator in global memory: D = 64 stages it
+//                           in shared memory for TMA reduce-adds issued by producer warps 1 and 2 and pipelines
+//                           the products of consecutive query tiles; D = 128 uses vector reductions from registers.
 //   3. bwd_dq_finish_kernel: fp32 accumulator * scale -> 16-bit dq (+ l2norm backward of q); writes the accumulator
 //                           back as zeros (the "zeroed" workspace is zero on entry and on exit of every call).
 // BIAS instantiation: additive attention bias (16-bit loads along the query axis) and d_bias = dS
@@ -38,21 +40,28 @@
 
 namespace fcsa {
 
+// D = 64 stages each warpgroup's dQ partial tile in shared memory for TMA reduce-adds and pipelines the
+// products of consecutive query tiles; D = 128 has neither the shared memory (two 32 KB staging tiles on top
+// of 194 KB) nor the registers (a second S^T / dP^T pair next to 128 dV / dK accumulators) for that, and keeps
+// the in-order loop with vector reductions from registers.
 template <int D>
 struct BwdCfg {
+  static constexpr bool kStaged = (D == 64);
   static constexpr int QT = 64;                           // query rows per tile
   static constexpr int kKV = 128 * D * 2;                 // bytes of the K (or V) tile
   static constexpr int kQ = QT * D * 2;                   // bytes of one Q (or dO) stage
-  static constexpr int NST = 3;                           // Q / dO / stats ring depth
+  static constexpr int NST = kStaged ? 4 : 3;             // Q / dO / stats ring depth
   static constexpr int kDS = 64 * QT * 2;                 // one warpgroup's dS^T: 64 keys x QT queries, 16-bit
+  static constexpr int kDQ = kStaged ? QT * D * 4 : 0;    // one fp32 dQ staging tile: D / 32 boxes of 32 x QT
   static constexpr int kOffK = 0;
   static constexpr int kOffV = kOffK + kKV;
   static constexpr int kOffQ = kOffV + kKV;
   static constexpr int kOffDO = kOffQ + NST * kQ;
   static constexpr int kOffDS = kOffDO + NST * kQ;        // 2 warpgroups x 2 buffers
-  static constexpr int kOffStats = kOffDS + 4 * kDS;      // NST stages x {c3, -delta} x QT floats
+  static constexpr int kOffDQ = kOffDS + 4 * kDS;         // 2 warpgroups x 2 buffers (1024-byte aligned)
+  static constexpr int kOffStats = kOffDQ + 4 * kDQ;      // NST stages x {c3, -delta} x QT floats
   static constexpr int kOffBar = kOffStats + NST * 8 * QT;
-  static constexpr int kSmem = kOffBar + 128 + 1024;
+  static constexpr int kSmem = kOffBar + 256 + 1024;
   static_assert(kSmem <= 232448, "backward kernel shared memory");
   static constexpr int kThreads = 384;                    // producer warpgroup + 2 consumer warpgroups
 };
@@ -233,9 +242,10 @@ template <typename T, int D, bool BIAS = false>
 __global__ void __launch_bounds__(384, 1)
 fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                 const __grid_constant__ CUtensorMap tm_v, const __grid_constant__ CUtensorMap tm_do,
-                const BwdArgs a) {
+                const __grid_constant__ CUtensorMap tm_dq, const BwdArgs a) {
   static_assert(D == 64 || D == 128, "head dim 64 or 128");
   using Cfg = BwdCfg<D>;
+  constexpr bool STAGED = Cfg::kStaged;
   constexpr int QT = Cfg::QT;              // query rows per tile
   constexpr int KCH = D / 64;              // 64-feature chunks of every operand tile
   constexpr int QCHUNK = QT * 128;         // bytes of one 64-feature chunk of a Q / dO stage
@@ -249,11 +259,14 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const uint32_t sQ = smem_u32(smem + Cfg::kOffQ);
   const uint32_t sDO = smem_u32(smem + Cfg::kOffDO);
   const uint32_t sDS = smem_u32(smem + Cfg::kOffDS);
+  const uint32_t sDQ = smem_u32(smem + Cfg::kOffDQ);
   const uint32_t sStats = smem_u32(smem + Cfg::kOffStats);
   const uint32_t bar0 = smem_u32(smem + Cfg::kOffBar);
   auto BAR = [&](int i) { return bar0 + 8u * i; };
-  constexpr int KV_FULL = 0, FULL = 1, EMPTY = FULL + NST, NBARS = EMPTY + NST;
-  static_assert(NBARS * 8 <= 128, "barrier area");
+  // DQ_FULL / DQ_EMPTY + 2 w + buffer: warpgroup w's dQ staging tiles (STAGED only)
+  constexpr int KV_FULL = 0, FULL = 1, EMPTY = FULL + NST, DQ_FULL = EMPTY + NST, DQ_EMPTY = DQ_FULL + 4,
+                NBARS = DQ_EMPTY + 4;
+  static_assert(NBARS * 8 <= 256, "barrier area");
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;
@@ -280,6 +293,10 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     for (int s = 0; s < NST; ++s) {
       mbar_init(BAR(FULL + s), 1);
       mbar_init(BAR(EMPTY + s), 256);
+    }
+    for (int s = 0; s < 4; ++s) {
+      mbar_init(BAR(DQ_FULL + s), 128);
+      mbar_init(BAR(DQ_EMPTY + s), 1);
     }
     fence_mbar_init();
   }
@@ -311,6 +328,22 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         }
         bulk_load_1d(sStats + st * 8 * QT, a.stats + ((long long)bh * a.nqt + qt) * 2 * QT, 8 * QT, BAR(FULL + st));
       }
+    } else if (STAGED && (warp == 1 || warp == 2) && elect_one()) {
+      // dQ reducer of consumer warpgroup warp - 1: each staged 64 x D fp32 tile is added into the accumulator
+      // by TMA (rows at or beyond Nq lie outside the tensor map and are not written)
+      const int rw = warp - 1;
+      if (rw == 0) tma_prefetch_desc(&tm_dq);
+      for (int i = 0; i < NI; ++i) {
+        const int sb = i & 1;
+        const uint32_t src = sDQ + (2 * rw + sb) * Cfg::kDQ;
+        mbar_wait(BAR(DQ_FULL + 2 * rw + sb), (i >> 1) & 1);
+#pragma unroll
+        for (int c = 0; c < D / 32; ++c) tma_reduce_add_4d(&tm_dq, src + c * (QT * 128), c * 32, (i_lo + i) * QT, h, b);
+        bulk_commit();
+        bulk_wait_read<0>();
+        mbar_arrive(BAR(DQ_EMPTY + 2 * rw + sb));
+      }
+      bulk_wait<0>();                          // every reduction performed before the dq finish kernel reads
     }
     return;
   }
@@ -319,7 +352,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   reg_alloc<kConsumerRegs>();
   const int w = wg - 1;                       // keys key0 + 64 w .. + 63
   const int wl = warp & 3;
-  const int kr = 16 * wl + (lane >> 2);       // this thread's key rows inside the warpgroup's 64: kr, kr + 8
+  const int r8 = lane >> 2;                   // row inside every 8-row group of an accumulator
+  const int kr = 16 * wl + r8;                // this thread's key rows inside the warpgroup's 64: kr, kr + 8
   const int cq = 2 * (lane & 3);              // first of the thread's two columns inside every 8-column block
   int key_g[2];
   bool key_ok[2];
@@ -329,22 +363,15 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     key_ok[hf] = key_g[hf] < a.Nk;
     if (a.has_mask && key_ok[hf]) key_ok[hf] = a.mask[(long long)b * a.mask_sb + key_g[hf]] != 0;
   }
+  // the warpgroup's keys are all real and unmasked: only query tiles crossing the causal diagonal or the end
+  // of the sequence need per-element selects
+  const bool keys_full = !a.has_mask && key0 + 64 * w + 64 <= a.Nk;
   const uint32_t sKw = sK + w * 64 * 128, sVw = sV + w * 64 * 128;    // the warpgroup's 64 rows of every chunk
+  const uint32_t ds_thr = kr * 128 + cq * 2;  // the thread's dS^T words: + 1024 hf + 16 (column block ^ r8)
   const float c1 = a.c1;
 
-  float dv[D / 2], dk[D / 2];
-#pragma unroll
-  for (int i = 0; i < D / 2; ++i) dv[i] = dk[i] = 0.f;
-  if (NI > 0) mbar_wait(BAR(KV_FULL), 0);
-
-  for (int i = 0; i < NI; ++i) {
-    const int st = i % NST, qt = i_lo + i;
-    const int row0 = qt * QT;
-    const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
-    mbar_wait(BAR(FULL + st), (i / NST) & 1);
-
-    // ---- S^T = K Q^T and dP^T = V dO^T (64 keys x QT queries each) ----
-    float s[QT / 2], dp[QT / 2];
+  // S^T = K Q^T and dP^T = V dO^T (64 keys x QT queries each), one commit group
+  auto issue_s_dp = [&](float (&s)[QT / 2], float (&dp)[QT / 2], uint32_t sQs, uint32_t sDOs) {
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk) {
@@ -359,60 +386,81 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
                             kk > 0 ? 1u : 0u);
     }
     wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(s);
-    fence_regs(dp);
+  };
 
-    // ---- P^T = exp2(S^T*c1 + c3 [+ bias*log2e]) (masked), dS^T = P^T * (dP^T - delta) ----
-    // element pair e: key row kr + 8 (e & 1), query columns 8 (e >> 1) + cq + {0, 1}
-    const int hi = min(QT - 1, a.Nq - 1 - row0);             // last valid query column of the tile
-    int lo[2];                                                // first visible query column of each key row
+  // P^T = exp2(S^T*c1 + c3 [+ bias*log2e]) (masked), dS^T = P^T * (dP^T - delta): 16-bit A fragments in
+  // pf / dsf, dS^T also to shared memory (row = key, 128-byte rows of QT = 64 queries, 128B swizzle).
+  // Element pair e = 2 j + hf: key row kr + 8 hf, query columns 8 j + cq + {0, 1}.
+  auto elementwise = [&](const bool MASKED, const float (&s)[QT / 2], const float (&dp)[QT / 2],
+                         uint32_t (&pf)[QT / 4], uint32_t (&dsf)[QT / 4], int row0, uint32_t stc3, uint32_t dsbuf) {
+    int hi = QT - 1, lo[2] = {0, 0};
+    if (MASKED) {
+      hi = min(QT - 1, a.Nq - 1 - row0);                      // last valid query column of the tile
 #pragma unroll
-    for (int hf = 0; hf < 2; ++hf) {
-      lo[hf] = a.causal ? max(0, key_g[hf] - off - row0) : 0;
-      if (!key_ok[hf]) lo[hf] = QT;
-    }
-    const uint32_t stc3 = sStats + st * 8 * QT, stdl = stc3 + 4 * QT;
-    const uint32_t dsbuf = sDS + (2 * w + (i & 1)) * Cfg::kDS;
-    uint32_t pf[QT / 4], dsf[QT / 4];
-#pragma unroll
-    for (int e = 0; e < QT / 4; ++e) {
-      const int hf = e & 1;
-      const int cc = 8 * (e >> 1) + cq;
-      const float2 c3 = lds64f(stc3 + 4 * cc);
-      const float2 ndl = lds64f(stdl + 4 * cc);
-      float x0 = fmaf(s[2 * e], c1, c3.x), x1 = fmaf(s[2 * e + 1], c1, c3.y);
-      if constexpr (BIAS) {
-        const uint8_t* bcol = reinterpret_cast<const uint8_t*>(a.bias) +
-                              2 * ((long long)b * a.bias_sb + (long long)h * a.bias_sh + min(key_g[hf], a.Nk - 1));
-        const int q0 = min(row0 + cc, a.Nq - 1), q1 = min(row0 + cc + 1, a.Nq - 1);
-        const float2 bv = unpack2<T>(ldg_u16(bcol + 2 * (long long)q0 * a.bias_sn) |
-                                     (ldg_u16(bcol + 2 * (long long)q1 * a.bias_sn) << 16));
-        x0 = fmaf(bv.x, 1.4426950408889634f, x0);
-        x1 = fmaf(bv.y, 1.4426950408889634f, x1);
+      for (int hf = 0; hf < 2; ++hf) {                        // first visible query column of each key row
+        lo[hf] = a.causal ? max(0, key_g[hf] - off - row0) : 0;
+        if (!key_ok[hf]) lo[hf] = QT;
       }
-      const bool v0 = cc >= lo[hf] && cc <= hi, v1 = cc + 1 >= lo[hf] && cc + 1 <= hi;
-      const float p0 = v0 ? ex2_approx(x0) : 0.f;
-      const float p1 = v1 ? ex2_approx(x1) : 0.f;
-      const float ds0 = p0 * (dp[2 * e] + ndl.x), ds1 = p1 * (dp[2 * e + 1] + ndl.y);
-      pf[e] = pack2<T>(p0, p1);
-      dsf[e] = pack2<T>(ds0, ds1);
-      // dS^T -> shared memory: row = key, 128-byte rows of QT = 64 queries, 128B swizzle
-      const int krow = kr + 8 * hf;
-      sts32(dsbuf + sw128_offset(krow, cc >> 3) + (cc & 7) * 2, dsf[e]);
-      if constexpr (BIAS) {
-        // d bias = dS (reference cu:1574-1576): fp32 reduction
-        if (a.dbias != nullptr) {
-          float* dst = a.dbias + (long long)b * a.dbias_sb + (long long)h * a.dbias_sh + key_g[hf];
-          if (v0) red_add_f32(dst + (long long)(row0 + cc) * a.Nk, ds0);
-          if (v1) red_add_f32(dst + (long long)(row0 + cc + 1) * a.Nk, ds1);
+    }
+#pragma unroll
+    for (int j = 0; j < QT / 8; ++j) {
+      const int cc = 8 * j + cq;
+      // {c3, -delta} of the two columns, loaded once for both key rows (per key row in the BIAS kernels, whose
+      // bias loads leave no registers to hold them)
+      float2 c3, ndl;
+      if constexpr (!BIAS) {
+        c3 = lds64f(stc3 + 4 * cc);
+        ndl = lds64f(stc3 + 4 * QT + 4 * cc);
+      }
+      const uint32_t ds_addr = dsbuf + ds_thr + ((j ^ r8) << 4);
+#pragma unroll
+      for (int hf = 0; hf < 2; ++hf) {
+        const int e = 2 * j + hf;
+        if constexpr (BIAS) {
+          c3 = lds64f(stc3 + 4 * cc);
+          ndl = lds64f(stc3 + 4 * QT + 4 * cc);
+        }
+        float x0 = fmaf(s[2 * e], c1, c3.x), x1 = fmaf(s[2 * e + 1], c1, c3.y);
+        if constexpr (BIAS) {
+          const uint8_t* bcol = reinterpret_cast<const uint8_t*>(a.bias) +
+                                2 * ((long long)b * a.bias_sb + (long long)h * a.bias_sh + min(key_g[hf], a.Nk - 1));
+          const int q0 = min(row0 + cc, a.Nq - 1), q1 = min(row0 + cc + 1, a.Nq - 1);
+          const float2 bv = unpack2<T>(ldg_u16(bcol + 2 * (long long)q0 * a.bias_sn) |
+                                       (ldg_u16(bcol + 2 * (long long)q1 * a.bias_sn) << 16));
+          x0 = fmaf(bv.x, 1.4426950408889634f, x0);
+          x1 = fmaf(bv.y, 1.4426950408889634f, x1);
+        }
+        const bool v0 = !MASKED || (cc >= lo[hf] && cc <= hi), v1 = !MASKED || (cc + 1 >= lo[hf] && cc + 1 <= hi);
+        const float p0 = v0 ? ex2_approx(x0) : 0.f;
+        const float p1 = v1 ? ex2_approx(x1) : 0.f;
+        const float ds0 = p0 * (dp[2 * e] + ndl.x), ds1 = p1 * (dp[2 * e + 1] + ndl.y);
+        pf[e] = pack2<T>(p0, p1);
+        dsf[e] = pack2<T>(ds0, ds1);
+        sts32(ds_addr + 1024 * hf, dsf[e]);
+        if constexpr (BIAS) {
+          // d bias = dS (reference cu:1574-1576): fp32 reduction
+          if (a.dbias != nullptr) {
+            float* dst = a.dbias + (long long)b * a.dbias_sb + (long long)h * a.dbias_sh + key_g[hf];
+            if (v0) red_add_f32(dst + (long long)(row0 + cc) * a.Nk, ds0);
+            if (v1) red_add_f32(dst + (long long)(row0 + cc + 1) * a.Nk, ds1);
+          }
         }
       }
     }
+  };
+  auto elementwise_tile = [&](const float (&s)[QT / 2], const float (&dp)[QT / 2], uint32_t (&pf)[QT / 4],
+                              uint32_t (&dsf)[QT / 4], int row0, uint32_t stc3, uint32_t dsbuf) {
+    // interior tile: every key of the warpgroup sees every query row (no causal diagonal, no ragged end)
+    const bool interior = keys_full && row0 + QT <= a.Nq && (!a.causal || key0 + 64 * w + 63 - off <= row0);
+    if (!BIAS && interior) elementwise(false, s, dp, pf, dsf, row0, stc3, dsbuf);
+    else elementwise(true, s, dp, pf, dsf, row0, stc3, dsbuf);
     fence_proxy_async_smem();
     named_bar_sync(1 + w, 128);               // the warpgroup's whole dS^T tile is in shared memory
+  };
 
-    // ---- dV += P^T dO, dK += dS^T Q (A from registers), then dQ_partial = dS K ----
+  // dV += P^T dO, dK += dS^T Q (A from registers)
+  auto issue_dv_dk = [&](const uint32_t (&pf)[QT / 4], const uint32_t (&dsf)[QT / 4], uint32_t sQs, uint32_t sDOs,
+                         float (&dv)[D / 2], float (&dk)[D / 2]) {
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < QT / 16; ++kk) {
@@ -428,39 +476,133 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       if constexpr (D == 64) wgmma_rs_n64<T, 1>(dk, af, db, 1u);
       else wgmma_rs_n128<T, 1>(dk, af, db, 1u);
     }
-    wgmma_commit();
-    if constexpr (D == 128) {                   // the dQ accumulator only fits once the A fragments are dead
-      wgmma_wait<0>();
-      fence_regs(pf);
-      fence_regs(dsf);
-    }
-    float dq[D / 2];
+  };
+  // dQ_partial = dS K: contraction over the warpgroup's 64 keys
+  auto issue_dq = [&](float (&dq)[D / 2], uint32_t dsbuf) {
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {            // contraction over the warpgroup's 64 keys
+    for (int kk = 0; kk < 4; ++kk) {
       const uint64_t da = gmma_desc_sw128(dsbuf + kk * 2048, 8192, 1024);     // dS: queries contiguous (MN-major)
       const uint64_t db = gmma_desc_sw128(sKw + kk * 2048, 16384, 1024);      // K: features contiguous (MN-major)
       if constexpr (D == 64) wgmma_ss_n64<T, 1, 1>(dq, da, db, kk > 0 ? 1u : 0u);
       else wgmma_ss_n128<T, 1, 1>(dq, da, db, kk > 0 ? 1u : 0u);
     }
-    wgmma_commit();
-    wgmma_wait<0>();
+  };
+
+  float dv[D / 2], dk[D / 2];
+#pragma unroll
+  for (int i = 0; i < D / 2; ++i) dv[i] = dk[i] = 0.f;
+  if (NI > 0) mbar_wait(BAR(KV_FULL), 0);
+
+  if constexpr (STAGED) {
+    // Query tiles overlap at the tensor cores: dV / dK / dQ of tile i and S^T / dP^T of tile i + 1 are issued back
+    // to back (20 wgmmas, one wait per tile instead of two), and the staging of dQ(i) and the next elementwise
+    // stage run after that single wait, while the tensor cores work on the other warpgroup's products.  dQ leaves
+    // through shared memory: the warpgroup stores the fp32 tile (128B swizzle, the layout of a 32-feature TMA
+    // box) and the reducer warp adds it into the accumulator.
+    // Staging word of accumulator pair (jb, hf): box jb / 4, row 16 wl + r8 + 8 hf, 16-byte chunk
+    // (2 (jb & 3) + (lane & 3) / 2) ^ r8, 8-byte half lane & 1.  Each warp store covers all 32 banks twice.
+    const uint32_t dq_thr = (16 * wl + r8) * 128 + (lane & 1) * 8;
+    const int dq_sx = ((lane & 3) >> 1) ^ r8;
+    float s[QT / 2], dp[QT / 2], dq[D / 2];
+    uint32_t pf[QT / 4], dsf[QT / 4];
+#pragma unroll
+    for (int k = 0; k < D / 2; ++k) dq[k] = 0.f;
+    auto stage_dq = [&](int i) {
+      const int sb = i & 1;
+      mbar_wait(BAR(DQ_EMPTY + 2 * w + sb), ((i >> 1) & 1) ^ 1);   // the reducer has read the buffer's last tile
+      const uint32_t dst = sDQ + (2 * w + sb) * Cfg::kDQ + dq_thr;
+#pragma unroll
+      for (int jb = 0; jb < D / 8; ++jb) {
+        const uint32_t o = dst + (jb >> 2) * (QT * 128) + (((2 * (jb & 3)) ^ dq_sx) << 4);
+        sts64f(o, dq[4 * jb], dq[4 * jb + 1]);
+        sts64f(o + 1024, dq[4 * jb + 2], dq[4 * jb + 3]);
+      }
+      fence_proxy_async_smem();
+      mbar_arrive(BAR(DQ_FULL + 2 * w + sb));
+    };
+
+    // The zero accumulators are pinned before the first issue: a register move of dV / dK / dQ that the compiler
+    // schedules while a wgmma is in flight makes ptxas serialise every wgmma of the kernel.
     fence_regs(dv);
     fence_regs(dk);
     fence_regs(dq);
-    fence_regs(pf);
-    fence_regs(dsf);
-    mbar_arrive(BAR(EMPTY + st));               // Q, dO and the stats of this stage are no longer read
+    if (NI > 0) {
+      mbar_wait(BAR(FULL), 0);
+      issue_s_dp(s, dp, sQ, sDO);
+      for (int i = 0; i < NI; ++i) {
+        const int st = i % NST;
+        const int row0 = (i_lo + i) * QT;
+        const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
+        wgmma_wait<0>();                        // S^T, dP^T of tile i; dV, dK, dQ of tile i - 1
+        fence_regs(s);
+        fence_regs(dp);
+        fence_regs(dv);
+        fence_regs(dk);
+        fence_regs(dq);
+        fence_regs(pf);
+        fence_regs(dsf);
+        if (i > 0) {
+          stage_dq(i - 1);
+          mbar_arrive(BAR(EMPTY + (i - 1) % NST));   // Q, dO and the stats of tile i - 1 are no longer read
+        }
+        const uint32_t dsbuf = sDS + (2 * w + (i & 1)) * Cfg::kDS;
+        elementwise_tile(s, dp, pf, dsf, row0, sStats + st * 8 * QT, dsbuf);
+        issue_dv_dk(pf, dsf, sQs, sDOs, dv, dk);
+        issue_dq(dq, dsbuf);
+        wgmma_commit();
+        if (i + 1 < NI) {
+          const int sn = (i + 1) % NST;
+          mbar_wait(BAR(FULL + sn), ((i + 1) / NST) & 1);
+          issue_s_dp(s, dp, sQ + sn * Cfg::kQ, sDO + sn * Cfg::kQ);
+        }
+      }
+      wgmma_wait<0>();
+      fence_regs(dv);
+      fence_regs(dk);
+      fence_regs(dq);
+      stage_dq(NI - 1);
+      mbar_arrive(BAR(EMPTY + (NI - 1) % NST));
+    }
+  } else {
+    for (int i = 0; i < NI; ++i) {
+      const int st = i % NST;
+      const int row0 = (i_lo + i) * QT;
+      const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
+      mbar_wait(BAR(FULL + st), (i / NST) & 1);
+      float s[QT / 2], dp[QT / 2];
+      issue_s_dp(s, dp, sQs, sDOs);
+      wgmma_wait<0>();
+      fence_regs(s);
+      fence_regs(dp);
 
-    // ---- dQ partial tile -> fp32 accumulator (rows = queries, columns = features) ----
-    float* acc = a.dq_acc + ((long long)bh * a.nqt * QT + row0) * D + cq;
+      const uint32_t dsbuf = sDS + (2 * w + (i & 1)) * Cfg::kDS;
+      uint32_t pf[QT / 4], dsf[QT / 4];
+      elementwise_tile(s, dp, pf, dsf, row0, sStats + st * 8 * QT, dsbuf);
+      issue_dv_dk(pf, dsf, sQs, sDOs, dv, dk);
+      wgmma_commit();
+      wgmma_wait<0>();                          // the dQ accumulator only fits once the A fragments are dead
+      fence_regs(pf);
+      fence_regs(dsf);
+      float dq[D / 2];
+      issue_dq(dq, dsbuf);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(dv);
+      fence_regs(dk);
+      fence_regs(dq);
+      mbar_arrive(BAR(EMPTY + st));             // Q, dO and the stats of this stage are no longer read
+
+      // ---- dQ partial tile -> fp32 accumulator (rows = queries, columns = features) ----
+      float* acc = a.dq_acc + ((long long)bh * a.nqt * QT + row0) * D + cq;
 #pragma unroll
-    for (int hf = 0; hf < 2; ++hf) {
-      const int q = 16 * wl + (lane >> 2) + 8 * hf;
-      if (row0 + q < a.Nq) {
+      for (int hf = 0; hf < 2; ++hf) {
+        const int q = 16 * wl + r8 + 8 * hf;
+        if (row0 + q < a.Nq) {
 #pragma unroll
-        for (int jb = 0; jb < D / 8; ++jb)
-          red_add_f32x2(acc + (long long)q * D + 8 * jb, dq[4 * jb + 2 * hf], dq[4 * jb + 2 * hf + 1]);
+          for (int jb = 0; jb < D / 8; ++jb)
+            red_add_f32x2(acc + (long long)q * D + 8 * jb, dq[4 * jb + 2 * hf], dq[4 * jb + 2 * hf + 1]);
+        }
       }
     }
   }
@@ -700,14 +842,24 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
   }
   // 2. main
   {
-    CUtensorMap tq, tk, tv, tdo;
-    if (make_tensor_map_bhnd(&tq, h.q.ptr, h.dtype_bf16, h.B, h.H, h.Nq, D, h.q.sb, h.q.sh, h.q.sn, Cfg::QT) ||
-        make_tensor_map_bhnd(&tk, h.k.ptr, h.dtype_bf16, h.B, h.kv_heads, h.Nk, D, h.k.sb, h.k.sh, h.k.sn, 128) ||
-        make_tensor_map_bhnd(&tv, h.v.ptr, h.dtype_bf16, h.B, h.kv_heads, h.Nk, D, h.v.sb, h.v.sh, h.v.sn, 128) ||
-        make_tensor_map_bhnd(&tdo, h.d_o.ptr, h.dtype_bf16, h.B, h.H, h.Nq, D, h.d_o.sb, h.d_o.sh, h.d_o.sn, Cfg::QT)) {
+    CUtensorMap tq, tk, tv, tdo, tdq;
+    const CUtensorMapDataType dt = tma_dtype16(h.dtype_bf16);
+    if (make_tensor_map_bhnd(&tq, h.q.ptr, dt, h.B, h.H, h.Nq, D, h.q.sb, h.q.sh, h.q.sn, Cfg::QT) ||
+        make_tensor_map_bhnd(&tk, h.k.ptr, dt, h.B, h.kv_heads, h.Nk, D, h.k.sb, h.k.sh, h.k.sn, 128) ||
+        make_tensor_map_bhnd(&tv, h.v.ptr, dt, h.B, h.kv_heads, h.Nk, D, h.v.sb, h.v.sh, h.v.sn, 128) ||
+        make_tensor_map_bhnd(&tdo, h.d_o.ptr, dt, h.B, h.H, h.Nq, D, h.d_o.sb, h.d_o.sh, h.d_o.sn, Cfg::QT)) {
       *err = "cuTensorMapEncodeTiled failed (backward): q, k, v, d_o must be views a TMA tensor map can express "
              "(positive strides, 16-byte aligned)";
       return FCSA_ERR_INVALID;
+    }
+    // the dq accumulator as [B][H][Nq][D] fp32 over its padded rows: boxes of 32 features x QT rows
+    memset(&tdq, 0, sizeof(tdq));
+    const long long acc_sh = (long long)w.nqt * Cfg::QT * D;
+    if (Cfg::kStaged &&
+        make_tensor_map_bhnd(&tdq, dq_acc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, h.B, h.H, h.Nq, D, h.H * acc_sh, acc_sh, D,
+                             Cfg::QT, 32)) {
+      *err = "cuTensorMapEncodeTiled failed (backward dq accumulator)";
+      return FCSA_ERR_CUDA;
     }
     BwdArgs a;
     a.B = h.B; a.H = h.H; a.Nq = h.Nq; a.Nk = h.Nk; a.kv_heads = h.kv_heads; a.causal = h.causal;
@@ -728,7 +880,7 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
     const long long items = (long long)((h.Nk + 127) / 128) * h.B * h.H;
     if (items > 0x7FFFFFFFLL) { *err = "problem too large for one launch"; return FCSA_ERR_INVALID; }
     if (h.ev_start) cudaEventRecord(h.ev_start, stream);
-    e = launch_pdl(kern, dim3((unsigned)items), dim3(Cfg::kThreads), Cfg::kSmem, stream, tq, tk, tv, tdo, a);
+    e = launch_pdl(kern, dim3((unsigned)items), dim3(Cfg::kThreads), Cfg::kSmem, stream, tq, tk, tv, tdo, tdq, a);
     if (h.ev_stop) cudaEventRecord(h.ev_stop, stream);
     if (e != cudaSuccess) { *err = "backward kernel launch"; *ce = e; return FCSA_ERR_CUDA; }
     ++*launches;

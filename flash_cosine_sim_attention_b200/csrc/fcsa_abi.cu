@@ -86,13 +86,13 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
   const bool bf = p->dtype == FCSA_BF16;
   CUtensorMap tq, tk, tv;
   int r;
-  if ((r = fcsa::make_tensor_map_bhnd(&tq, q->ptr, bf, p->batch, p->heads, p->seq_q, D, q->sb, q->sh,
+  if ((r = fcsa::make_tensor_map_bhnd(&tq, q->ptr, fcsa::tma_dtype16(bf), p->batch, p->heads, p->seq_q, D, q->sb, q->sh,
                                       q->sn, 128)))
     return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "q: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - make the tensor contiguous" : "cuTensorMapEncodeTiled failed", r);
-  if ((r = fcsa::make_tensor_map_bhnd(&tk, k->ptr, bf, p->batch, p->kv_heads, p->seq_k, D, k->sb,
+  if ((r = fcsa::make_tensor_map_bhnd(&tk, k->ptr, fcsa::tma_dtype16(bf), p->batch, p->kv_heads, p->seq_k, D, k->sb,
                                       k->sh, k->sn, 128)))
     return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "k: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - make the tensor contiguous" : "cuTensorMapEncodeTiled failed", r);
-  if ((r = fcsa::make_tensor_map_bhnd(&tv, v->ptr, bf, p->batch, p->kv_heads, p->seq_k, D, v->sb,
+  if ((r = fcsa::make_tensor_map_bhnd(&tv, v->ptr, fcsa::tma_dtype16(bf), p->batch, p->kv_heads, p->seq_k, D, v->sb,
                                       v->sh, v->sn, 128)))
     return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "v: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - make the tensor contiguous" : "cuTensorMapEncodeTiled failed", r);
 

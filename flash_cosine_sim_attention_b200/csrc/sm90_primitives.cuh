@@ -132,6 +132,27 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t smem_dst, const void* gsrc
       : "memory");
 }
 
+// 4-D tiled reduce-add shared -> global (the box at coordinates (c0, c1, c2, c3) += the shared tile), tracked by
+// the issuing thread's bulk async-groups.  Box elements outside the tensor are not written.
+__device__ __forceinline__ void tma_reduce_add_4d(const CUtensorMap* tm, uint32_t smem_src, int c0, int c1, int c2,
+                                                  int c3) {
+  asm volatile(
+      "cp.reduce.async.bulk.tensor.4d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+      ::"l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// all but the N most recent bulk groups have finished reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// all but the N most recent bulk groups have completed (their global writes are performed)
+template <int N>
+__device__ __forceinline__ void bulk_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
+
 // Register split of the warp-specialised kernels (384 threads: one producer warpgroup, two consumer
 // warpgroups): 128 x 40 + 256 x 232 = 384 x 168, the pool a CTA of __launch_bounds__(384, 1) is launched with.
 constexpr int kProducerRegs = 40;
@@ -324,6 +345,9 @@ __device__ __forceinline__ uint32_t sw128_offset(uint32_t r, uint32_t c) {
 
 __device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) {
   asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void sts64f(uint32_t addr, float x, float y) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
 }
 __device__ __forceinline__ float2 lds64f(uint32_t addr) {
   float2 v;

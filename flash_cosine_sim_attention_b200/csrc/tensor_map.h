@@ -33,9 +33,10 @@ inline PFN_encodeTiled get_encode_tiled() {
   return fn;
 }
 
-// Tensor map over a 16-bit tensor addressed as [b][h][n][d] with element strides
-// (sb, sh, sn, 1).  The box is box_cols features x box_rows rows: 64 features = one 128-byte swizzle
-// span for the operand tiles, 16 features = one 32-byte span (swizzle_bytes = 32) for the K = 16 slivers.
+// Tensor map over a 16-bit or fp32 tensor addressed as [b][h][n][d] with element strides
+// (sb, sh, sn, 1).  The box is box_cols features x box_rows rows: 64 16-bit features = one 128-byte swizzle
+// span for the operand tiles, 32 fp32 features = one 128-byte span for the dq accumulator tiles, 16 16-bit
+// features = one 32-byte span (swizzle_bytes = 32) for the K = 16 slivers.
 // A dimension of extent 1 gets a dummy stride (the driver rejects zero strides); a zero or negative
 // stride on a dimension of extent > 1 (an expanded / broadcast view) cannot be expressed by a tensor
 // map and is refused (-2) - callers make such tensors contiguous first.
@@ -44,24 +45,29 @@ inline PFN_encodeTiled get_encode_tiled() {
 struct TensorMapKey {
   const void* base;
   int64_t B, H, N, D, sb, sh, sn;
-  int32_t is_bf16, box_rows, box_cols, swizzle_bytes;
+  int32_t dtype, box_rows, box_cols, swizzle_bytes;     // dtype: a CUtensorMapDataType
 };
+
+inline CUtensorMapDataType tma_dtype16(bool is_bf16) {
+  return is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+}
 
 inline int encode_tensor_map_bhnd(CUtensorMap* tm, const TensorMapKey& k) {
   PFN_encodeTiled enc = get_encode_tiled();
   if (!enc) return -1;
   cuuint64_t dims[4] = {(cuuint64_t)k.D, (cuuint64_t)k.N, (cuuint64_t)k.H, (cuuint64_t)k.B};
+  const CUtensorMapDataType dt = (CUtensorMapDataType)k.dtype;
+  const int64_t es = dt == CU_TENSOR_MAP_DATA_TYPE_FLOAT32 ? 4 : 2;     // element bytes
   // strides in bytes for dims 1..3
-  int64_t sn_b = k.sn * 2, sh_b = k.sh * 2, sb_b = k.sb * 2;
+  int64_t sn_b = k.sn * es, sh_b = k.sh * es, sb_b = k.sb * es;
   if ((k.N > 1 && sn_b <= 0) || (k.H > 1 && sh_b <= 0) || (k.B > 1 && sb_b <= 0)) return -2;
-  if (k.N == 1) sn_b = k.D * 2;
+  if (k.N == 1) sn_b = k.D * es;
   if (k.H == 1) sh_b = sn_b * k.N;
   if (k.B == 1) sb_b = sh_b * k.H;
   cuuint64_t strides[3] = {(cuuint64_t)sn_b, (cuuint64_t)sh_b, (cuuint64_t)sb_b};
   cuuint32_t box[4] = {(cuuint32_t)k.box_cols, (cuuint32_t)k.box_rows, 1, 1};
   cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(tm, k.is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
-                   4, const_cast<void*>(k.base), dims, strides, box, estr,
+  CUresult r = enc(tm, dt, 4, const_cast<void*>(k.base), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE,
                    k.swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
                                           : (k.swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE),
@@ -70,8 +76,8 @@ inline int encode_tensor_map_bhnd(CUtensorMap* tm, const TensorMapKey& k) {
 }
 
 // A tensor map is a pure function of (pointer, shape, strides, box): training loops present the same
-// few views again and again, so each thread keeps the last few encodings.  32 entries x 7 maps per step cover several layers' worth of views.
-inline int make_tensor_map_bhnd(CUtensorMap* tm, const void* base, bool is_bf16, int64_t B,
+// few views again and again, so each thread keeps the last few encodings.  32 entries x 8 maps per step (3 forward, 5 backward) cover several layers' worth of views.
+inline int make_tensor_map_bhnd(CUtensorMap* tm, const void* base, CUtensorMapDataType dtype, int64_t B,
                                 int64_t H, int64_t N, int64_t D, int64_t sb, int64_t sh, int64_t sn,
                                 int box_rows, int box_cols = 64, int swizzle_bytes = 128) {
   struct Entry {
@@ -85,7 +91,7 @@ inline int make_tensor_map_bhnd(CUtensorMap* tm, const void* base, bool is_bf16,
   TensorMapKey key;
   memset(&key, 0, sizeof(key));
   key.base = base; key.B = B; key.H = H; key.N = N; key.D = D; key.sb = sb; key.sh = sh; key.sn = sn;
-  key.is_bf16 = is_bf16 ? 1 : 0; key.box_rows = box_rows; key.box_cols = box_cols; key.swizzle_bytes = swizzle_bytes;
+  key.dtype = (int32_t)dtype; key.box_rows = box_rows; key.box_cols = box_cols; key.swizzle_bytes = swizzle_bytes;
   for (int i = 0; i < kEntries; ++i)
     if (cache[i].used && memcmp(&cache[i].key, &key, sizeof(key)) == 0) {
       *tm = cache[i].map;
