@@ -17,12 +17,15 @@
 //                             S^T = K Q^T, dP^T = V dO^T            (wgmma, both operands in shared memory)
 //                             P^T, dS^T in registers                 (16-bit A fragments for the next two products)
 //                             dV += P^T dO, dK += dS^T Q             (wgmma, A from registers)
-//                             dQ_partial = dS K                      (wgmma; dS^T through shared memory)
+//                             dQ = dS K                              (wgmma; dS^T through shared memory)
 //                           Everything is computed TRANSPOSED (rows = keys) so that P^T and dS^T come out of the
-//                           accumulators in the register layout of a wgmma A operand.  The dQ partial tile of the
-//                           warpgroup's 64 keys is added to an fp32 accumulator in global memory: D = 64 stages it
-//                           in shared memory for TMA reduce-adds issued by producer warps 1 and 2 and pipelines
-//                           the products of consecutive query tiles; D = 128 uses vector reductions from registers.
+//                           accumulators in the register layout of a wgmma A operand.  The dQ tile is added to an
+//                           fp32 accumulator in global memory: D = 64 computes it once per query tile over all
+//                           128 keys (the warpgroups take turns), stages it in shared memory for TMA reduce-adds
+//                           issued by producer warps 1 and 2 and pipelines the products of consecutive query
+//                           tiles; D = 128 adds a partial over each warpgroup's 64 keys with vector reductions
+//                           from registers.  With the fused l2norm (and keys of their own per head) the epilogue
+//                           writes the gradient w.r.t. the raw keys.
 //   3. bwd_dq_finish_kernel: fp32 accumulator * scale -> 16-bit dq (+ l2norm backward of q); writes the accumulator
 //                           back as zeros (the "zeroed" workspace is zero on entry and on exit of every call).
 // BIAS instantiation: additive attention bias (16-bit loads along the query axis) and d_bias = dS
@@ -40,10 +43,11 @@
 
 namespace fcsa {
 
-// D = 64 stages each warpgroup's dQ partial tile in shared memory for TMA reduce-adds and pipelines the
-// products of consecutive query tiles; D = 128 has neither the shared memory (two 32 KB staging tiles on top
-// of 194 KB) nor the registers (a second S^T / dP^T pair next to 128 dV / dK accumulators) for that, and keeps
-// the in-order loop with vector reductions from registers.
+// D = 64 computes one dQ tile per query tile and CTA (a contraction over all 128 keys, shared by the two
+// warpgroups through shared memory), stages it for TMA reduce-adds and pipelines the products of consecutive
+// query tiles; D = 128 has neither the shared memory (two 32 KB staging tiles on top of 194 KB) nor the
+// registers (a second S^T / dP^T pair next to 128 dV / dK accumulators) for that, and keeps the in-order loop
+// with a dQ partial per warpgroup and vector reductions from registers.
 template <int D>
 struct BwdCfg {
   static constexpr bool kStaged = (D == 64);
@@ -52,17 +56,20 @@ struct BwdCfg {
   static constexpr int kQ = QT * D * 2;                   // bytes of one Q (or dO) stage
   static constexpr int NST = kStaged ? 4 : 3;             // Q / dO / stats ring depth
   static constexpr int kDS = 64 * QT * 2;                 // one warpgroup's dS^T: 64 keys x QT queries, 16-bit
+  static constexpr int NDS = kStaged ? 3 : 2;             // dS^T slots (one buffer per warpgroup each)
+  static constexpr int NDQ = kStaged ? 1 : 0;             // dQ staging buffers per warpgroup
   static constexpr int kDQ = kStaged ? QT * D * 4 : 0;    // one fp32 dQ staging tile: D / 32 boxes of 32 x QT
   static constexpr int kOffK = 0;
   static constexpr int kOffV = kOffK + kKV;
   static constexpr int kOffQ = kOffV + kKV;
   static constexpr int kOffDO = kOffQ + NST * kQ;
-  static constexpr int kOffDS = kOffDO + NST * kQ;        // 2 warpgroups x 2 buffers
-  static constexpr int kOffDQ = kOffDS + 4 * kDS;         // 2 warpgroups x 2 buffers (1024-byte aligned)
-  static constexpr int kOffStats = kOffDQ + 4 * kDQ;      // NST stages x {c3, -delta} x QT floats
+  static constexpr int kOffDS = kOffDO + NST * kQ;        // NDS slots x 2 warpgroups (slot-major: 128 keys each)
+  static constexpr int kOffDQ = kOffDS + 2 * NDS * kDS;   // 2 warpgroups x NDQ buffers (1024-byte aligned)
+  static constexpr int kOffStats = kOffDQ + 2 * NDQ * kDQ;  // NST stages x {c3, -delta} x QT floats
   static constexpr int kOffBar = kOffStats + NST * 8 * QT;
   static constexpr int kSmem = kOffBar + 256 + 1024;
   static_assert(kSmem <= 232448, "backward kernel shared memory");
+  static_assert(kOffDQ % 1024 == 0, "128B-swizzled staging tiles");
   static constexpr int kThreads = 384;                    // producer warpgroup + 2 consumer warpgroups
 };
 
@@ -214,6 +221,10 @@ struct BwdArgs {
   const void* bias; long long bias_sb, bias_sh, bias_sn;
   float* dbias; long long dbias_sb, dbias_sh;
   int out_f32;                      // 1: dk, dv are float32 tensors (strides in float32 elements)
+  // fused l2norm: k is the normalised k_hat and dk the gradient w.r.t. the raw keys (written by the epilogue
+  // unless keys/values are shared by all heads); k_rnorm (B, kv_heads, Nk, groups) or nullptr
+  const float* k_rnorm;
+  int groups;
 };
 
 // 16-bit global load through the read-only path (bias elements along the query axis are strided)
@@ -236,6 +247,66 @@ __device__ __forceinline__ float4 ldg_cg128f(const float* p) {
                : "l"(p)
                : "memory");
   return v;
+}
+
+// l2norm backward of one key row in the backward epilogue: dk = (dk_hat - k_hat <k_hat, dk_hat>_group) * rnorm_group.
+// The thread holds features 8 jb + cq + {0, 1} (g[2 jb], g[2 jb + 1]) of the row; the row's other features are in the
+// other three lanes of its quad.  k_hat comes from the resident K tile (row address sk_row, 128B swizzle, 64-feature
+// chunks 16 KB apart).  All lanes of the warp must call it (quad shuffles); `in` = the key exists.
+template <typename T, int D>
+__device__ __forceinline__ void l2norm_bwd_key_row(float (&g)[D / 4], const BwdArgs& a, uint32_t sk_row, int b, int hk,
+                                                   int key, bool in) {
+  const int lane = threadIdx.x & 31;
+  const int r8 = (lane >> 2) & 7, cq = 2 * (lane & 3);
+  const int gs = D / a.groups;                  // features per group (a power of two)
+  float y[D / 4], dot[D / 4];
+#pragma unroll
+  for (int jb = 0; jb < D / 8; ++jb) {
+    const float2 v = unpack2<T>(lds32(sk_row + (jb >> 3) * 16384 + ((((jb & 7) ^ r8)) << 4) + 2 * cq));
+    y[2 * jb] = v.x;
+    y[2 * jb + 1] = v.y;
+  }
+  if (gs == 1) {
+#pragma unroll
+    for (int e = 0; e < D / 4; ++e) dot[e] = y[e] * g[e];
+  } else {
+    float q[D / 8];                             // sums over the thread's feature pairs, then over the group
+#pragma unroll
+    for (int jb = 0; jb < D / 8; ++jb) q[jb] = y[2 * jb] * g[2 * jb] + y[2 * jb + 1] * g[2 * jb + 1];
+    // groups wider than 8 features: aligned blocks of gs / 8 pairs (compile-time register indices only)
+#pragma unroll
+    for (int m = 1; m < D / 8; m <<= 1) {
+      float t[D / 8];
+#pragma unroll
+      for (int jb = 0; jb < D / 8; ++jb) t[jb] = q[jb] + q[jb ^ m];
+      if (8 * m < gs) {
+#pragma unroll
+        for (int jb = 0; jb < D / 8; ++jb) q[jb] = t[jb];
+      }
+    }
+    // across the quad: gs = 4 spans lane pairs, gs >= 8 all four lanes
+    if (gs >= 4) {
+#pragma unroll
+      for (int jb = 0; jb < D / 8; ++jb) q[jb] += __shfl_xor_sync(0xFFFFFFFFu, q[jb], 1);
+    }
+    if (gs >= 8) {
+#pragma unroll
+      for (int jb = 0; jb < D / 8; ++jb) q[jb] += __shfl_xor_sync(0xFFFFFFFFu, q[jb], 2);
+    }
+#pragma unroll
+    for (int jb = 0; jb < D / 8; ++jb) dot[2 * jb] = dot[2 * jb + 1] = q[jb];
+  }
+  const int lg = __ffs(gs) - 1;
+  const float* rn = a.k_rnorm + (((long long)b * a.kv_heads + hk) * a.Nk + (in ? key : 0)) * a.groups;
+  // one load per feature pair (a pair shares its group unless gs = 1); the pairs of one group hit the same L1 line
+#pragma unroll
+  for (int jb = 0; jb < D / 8; ++jb) {
+    const int f = 8 * jb + cq;
+    const float r0 = in ? __ldg(rn + (f >> lg)) : 0.f;
+    const float r1 = gs == 1 && in ? __ldg(rn + f + 1) : r0;
+    g[2 * jb] = (g[2 * jb] - y[2 * jb] * dot[2 * jb]) * r0;
+    g[2 * jb + 1] = (g[2 * jb + 1] - y[2 * jb + 1] * dot[2 * jb + 1]) * r1;
+  }
 }
 
 template <typename T, int D, bool BIAS = false>
@@ -263,9 +334,11 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const uint32_t sStats = smem_u32(smem + Cfg::kOffStats);
   const uint32_t bar0 = smem_u32(smem + Cfg::kOffBar);
   auto BAR = [&](int i) { return bar0 + 8u * i; };
-  // DQ_FULL / DQ_EMPTY + 2 w + buffer: warpgroup w's dQ staging tiles (STAGED only)
-  constexpr int KV_FULL = 0, FULL = 1, EMPTY = FULL + NST, DQ_FULL = EMPTY + NST, DQ_EMPTY = DQ_FULL + 4,
-                NBARS = DQ_EMPTY + 4;
+  // STAGED only: DQ_FULL / DQ_EMPTY + NDQ w + buffer: warpgroup w's dQ staging tiles; DS_FULL / DS_EMPTY + slot:
+  // the dS^T slot holds both halves of the tile that uses it / the dQ product reading the slot has retired
+  constexpr int NDQ = STAGED ? Cfg::NDQ : 1, NDS = Cfg::NDS;    // (a divisor even where the staging is compiled out)
+  constexpr int KV_FULL = 0, FULL = 1, EMPTY = FULL + NST, DQ_FULL = EMPTY + NST, DQ_EMPTY = DQ_FULL + 2 * NDQ,
+                DS_FULL = DQ_EMPTY + 2 * NDQ, DS_EMPTY = DS_FULL + NDS, NBARS = DS_EMPTY + NDS;
   static_assert(NBARS * 8 <= 256, "barrier area");
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -294,9 +367,13 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       mbar_init(BAR(FULL + s), 1);
       mbar_init(BAR(EMPTY + s), 256);
     }
-    for (int s = 0; s < 4; ++s) {
+    for (int s = 0; s < 2 * NDQ; ++s) {
       mbar_init(BAR(DQ_FULL + s), 128);
       mbar_init(BAR(DQ_EMPTY + s), 1);
+    }
+    for (int s = 0; s < NDS; ++s) {
+      mbar_init(BAR(DS_FULL + s), 128);
+      mbar_init(BAR(DS_EMPTY + s), 128);
     }
     fence_mbar_init();
   }
@@ -329,19 +406,20 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         bulk_load_1d(sStats + st * 8 * QT, a.stats + ((long long)bh * a.nqt + qt) * 2 * QT, 8 * QT, BAR(FULL + st));
       }
     } else if (STAGED && (warp == 1 || warp == 2) && elect_one()) {
-      // dQ reducer of consumer warpgroup warp - 1: each staged 64 x D fp32 tile is added into the accumulator
-      // by TMA (rows at or beyond Nq lie outside the tensor map and are not written)
+      // dQ reducer of consumer warpgroup warp - 1, which owns the query tiles i = warp - 1 (mod 2): each staged
+      // 64 x D fp32 tile is added into the accumulator by TMA (rows at or beyond Nq lie outside the tensor map
+      // and are not written)
       const int rw = warp - 1;
       if (rw == 0) tma_prefetch_desc(&tm_dq);
-      for (int i = 0; i < NI; ++i) {
-        const int sb = i & 1;
-        const uint32_t src = sDQ + (2 * rw + sb) * Cfg::kDQ;
-        mbar_wait(BAR(DQ_FULL + 2 * rw + sb), (i >> 1) & 1);
+      for (int i = rw; i < NI; i += 2) {
+        const int n = i >> 1, sb = n % NDQ;        // the warpgroup's n-th tile
+        const uint32_t src = sDQ + (NDQ * rw + sb) * Cfg::kDQ;
+        mbar_wait(BAR(DQ_FULL + NDQ * rw + sb), (n / NDQ) & 1);
 #pragma unroll
         for (int c = 0; c < D / 32; ++c) tma_reduce_add_4d(&tm_dq, src + c * (QT * 128), c * 32, (i_lo + i) * QT, h, b);
         bulk_commit();
         bulk_wait_read<0>();
-        mbar_arrive(BAR(DQ_EMPTY + 2 * rw + sb));
+        mbar_arrive(BAR(DQ_EMPTY + NDQ * rw + sb));
       }
       bulk_wait<0>();                          // every reduction performed before the dq finish kernel reads
     }
@@ -355,13 +433,15 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int r8 = lane >> 2;                   // row inside every 8-row group of an accumulator
   const int kr = 16 * wl + r8;                // this thread's key rows inside the warpgroup's 64: kr, kr + 8
   const int cq = 2 * (lane & 3);              // first of the thread's two columns inside every 8-column block
-  int key_g[2];
-  bool key_ok[2];
+  // key_lo[hf]: the first query row that sees key row kr + 8 hf (causal: key - (Nk - Nq), else 0), or Nq + QT when
+  // the key does not exist or is masked - one register per row for the masked elementwise stage
+  int key_g[2], key_lo[2];
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     key_g[hf] = key0 + 64 * w + kr + 8 * hf;
-    key_ok[hf] = key_g[hf] < a.Nk;
-    if (a.has_mask && key_ok[hf]) key_ok[hf] = a.mask[(long long)b * a.mask_sb + key_g[hf]] != 0;
+    bool ok = key_g[hf] < a.Nk;
+    if (a.has_mask && ok) ok = a.mask[(long long)b * a.mask_sb + key_g[hf]] != 0;
+    key_lo[hf] = !ok ? a.Nq + QT : (a.causal ? key_g[hf] - off : 0);
   }
   // the warpgroup's keys are all real and unmasked: only query tiles crossing the causal diagonal or the end
   // of the sequence need per-element selects
@@ -398,8 +478,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       hi = min(QT - 1, a.Nq - 1 - row0);                      // last valid query column of the tile
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {                        // first visible query column of each key row
-        lo[hf] = a.causal ? max(0, key_g[hf] - off - row0) : 0;
-        if (!key_ok[hf]) lo[hf] = QT;
+        lo[hf] = max(0, key_lo[hf] - row0);
       }
     }
 #pragma unroll
@@ -477,13 +556,16 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       else wgmma_rs_n128<T, 1>(dk, af, db, 1u);
     }
   };
-  // dQ_partial = dS K: contraction over the warpgroup's 64 keys
+  // dQ = dS K.  STAGED: contraction over all 128 keys of the CTA (dsbuf = a dS^T slot, whose two warpgroup halves
+  // are contiguous: 16 keys = 2048 bytes throughout); otherwise a partial over the warpgroup's 64 keys.
   auto issue_dq = [&](float (&dq)[D / 2], uint32_t dsbuf) {
+    constexpr int NKK = STAGED ? 8 : 4;
+    const uint32_t sKd = STAGED ? sK : sKw;
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
+    for (int kk = 0; kk < NKK; ++kk) {
       const uint64_t da = gmma_desc_sw128(dsbuf + kk * 2048, 8192, 1024);     // dS: queries contiguous (MN-major)
-      const uint64_t db = gmma_desc_sw128(sKw + kk * 2048, 16384, 1024);      // K: features contiguous (MN-major)
+      const uint64_t db = gmma_desc_sw128(sKd + kk * 2048, 16384, 1024);      // K: features contiguous (MN-major)
       if constexpr (D == 64) wgmma_ss_n64<T, 1, 1>(dq, da, db, kk > 0 ? 1u : 0u);
       else wgmma_ss_n128<T, 1, 1>(dq, da, db, kk > 0 ? 1u : 0u);
     }
@@ -492,26 +574,37 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   float dv[D / 2], dk[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) dv[i] = dk[i] = 0.f;
-  if (NI > 0) mbar_wait(BAR(KV_FULL), 0);
+  // the producer loads K and V whatever NI; the epilogue reads K (l2norm backward) even when no query tile is visited
+  mbar_wait(BAR(KV_FULL), 0);
 
   if constexpr (STAGED) {
-    // Query tiles overlap at the tensor cores: dV / dK / dQ of tile i and S^T / dP^T of tile i + 1 are issued back
-    // to back (20 wgmmas, one wait per tile instead of two), and the staging of dQ(i) and the next elementwise
-    // stage run after that single wait, while the tensor cores work on the other warpgroup's products.  dQ leaves
-    // through shared memory: the warpgroup stores the fp32 tile (128B swizzle, the layout of a 32-feature TMA
-    // box) and the reducer warp adds it into the accumulator.
+    // One dQ tile per query tile and CTA, dQ(i) = [dS_0(i) | dS_1(i)] K over all 128 keys, owned by warpgroup i & 1
+    // (i = loop index, so both warpgroups agree; the last tile has one owner whatever NI).  The owner issues it one
+    // tile late, in the batch of tile i + 1 behind dV / dK(i + 1) and ahead of S^T / dP^T(i + 2) (20 wgmmas, one
+    // wait per tile); the other warpgroup has then almost always written its half of dS^T(i).  Tile i's dS^T lives
+    // in slot i % NDS (both halves, slot-major):
+    //   DS_FULL  : the non-owner fences its half to the async proxy and arrives (128 threads) after writing it;
+    //              the owner waits before issuing dQ(i)
+    //   DS_EMPTY : the owner arrives (128 threads) after the wait that retires dQ(i); the owner of tile
+    //              i + NDS (the other warpgroup, NDS being odd) waits before writing its half of the slot again.
+    //              The non-owner of i + NDS owns i and has retired dQ(i) itself.
+    // dQ(i) is retired by the owner's wait at iteration i + 2 and leaves through shared memory: the warpgroup
+    // stores the fp32 tile (128B swizzle, the layout of a 32-feature TMA box) and its reducer warp adds it into
+    // the accumulator.  Each warpgroup stages every other tile.
     // Staging word of accumulator pair (jb, hf): box jb / 4, row 16 wl + r8 + 8 hf, 16-byte chunk
     // (2 (jb & 3) + (lane & 3) / 2) ^ r8, 8-byte half lane & 1.  Each warp store covers all 32 banks twice.
+    static_assert(NDS % 2 == 1, "consecutive users of a dS^T slot must have different owners");
     const uint32_t dq_thr = (16 * wl + r8) * 128 + (lane & 1) * 8;
     const int dq_sx = ((lane & 3) >> 1) ^ r8;
     float s[QT / 2], dp[QT / 2], dq[D / 2];
     uint32_t pf[QT / 4], dsf[QT / 4];
 #pragma unroll
     for (int k = 0; k < D / 2; ++k) dq[k] = 0.f;
-    auto stage_dq = [&](int i) {
-      const int sb = i & 1;
-      mbar_wait(BAR(DQ_EMPTY + 2 * w + sb), ((i >> 1) & 1) ^ 1);   // the reducer has read the buffer's last tile
-      const uint32_t dst = sDQ + (2 * w + sb) * Cfg::kDQ + dq_thr;
+    auto ds_slot = [&](int i) { return sDS + 2 * (i % NDS) * Cfg::kDS; };
+    auto stage_dq = [&](int i) {              // i & 1 == w
+      const int n = i >> 1, sb = n % NDQ;
+      mbar_wait(BAR(DQ_EMPTY + NDQ * w + sb), ((n / NDQ) & 1) ^ 1);   // the reducer has read the buffer's last tile
+      const uint32_t dst = sDQ + (NDQ * w + sb) * Cfg::kDQ + dq_thr;
 #pragma unroll
       for (int jb = 0; jb < D / 8; ++jb) {
         const uint32_t o = dst + (jb >> 2) * (QT * 128) + (((2 * (jb & 3)) ^ dq_sx) << 4);
@@ -519,7 +612,16 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         sts64f(o + 1024, dq[4 * jb + 2], dq[4 * jb + 3]);
       }
       fence_proxy_async_smem();
-      mbar_arrive(BAR(DQ_FULL + 2 * w + sb));
+      mbar_arrive(BAR(DQ_FULL + NDQ * w + sb));
+    };
+    // dQ(i) retired: release its dS^T slot, stage the tile
+    auto retire_dq = [&](int i) {
+      mbar_arrive(BAR(DS_EMPTY + i % NDS));
+      stage_dq(i);
+    };
+    auto issue_owned_dq = [&](int i) {        // i & 1 == w
+      mbar_wait(BAR(DS_FULL + i % NDS), (i / NDS) & 1);
+      issue_dq(dq, ds_slot(i));
     };
 
     // The zero accumulators are pinned before the first issue: a register move of dV / dK / dQ that the compiler
@@ -530,11 +632,10 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     if (NI > 0) {
       mbar_wait(BAR(FULL), 0);
       issue_s_dp(s, dp, sQ, sDO);
-      for (int i = 0; i < NI; ++i) {
+      for (int i = 0, row0 = i_lo * QT; i < NI; ++i, row0 += QT) {
         const int st = i % NST;
-        const int row0 = (i_lo + i) * QT;
         const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
-        wgmma_wait<0>();                        // S^T, dP^T of tile i; dV, dK, dQ of tile i - 1
+        wgmma_wait<0>();                        // S^T, dP^T of tile i; dV, dK of tile i - 1; dQ of tile i - 2
         fence_regs(s);
         fence_regs(dp);
         fence_regs(dv);
@@ -542,14 +643,18 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         fence_regs(dq);
         fence_regs(pf);
         fence_regs(dsf);
-        if (i > 0) {
-          stage_dq(i - 1);
-          mbar_arrive(BAR(EMPTY + (i - 1) % NST));   // Q, dO and the stats of tile i - 1 are no longer read
-        }
-        const uint32_t dsbuf = sDS + (2 * w + (i & 1)) * Cfg::kDS;
-        elementwise_tile(s, dp, pf, dsf, row0, sStats + st * 8 * QT, dsbuf);
+        if (i >= 2 && ((i - 2) & 1) == w) retire_dq(i - 2);
+        if (i > 0) mbar_arrive(BAR(EMPTY + (i - 1) % NST));   // Q, dO and the stats of tile i - 1 are no longer read
+        const bool own = (i & 1) == w;
+        if (own && i >= NDS) mbar_wait(BAR(DS_EMPTY + i % NDS), ((i - NDS) / NDS) & 1);
+        elementwise_tile(s, dp, pf, dsf, row0, sStats + st * 8 * QT, ds_slot(i) + w * Cfg::kDS);
+        // the slot arithmetic below is redone from an opaque copy of i rather than kept live through the elementwise
+        // stage (the BIAS kernels have no register to spare there)
+        int io = i;
+        asm volatile("" : "+r"(io));
+        if ((io & 1) != w) mbar_arrive(BAR(DS_FULL + io % NDS));
         issue_dv_dk(pf, dsf, sQs, sDOs, dv, dk);
-        issue_dq(dq, dsbuf);
+        if (io >= 1 && (io & 1) != w) issue_owned_dq(io - 1);
         wgmma_commit();
         if (i + 1 < NI) {
           const int sn = (i + 1) % NST;
@@ -557,12 +662,20 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           issue_s_dp(s, dp, sQ + sn * Cfg::kQ, sDO + sn * Cfg::kQ);
         }
       }
+      // drain: dQ(NI - 2) is in flight if this warpgroup owns it, dQ(NI - 1) is not issued yet
       wgmma_wait<0>();
       fence_regs(dv);
       fence_regs(dk);
       fence_regs(dq);
-      stage_dq(NI - 1);
+      if (NI >= 2 && ((NI - 2) & 1) == w) retire_dq(NI - 2);
       mbar_arrive(BAR(EMPTY + (NI - 1) % NST));
+      if (((NI - 1) & 1) == w) {
+        issue_owned_dq(NI - 1);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(dq);
+        retire_dq(NI - 1);
+      }
     }
   } else {
     for (int i = 0; i < NI; ++i) {
@@ -576,7 +689,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       fence_regs(s);
       fence_regs(dp);
 
-      const uint32_t dsbuf = sDS + (2 * w + (i & 1)) * Cfg::kDS;
+      const uint32_t dsbuf = sDS + (2 * (i & 1) + w) * Cfg::kDS;
       uint32_t pf[QT / 4], dsf[QT / 4];
       elementwise_tile(s, dp, pf, dsf, row0, sStats + st * 8 * QT, dsbuf);
       issue_dv_dk(pf, dsf, sQs, sDOs, dv, dk);
@@ -608,37 +721,54 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   }
 
   // ---- epilogue: dV and dK * scale of the warpgroup's 64 keys ---------------------------------
+  // (no early exit for keys at or beyond Nk: the l2norm backward below shuffles within the quad of a key row)
   const bool shared_kv = (a.kv_heads == 1 && a.H > 1);
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     const int key = key_g[hf];
-    if (key >= a.Nk) continue;
+    const bool in = key < a.Nk;
     if (shared_kv) {
       // keys/values shared by all heads: sum over heads in fp32 (reference: cu:1613-1619)
       float* pv = a.dv_acc + ((long long)b * a.Nk + key) * D + cq;
       float* pk = a.dk_acc + ((long long)b * a.Nk + key) * D + cq;
+      if (in) {
 #pragma unroll
-      for (int jb = 0; jb < D / 8; ++jb) {
-        red_add_f32x2(pv + 8 * jb, dv[4 * jb + 2 * hf], dv[4 * jb + 2 * hf + 1]);
-        red_add_f32x2(pk + 8 * jb, dk[4 * jb + 2 * hf] * a.scale, dk[4 * jb + 2 * hf + 1] * a.scale);
+        for (int jb = 0; jb < D / 8; ++jb) {
+          red_add_f32x2(pv + 8 * jb, dv[4 * jb + 2 * hf], dv[4 * jb + 2 * hf + 1]);
+          red_add_f32x2(pk + 8 * jb, dk[4 * jb + 2 * hf] * a.scale, dk[4 * jb + 2 * hf + 1] * a.scale);
+        }
       }
     } else if (a.out_f32) {
       float* pv = reinterpret_cast<float*>(a.dv) + b * a.dv_sb + hk * a.dv_sh + (long long)key * a.dv_sn + cq;
       float* pk = reinterpret_cast<float*>(a.dk) + b * a.dk_sb + hk * a.dk_sh + (long long)key * a.dk_sn + cq;
+      if (in) {
 #pragma unroll
-      for (int jb = 0; jb < D / 8; ++jb) {
-        *reinterpret_cast<float2*>(pv + 8 * jb) = make_float2(dv[4 * jb + 2 * hf], dv[4 * jb + 2 * hf + 1]);
-        *reinterpret_cast<float2*>(pk + 8 * jb) =
-            make_float2(dk[4 * jb + 2 * hf] * a.scale, dk[4 * jb + 2 * hf + 1] * a.scale);
+        for (int jb = 0; jb < D / 8; ++jb) {
+          *reinterpret_cast<float2*>(pv + 8 * jb) = make_float2(dv[4 * jb + 2 * hf], dv[4 * jb + 2 * hf + 1]);
+          *reinterpret_cast<float2*>(pk + 8 * jb) =
+              make_float2(dk[4 * jb + 2 * hf] * a.scale, dk[4 * jb + 2 * hf + 1] * a.scale);
+        }
       }
     } else {
       T* pv = reinterpret_cast<T*>(a.dv) + b * a.dv_sb + hk * a.dv_sh + (long long)key * a.dv_sn + cq;
       T* pk = reinterpret_cast<T*>(a.dk) + b * a.dk_sb + hk * a.dk_sh + (long long)key * a.dk_sn + cq;
+      if (in) {
+#pragma unroll
+        for (int jb = 0; jb < D / 8; ++jb)
+          *reinterpret_cast<uint32_t*>(pv + 8 * jb) = pack2<T>(dv[4 * jb + 2 * hf], dv[4 * jb + 2 * hf + 1]);
+      }
+      // g[2 jb + e] = dk_hat of feature 8 jb + cq + e
+      float g[D / 4];
 #pragma unroll
       for (int jb = 0; jb < D / 8; ++jb) {
-        *reinterpret_cast<uint32_t*>(pv + 8 * jb) = pack2<T>(dv[4 * jb + 2 * hf], dv[4 * jb + 2 * hf + 1]);
-        *reinterpret_cast<uint32_t*>(pk + 8 * jb) =
-            pack2<T>(dk[4 * jb + 2 * hf] * a.scale, dk[4 * jb + 2 * hf + 1] * a.scale);
+        g[2 * jb] = dk[4 * jb + 2 * hf] * a.scale;
+        g[2 * jb + 1] = dk[4 * jb + 2 * hf + 1] * a.scale;
+      }
+      if (a.k_rnorm != nullptr) l2norm_bwd_key_row<T, D>(g, a, sK + (64 * w + kr + 8 * hf) * 128, b, hk, key, in);
+      if (in) {
+#pragma unroll
+        for (int jb = 0; jb < D / 8; ++jb)
+          *reinterpret_cast<uint32_t*>(pk + 8 * jb) = pack2<T>(g[2 * jb], g[2 * jb + 1]);
       }
     }
   }
@@ -873,6 +1003,7 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
     a.bias = h.bias; a.bias_sb = h.bias_sb; a.bias_sh = h.bias_sh; a.bias_sn = h.bias_sn;
     a.dbias = h.dbias; a.dbias_sb = h.dbias_sb; a.dbias_sh = h.dbias_sh;
     a.out_f32 = h.out_f32 ? 1 : 0;
+    a.k_rnorm = h.k_rnorm; a.groups = h.groups;
     auto kern = fcsa_bwd_kernel<T, D, BIAS>;
     e = ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS>>(Cfg::kSmem);
     if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(bwd)"; *ce = e; return FCSA_ERR_CUDA; }
@@ -914,8 +1045,9 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
         ++*launches;
       }
     }
-    if (h.k_rnorm != nullptr) {
-      // l2norm backward of dk (gradient w.r.t. the raw keys) as its own pass
+    if (h.k_rnorm != nullptr && shared_kv) {
+      // l2norm backward of dk (gradient w.r.t. the raw keys) as its own pass over the head-summed dk; otherwise
+      // the main kernel's epilogue applies it
       L2Args la;
       la.B = h.B; la.H = h.kv_heads; la.N = h.Nk; la.D = D; la.G = h.groups;
       la.x_sb = h.dk.sb; la.x_sh = h.dk.sh; la.x_sn = h.dk.sn;
