@@ -152,6 +152,9 @@ def context_parallel_cosine_sim_attention(q, k, v, *, scale=8, groups=1, causal=
     from .flash_cosine_sim_attention import _choose_shift, l2norm_tensors
     assert dist.is_initialized(), "context parallelism needs an initialised process group"
     assert q.shape[-2] == k.shape[-2] == v.shape[-2], "every rank holds the same number of queries and keys"
+    assert k.shape[:-2] == q.shape[:-2] and v.shape[:-2] == q.shape[:-2], (
+        "context parallelism needs keys/values with as many heads as the queries (grouped-query or single-head "
+        "keys/values are not supported on this path: expand them with repeat_interleave first)")
     if l2norm_qk:
         q, k = l2norm_tensors(q, k, groups=groups)        # per row: local, differentiable (fused kernels on CUDA)
     if primitives is None:

@@ -10,8 +10,10 @@
 // The machine mapping is new.  Three kernels:
 //   1. bwd_prep_kernel    : per query row {c3 = log2(inv_l) - shift*log2e, -delta} (fp32, never
 //                           rounded to 16 bit as the reference does at cu:1260/1820)
-//   2. fcsa_bwd_kernel    : one CTA = one 128-key tile of one (batch, head), K and V stationary in shared memory,
-//                           loop over the query tiles of QT = 64 rows that can see it.  Warpgroup 0 is the TMA
+//   2. fcsa_bwd_kernel    : one CTA = one 128-key tile of one (batch, kv head), K and V stationary in shared memory,
+//                           loop over the query tiles of QT = 64 rows that can see it, for each query head of the
+//                           CTA's slice of the kv head's group (grouped-query attention; one head for MHA): the
+//                           (head, query tile) pairs form one flat sequence of tiles.  Warpgroup 0 is the TMA
 //                           producer (K, V once; Q, dO and the per-query constants through an mbarrier ring);
 //                           warpgroups 1 and 2 own 64 keys each and run, per query tile, independently of each other:
 //                             S^T = K Q^T, dP^T = V dO^T            (wgmma, both operands in shared memory)
@@ -24,8 +26,9 @@
 //                           128 keys (the warpgroups take turns), stages it in shared memory for TMA reduce-adds
 //                           issued by producer warps 1 and 2 and pipelines the products of consecutive query
 //                           tiles; D = 128 adds a partial over each warpgroup's 64 keys with vector reductions
-//                           from registers.  With the fused l2norm (and keys of their own per head) the epilogue
-//                           writes the gradient w.r.t. the raw keys.
+//                           from registers.  dK / dV accumulate in registers over all the CTA's heads; when the
+//                           CTA covers its whole group the epilogue writes them (with the fused l2norm: the
+//                           gradient w.r.t. the raw keys), otherwise it adds them to fp32 accumulators.
 //   3. bwd_dq_finish_kernel: fp32 accumulator * scale -> 16-bit dq (+ l2norm backward of q); writes the accumulator
 //                           back as zeros (the "zeroed" workspace is zero on entry and on exit of every call).
 // BIAS instantiation: additive attention bias (16-bit loads along the query axis) and d_bias = dS
@@ -78,7 +81,8 @@ struct BwdCfg {
 //
 // SCRATCH workspace (contents irrelevant on entry, garbage on exit):
 //   stats : fp32 [B*H][nqt][2][QT]   c3 then -delta for each query tile (padded rows = 0)
-//   dkv_acc (kv_heads == 1 < heads only): fp32 dk [B][Nk][D] then dv [B][Nk][D]
+//   dkv_acc (kv_heads < heads only): fp32 dk [B][kv_heads][Nk][D] then dv [B][kv_heads][Nk][D]; used when a
+//            group's query heads are split over several CTAs (BwdArgs::split > 1)
 //
 // ZEROED workspace (all zero on entry - the caller zero-fills it ONCE, fcsa_zeroed_init - and all
 // zero again on exit: the dq conversion pass clears every accumulator row it converts, so no per-call
@@ -97,7 +101,7 @@ inline BwdWorkspace bwd_workspace_layout(int B, int H, int kv_heads, int Nq, int
   w.nqt = (Nq + w.QT - 1) / w.QT;
   size_t stats = (size_t)B * H * w.nqt * 2 * w.QT * 4;
   size_t dq = (size_t)B * H * w.nqt * w.QT * D * 4;
-  size_t dkv = (kv_heads == 1 && H > 1) ? (size_t)2 * B * Nk * D * 4 : 0;
+  size_t dkv = kv_heads < H ? (size_t)2 * B * kv_heads * Nk * D * 4 : 0;
   auto up = [](size_t x) { return (x + 255) & ~size_t(255); };
   w.stats_off = 0;
   w.dkv_off = up(stats);
@@ -207,12 +211,16 @@ __global__ void __launch_bounds__(256) bwd_prep_kernel(const PrepArgs a) {
 // ------------------------------------------------------------------------------------------
 struct BwdArgs {
   int B, H, Nq, Nk, kv_heads, causal, has_mask, nqt;
+  // query heads per CTA: the group of kv head hk (query heads hk * G .. + G - 1, G = H / kv_heads) is split into
+  // `split` slices of `hpc` = G / split consecutive heads, one slice per CTA.  split > 1: dk / dv are reduced over
+  // the slices in the fp32 accumulators.  BIAS launches have hpc = 1.
+  int split, hpc;
   float c1;                         // scale * log2e
   float scale;
   const uint8_t* mask; long long mask_sb;
   const float* stats;
   float* dq_acc;
-  float* dk_acc; float* dv_acc;     // fp32 (B, Nk, D) accumulators when kv_heads == 1 < H
+  float* dk_acc; float* dv_acc;     // fp32 (B, kv_heads, Nk, D) accumulators when split > 1
   void* dk; long long dk_sb, dk_sh, dk_sn;
   void* dv; long long dv_sb, dv_sh, dv_sn;
   // additive bias on the logits (BIAS instantiation only): element type T, [b][h][query][key], element
@@ -222,7 +230,7 @@ struct BwdArgs {
   float* dbias; long long dbias_sb, dbias_sh;
   int out_f32;                      // 1: dk, dv are float32 tensors (strides in float32 elements)
   // fused l2norm: k is the normalised k_hat and dk the gradient w.r.t. the raw keys (written by the epilogue
-  // unless keys/values are shared by all heads); k_rnorm (B, kv_heads, Nk, groups) or nullptr
+  // when split == 1); k_rnorm (B, kv_heads, Nk, groups) or nullptr
   const float* k_rnorm;
   int groups;
 };
@@ -309,12 +317,15 @@ __device__ __forceinline__ void l2norm_bwd_key_row(float (&g)[D / 4], const BwdA
   }
 }
 
-template <typename T, int D, bool BIAS = false>
+// HEAD_LOOP: the CTA works through several query heads (hpc > 1, grouped-query launches); otherwise hpc = 1 is a
+// compile-time constant and the loops below are those of one query head (MHA, MQA, BIAS and split groups of one head).
+template <typename T, int D, bool BIAS = false, bool HEAD_LOOP = false>
 __global__ void __launch_bounds__(384, 1)
 fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                 const __grid_constant__ CUtensorMap tm_v, const __grid_constant__ CUtensorMap tm_do,
                 const __grid_constant__ CUtensorMap tm_dq, const BwdArgs a) {
   static_assert(D == 64 || D == 128, "head dim 64 or 128");
+  static_assert(!(BIAS && HEAD_LOOP), "BIAS launches have one query head per CTA");
   using Cfg = BwdCfg<D>;
   constexpr bool STAGED = Cfg::kStaged;
   constexpr int QT = Cfg::QT;              // query rows per tile
@@ -345,12 +356,17 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int wg = warp >> 2;
   pdl_launch_dependents();
 
-  // ---- work item: one 128-key tile of one (batch, head); key tiles ascending = heaviest first (causal) ----
-  const int bh_count = a.B * a.H;
-  const int jt = blockIdx.x / bh_count;
-  const int bh = blockIdx.x - jt * bh_count;
-  const int b = bh / a.H, h = bh - b * a.H;
-  const int hk = (a.kv_heads == 1) ? 0 : h;
+  // ---- work item: one 128-key tile of one (batch, kv head) and a slice of hpc query heads of its group, numbered
+  // (key tile, batch, kv head, slice) = (key tile, batch, first query head h0 / hpc); key tiles ascending = heaviest
+  // first (causal) ----
+  const int slices = HEAD_LOOP ? a.kv_heads * a.split : a.H;     // one query head per CTA: a slice per head
+  const int bs_count = a.B * slices;
+  const int jt = blockIdx.x / bs_count;
+  const int bs = blockIdx.x - jt * bs_count;
+  const int b = bs / slices, sl = bs - b * slices;
+  const int hk = (HEAD_LOOP || a.split > 1) ? sl / a.split : sl;
+  const int hpc = HEAD_LOOP ? a.hpc : 1;
+  const int h0 = sl * hpc;                    // = hk * G + (slice within the group) * hpc
   const int key0 = jt * 128;
   const int off = a.Nk - a.Nq;
   int i_lo = 0;
@@ -359,7 +375,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     const int x = key0 - off - (QT - 1);
     i_lo = x <= 0 ? 0 : (x + QT - 1) / QT;
   }
-  const int NI = max(0, a.nqt - i_lo);        // number of query tiles to visit
+  const int NI = max(0, a.nqt - i_lo);        // number of query tiles to visit per query head
+  const int NT = hpc * NI;                    // flat tile index i: head h0 + i / NI, query tile i_lo + i % NI
 
   if (threadIdx.x == 0) {
     mbar_init(BAR(KV_FULL), 1);
@@ -394,16 +411,19 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         tma_load_4d(sK + ch * 16384, &tm_k, BAR(KV_FULL), ch * 64, key0, hk, b);
         tma_load_4d(sV + ch * 16384, &tm_v, BAR(KV_FULL), ch * 64, key0, hk, b);
       }
-      for (int i = 0; i < NI; ++i) {
-        const int st = i % NST, qt = i_lo + i;
-        mbar_wait(BAR(EMPTY + st), ((i / NST) & 1) ^ 1);
-        mbar_expect_tx(BAR(FULL + st), 2 * Cfg::kQ + 8 * QT);
+      for (int i = 0, h = h0; h < h0 + hpc; ++h) {
+        const float* stats_h = a.stats + ((long long)b * a.H + h) * a.nqt * 2 * QT;
+        for (int qt = i_lo; qt < a.nqt; ++qt, ++i) {
+          const int st = i % NST;
+          mbar_wait(BAR(EMPTY + st), ((i / NST) & 1) ^ 1);
+          mbar_expect_tx(BAR(FULL + st), 2 * Cfg::kQ + 8 * QT);
 #pragma unroll
-        for (int ch = 0; ch < KCH; ++ch) {
-          tma_load_4d(sQ + st * Cfg::kQ + ch * QCHUNK, &tm_q, BAR(FULL + st), ch * 64, qt * QT, h, b);
-          tma_load_4d(sDO + st * Cfg::kQ + ch * QCHUNK, &tm_do, BAR(FULL + st), ch * 64, qt * QT, h, b);
+          for (int ch = 0; ch < KCH; ++ch) {
+            tma_load_4d(sQ + st * Cfg::kQ + ch * QCHUNK, &tm_q, BAR(FULL + st), ch * 64, qt * QT, h, b);
+            tma_load_4d(sDO + st * Cfg::kQ + ch * QCHUNK, &tm_do, BAR(FULL + st), ch * 64, qt * QT, h, b);
+          }
+          bulk_load_1d(sStats + st * 8 * QT, stats_h + (long long)qt * 2 * QT, 8 * QT, BAR(FULL + st));
         }
-        bulk_load_1d(sStats + st * 8 * QT, a.stats + ((long long)bh * a.nqt + qt) * 2 * QT, 8 * QT, BAR(FULL + st));
       }
     } else if (STAGED && (warp == 1 || warp == 2) && elect_one()) {
       // dQ reducer of consumer warpgroup warp - 1, which owns the query tiles i = warp - 1 (mod 2): each staged
@@ -411,12 +431,13 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       // and are not written)
       const int rw = warp - 1;
       if (rw == 0) tma_prefetch_desc(&tm_dq);
-      for (int i = rw; i < NI; i += 2) {
+      for (int i = rw; i < NT; i += 2) {
         const int n = i >> 1, sb = n % NDQ;        // the warpgroup's n-th tile
+        const int hh = HEAD_LOOP ? i / NI : 0, qt = i_lo + i - hh * NI;
         const uint32_t src = sDQ + (NDQ * rw + sb) * Cfg::kDQ;
         mbar_wait(BAR(DQ_FULL + NDQ * rw + sb), (n / NDQ) & 1);
 #pragma unroll
-        for (int c = 0; c < D / 32; ++c) tma_reduce_add_4d(&tm_dq, src + c * (QT * 128), c * 32, (i_lo + i) * QT, h, b);
+        for (int c = 0; c < D / 32; ++c) tma_reduce_add_4d(&tm_dq, src + c * (QT * 128), c * 32, qt * QT, h0 + hh, b);
         bulk_commit();
         bulk_wait_read<0>();
         mbar_arrive(BAR(DQ_EMPTY + NDQ * rw + sb));
@@ -501,8 +522,9 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         }
         float x0 = fmaf(s[2 * e], c1, c3.x), x1 = fmaf(s[2 * e + 1], c1, c3.y);
         if constexpr (BIAS) {
+          // (BIAS launches have one query head per CTA: h0)
           const uint8_t* bcol = reinterpret_cast<const uint8_t*>(a.bias) +
-                                2 * ((long long)b * a.bias_sb + (long long)h * a.bias_sh + min(key_g[hf], a.Nk - 1));
+                                2 * ((long long)b * a.bias_sb + (long long)h0 * a.bias_sh + min(key_g[hf], a.Nk - 1));
           const int q0 = min(row0 + cc, a.Nq - 1), q1 = min(row0 + cc + 1, a.Nq - 1);
           const float2 bv = unpack2<T>(ldg_u16(bcol + 2 * (long long)q0 * a.bias_sn) |
                                        (ldg_u16(bcol + 2 * (long long)q1 * a.bias_sn) << 16));
@@ -519,7 +541,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         if constexpr (BIAS) {
           // d bias = dS (reference cu:1574-1576): fp32 reduction
           if (a.dbias != nullptr) {
-            float* dst = a.dbias + (long long)b * a.dbias_sb + (long long)h * a.dbias_sh + key_g[hf];
+            float* dst = a.dbias + (long long)b * a.dbias_sb + (long long)h0 * a.dbias_sh + key_g[hf];
             if (v0) red_add_f32(dst + (long long)(row0 + cc) * a.Nk, ds0);
             if (v1) red_add_f32(dst + (long long)(row0 + cc + 1) * a.Nk, ds1);
           }
@@ -629,10 +651,11 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     fence_regs(dv);
     fence_regs(dk);
     fence_regs(dq);
-    if (NI > 0) {
+    if (NT > 0) {
       mbar_wait(BAR(FULL), 0);
       issue_s_dp(s, dp, sQ, sDO);
-      for (int i = 0, row0 = i_lo * QT; i < NI; ++i, row0 += QT) {
+      // i runs over the flat (head, query tile) sequence; row0 restarts at i_lo * QT with every head
+      for (int i = 0, row0 = i_lo * QT; i < NT; ++i, row0 = (!HEAD_LOOP || row0 + QT < a.nqt * QT) ? row0 + QT : i_lo * QT) {
         const int st = i % NST;
         const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
         wgmma_wait<0>();                        // S^T, dP^T of tile i; dV, dK of tile i - 1; dQ of tile i - 2
@@ -656,31 +679,32 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         issue_dv_dk(pf, dsf, sQs, sDOs, dv, dk);
         if (io >= 1 && (io & 1) != w) issue_owned_dq(io - 1);
         wgmma_commit();
-        if (i + 1 < NI) {
+        if (i + 1 < NT) {
           const int sn = (i + 1) % NST;
           mbar_wait(BAR(FULL + sn), ((i + 1) / NST) & 1);
           issue_s_dp(s, dp, sQ + sn * Cfg::kQ, sDO + sn * Cfg::kQ);
         }
       }
-      // drain: dQ(NI - 2) is in flight if this warpgroup owns it, dQ(NI - 1) is not issued yet
+      // drain: dQ(NT - 2) is in flight if this warpgroup owns it, dQ(NT - 1) is not issued yet
       wgmma_wait<0>();
       fence_regs(dv);
       fence_regs(dk);
       fence_regs(dq);
-      if (NI >= 2 && ((NI - 2) & 1) == w) retire_dq(NI - 2);
-      mbar_arrive(BAR(EMPTY + (NI - 1) % NST));
-      if (((NI - 1) & 1) == w) {
-        issue_owned_dq(NI - 1);
+      if (NT >= 2 && ((NT - 2) & 1) == w) retire_dq(NT - 2);
+      mbar_arrive(BAR(EMPTY + (NT - 1) % NST));
+      if (((NT - 1) & 1) == w) {
+        issue_owned_dq(NT - 1);
         wgmma_commit();
         wgmma_wait<0>();
         fence_regs(dq);
-        retire_dq(NI - 1);
+        retire_dq(NT - 1);
       }
     }
   } else {
-    for (int i = 0; i < NI; ++i) {
+    for (int i = 0; i < NT; ++i) {
       const int st = i % NST;
-      const int row0 = (i_lo + i) * QT;
+      const int hh = HEAD_LOOP ? i / NI : 0;    // head h0 + hh, query tile i_lo + i % NI
+      const int row0 = (i_lo + i - hh * NI) * QT;
       const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
       mbar_wait(BAR(FULL + st), (i / NST) & 1);
       float s[QT / 2], dp[QT / 2];
@@ -707,7 +731,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       mbar_arrive(BAR(EMPTY + st));             // Q, dO and the stats of this stage are no longer read
 
       // ---- dQ partial tile -> fp32 accumulator (rows = queries, columns = features) ----
-      float* acc = a.dq_acc + ((long long)bh * a.nqt * QT + row0) * D + cq;
+      float* acc = a.dq_acc + (((long long)b * a.H + h0 + hh) * a.nqt * QT + row0) * D + cq;
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {
         const int q = 16 * wl + r8 + 8 * hf;
@@ -722,15 +746,15 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
   // ---- epilogue: dV and dK * scale of the warpgroup's 64 keys ---------------------------------
   // (no early exit for keys at or beyond Nk: the l2norm backward below shuffles within the quad of a key row)
-  const bool shared_kv = (a.kv_heads == 1 && a.H > 1);
+  const bool to_acc = a.split > 1;
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     const int key = key_g[hf];
     const bool in = key < a.Nk;
-    if (shared_kv) {
-      // keys/values shared by all heads: sum over heads in fp32 (reference: cu:1613-1619)
-      float* pv = a.dv_acc + ((long long)b * a.Nk + key) * D + cq;
-      float* pk = a.dk_acc + ((long long)b * a.Nk + key) * D + cq;
+    if (to_acc) {
+      // the group's heads are split over several CTAs: sum over them in fp32 (reference: cu:1613-1619)
+      float* pv = a.dv_acc + (((long long)b * a.kv_heads + hk) * a.Nk + key) * D + cq;
+      float* pk = a.dk_acc + (((long long)b * a.kv_heads + hk) * a.Nk + key) * D + cq;
       if (in) {
 #pragma unroll
         for (int jb = 0; jb < D / 8; ++jb) {
@@ -871,25 +895,27 @@ __global__ void __launch_bounds__(256) bwd_dq_finish_kernel(const DqFinishArgs a
 }
 
 struct KvFinishArgs {
-  int B, Nk, D, out_f32;
-  const float* acc;                 // (B, Nk, D) fp32
-  void* out; long long sb, sn;
+  int B, Hk, Nk, D, out_f32;
+  const float* acc;                 // (B, Hk, Nk, D) fp32
+  void* out; long long sb, sh, sn;
 };
 template <typename T>
 __global__ void __launch_bounds__(256) bwd_kv_finish_kernel(const KvFinishArgs a) {
   const int tpr = a.D >> 3;
   const long long idx = (long long)blockIdx.x * 256 + threadIdx.x;
-  const long long total = (long long)a.B * a.Nk * tpr;
+  const long long total = (long long)a.B * a.Hk * a.Nk * tpr;
   if (idx >= total) return;
   const int c8 = (int)(idx % tpr);
   const long long rowid = idx / tpr;
   const int n = (int)(rowid % a.Nk);
-  const int b = (int)(rowid / a.Nk);
+  const long long bh = rowid / a.Nk;
+  const int b = (int)(bh / a.Hk), h = (int)(bh % a.Hk);
   const float* src = a.acc + rowid * a.D + c8 * 8;
   const float4 lo = *reinterpret_cast<const float4*>(src);
   const float4 hi = *reinterpret_cast<const float4*>(src + 4);
+  const long long doff = b * a.sb + h * a.sh + (long long)n * a.sn + c8 * 8;
   if (a.out_f32) {
-    float* dst = reinterpret_cast<float*>(a.out) + b * a.sb + (long long)n * a.sn + c8 * 8;
+    float* dst = reinterpret_cast<float*>(a.out) + doff;
     *reinterpret_cast<float4*>(dst) = lo;
     *reinterpret_cast<float4*>(dst + 4) = hi;
     return;
@@ -899,7 +925,7 @@ __global__ void __launch_bounds__(256) bwd_kv_finish_kernel(const KvFinishArgs a
   o4.y = pack2<T>(lo.z, lo.w);
   o4.z = pack2<T>(hi.x, hi.y);
   o4.w = pack2<T>(hi.z, hi.w);
-  T* dst = reinterpret_cast<T*>(a.out) + b * a.sb + (long long)n * a.sn + c8 * 8;
+  T* dst = reinterpret_cast<T*>(a.out) + doff;
   *reinterpret_cast<uint4*>(dst) = o4;
 }
 
@@ -929,6 +955,21 @@ struct BwdHostArgs {
   float* dbias = nullptr; long long dbias_sb = 0, dbias_sh = 0;
 };
 
+// Slices per key/value-head group (query heads per CTA = G / split).  One CTA per group keeps dk / dv in registers
+// (no accumulator, no finish pass, bitwise reproducible), but the grid then has B * kv_heads * key tiles CTAs; below
+// one CTA per SM the group is split into the fewest slices that fill the device.  Keys/values shared by all heads
+// (kv_heads == 1) and the BIAS kernels (no registers to spare for the head loop) take one query head per CTA.
+inline int bwd_group_split(int B, int H, int kv_heads, int Nk, bool bias, int sm_count) {
+  const int G = H / kv_heads;
+  if (G == 1) return 1;
+  if (bias || kv_heads == 1) return G;
+  const long long unsplit = (long long)((Nk + 127) / 128) * B * kv_heads;
+  if (unsplit >= sm_count) return 1;
+  for (int s = 2; s < G; ++s)
+    if (G % s == 0 && unsplit * s >= sm_count) return s;
+  return G;
+}
+
 template <typename T, int D, bool BIAS = false>
 int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, const char** err,
                    cudaError_t* ce) {
@@ -939,13 +980,21 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
   float* stats = reinterpret_cast<float*>(ws + w.stats_off);
   float* dq_acc = reinterpret_cast<float*>(zs + w.dq_off);
   float* dkv_acc = reinterpret_cast<float*>(ws + w.dkv_off);
-  const bool shared_kv = (h.kv_heads == 1 && h.H > 1);
   const float log2e = 1.4426950408889634f;
   cudaError_t e;
+  int split = 1;
+  if (h.kv_heads < h.H) {
+    int sms = 0;
+    e = device_sm_count(&sms);
+    if (e != cudaSuccess) { *err = "cudaDeviceGetAttribute(multiProcessorCount)"; *ce = e; return FCSA_ERR_CUDA; }
+    split = bwd_group_split(h.B, h.H, h.kv_heads, h.Nk, BIAS, sms);
+  }
+  const bool to_acc = split > 1;
+  const size_t dkv_elems = (size_t)h.B * h.kv_heads * h.Nk * D;
 
-  // dk/dv accumulators of shared keys/values are per call (the dq accumulator is self-cleaning)
-  if (shared_kv) {
-    e = cudaMemsetAsync(dkv_acc, 0, (size_t)2 * h.B * h.Nk * D * 4, stream);
+  // dk/dv accumulators of split groups are per call (the dq accumulator is self-cleaning)
+  if (to_acc) {
+    e = cudaMemsetAsync(dkv_acc, 0, 2 * dkv_elems * 4, stream);
     if (e != cudaSuccess) { *err = "cudaMemsetAsync(workspace)"; *ce = e; return FCSA_ERR_CUDA; }
   }
 
@@ -994,21 +1043,24 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
     BwdArgs a;
     a.B = h.B; a.H = h.H; a.Nq = h.Nq; a.Nk = h.Nk; a.kv_heads = h.kv_heads; a.causal = h.causal;
     a.has_mask = h.mask ? 1 : 0; a.nqt = w.nqt;
+    a.split = split; a.hpc = h.H / h.kv_heads / split;
     a.c1 = h.scale * log2e; a.scale = h.scale;
     a.mask = h.mask; a.mask_sb = h.mask_sb;
     a.stats = stats; a.dq_acc = dq_acc;
-    a.dk_acc = dkv_acc; a.dv_acc = dkv_acc + (size_t)h.B * h.Nk * D;
+    a.dk_acc = dkv_acc; a.dv_acc = dkv_acc + dkv_elems;
     a.dk = h.dk.ptr; a.dk_sb = h.dk.sb; a.dk_sh = h.dk.sh; a.dk_sn = h.dk.sn;
     a.dv = h.dv.ptr; a.dv_sb = h.dv.sb; a.dv_sh = h.dv.sh; a.dv_sn = h.dv.sn;
     a.bias = h.bias; a.bias_sb = h.bias_sb; a.bias_sh = h.bias_sh; a.bias_sn = h.bias_sn;
     a.dbias = h.dbias; a.dbias_sb = h.dbias_sb; a.dbias_sh = h.dbias_sh;
     a.out_f32 = h.out_f32 ? 1 : 0;
     a.k_rnorm = h.k_rnorm; a.groups = h.groups;
-    auto kern = fcsa_bwd_kernel<T, D, BIAS>;
-    e = ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS>>(Cfg::kSmem);
+    constexpr bool kLoop = !BIAS;
+    auto kern = a.hpc > 1 ? fcsa_bwd_kernel<T, D, BIAS, kLoop> : fcsa_bwd_kernel<T, D, BIAS>;
+    e = a.hpc > 1 ? ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS, kLoop>>(Cfg::kSmem)
+                  : ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS>>(Cfg::kSmem);
     if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(bwd)"; *ce = e; return FCSA_ERR_CUDA; }
-    // one CTA per (key tile, batch, head)
-    const long long items = (long long)((h.Nk + 127) / 128) * h.B * h.H;
+    // one CTA per (key tile, batch, kv head, slice of its group)
+    const long long items = (long long)((h.Nk + 127) / 128) * h.B * h.kv_heads * split;
     if (items > 0x7FFFFFFFLL) { *err = "problem too large for one launch"; return FCSA_ERR_INVALID; }
     if (h.ev_start) cudaEventRecord(h.ev_start, stream);
     e = launch_pdl(kern, dim3((unsigned)items), dim3(Cfg::kThreads), Cfg::kSmem, stream, tq, tk, tv, tdo, tdq, a);
@@ -1031,21 +1083,21 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
     if (h.ev_finish[1]) cudaEventRecord(h.ev_finish[1], stream);
     if (e != cudaSuccess) { *err = "dq finish launch"; *ce = e; return FCSA_ERR_CUDA; }
     ++*launches;
-    if (shared_kv) {
+    if (to_acc) {
       for (int which = 0; which < 2; ++which) {
         KvFinishArgs ka;
-        ka.B = h.B; ka.Nk = h.Nk; ka.D = D; ka.out_f32 = h.out_f32 ? 1 : 0;
-        ka.acc = dkv_acc + (which ? (size_t)h.B * h.Nk * D : 0);
+        ka.B = h.B; ka.Hk = h.kv_heads; ka.Nk = h.Nk; ka.D = D; ka.out_f32 = h.out_f32 ? 1 : 0;
+        ka.acc = dkv_acc + (which ? dkv_elems : 0);
         const fcsa_tensor& t = which ? h.dv : h.dk;
-        ka.out = t.ptr; ka.sb = t.sb; ka.sn = t.sn;
-        const long long tot = (long long)h.B * h.Nk * (D / 8);
+        ka.out = t.ptr; ka.sb = t.sb; ka.sh = t.sh; ka.sn = t.sn;
+        const long long tot = (long long)dkv_elems / 8;
         bwd_kv_finish_kernel<T><<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(ka);
         e = cudaGetLastError();
         if (e != cudaSuccess) { *err = "dk/dv finish launch"; *ce = e; return FCSA_ERR_CUDA; }
         ++*launches;
       }
     }
-    if (h.k_rnorm != nullptr && shared_kv) {
+    if (h.k_rnorm != nullptr && to_acc) {
       // l2norm backward of dk (gradient w.r.t. the raw keys) as its own pass over the head-summed dk; otherwise
       // the main kernel's epilogue applies it
       L2Args la;

@@ -61,8 +61,8 @@ int check_problem(const fcsa_problem* p) {
   if (p->batch <= 0 || p->heads <= 0 || p->seq_q <= 0 || p->seq_k <= 0)
     return fail(FCSA_ERR_INVALID, "empty problem (batch %d heads %d seq_q %d seq_k %d)", p->batch,
                 p->heads, p->seq_q, p->seq_k);
-  if (p->kv_heads != p->heads && p->kv_heads != 1)
-    return fail(FCSA_ERR_INVALID, "kv_heads must equal heads or be 1 (got %d vs %d)", p->kv_heads,
+  if (p->kv_heads <= 0 || p->heads % p->kv_heads != 0)
+    return fail(FCSA_ERR_INVALID, "kv_heads must divide heads (got %d kv_heads for %d heads)", p->kv_heads,
                 p->heads);
   if (p->causal && p->key_mask)
     return fail(FCSA_ERR_INVALID, "mask should not be supplied if causality is needed");
@@ -103,7 +103,7 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
   a.Nk = p->seq_k;
   a.causal = p->causal ? 1 : 0;
   a.has_mask = p->key_mask ? 1 : 0;
-  a.kv_heads = p->kv_heads;
+  a.group = p->heads / p->kv_heads;
   a.n_qblk = (p->seq_q + 127) / 128;
   const float log2e = 1.4426950408889634f;
   a.c1 = p->scale * log2e;
@@ -179,7 +179,7 @@ int check_l2(int32_t dtype, int32_t B, int32_t H, int32_t N, int32_t D, int32_t 
 
 extern "C" {
 
-int fcsa_version(void) { return 200; }
+int fcsa_version(void) { return 300; }
 
 const char* fcsa_last_error(void) { return g_err; }
 

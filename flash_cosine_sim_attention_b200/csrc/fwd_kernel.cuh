@@ -24,7 +24,7 @@ struct FwdArgs {
   int B, H, Nq, Nk;
   int causal;        // bottom-right aligned: key j visible to query i iff j <= i + (Nk - Nq)
   int has_mask;      // key padding mask (B, Nk), nonzero = keep
-  int kv_heads;      // 1 => keys/values shared by all heads, else == H
+  int group;         // query heads per key/value head (H / kv_heads): head h reads kv head h / group
   int n_qblk;        // ceil(Nq / 128)
   float c1;          // scale * log2(e)
   float c2;          // shift * log2(e)
@@ -79,12 +79,14 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   pdl_launch_dependents();
 
   // ---- work item: 128 query rows of one (batch, head) ------------------------------------
+  // (the heads of one (batch, query block) are consecutive CTAs: the `group` heads sharing a key/value head
+  // stream the same K / V tiles close together in time and meet in L2)
   const int bh_count = a.B * a.H;
   const int rank = blockIdx.x / bh_count;
   const int bh = blockIdx.x - rank * bh_count;
   const int qblk = a.causal ? (a.n_qblk - 1 - rank) : rank;   // heaviest causal blocks first
   const int b = bh / a.H, h = bh - b * a.H;
-  const int hk = (a.kv_heads == 1) ? 0 : h;
+  const int hk = h / a.group;
   const int m0 = qblk * 128;
   const int off = a.Nk - a.Nq;
   int NT = (a.Nk + 127) >> 7;                                 // key tiles this block visits

@@ -123,6 +123,18 @@ inline cudaError_t ensure_dynamic_smem(int bytes) {
   return e;
 }
 
+// Number of SMs of the current device, read once per device (0 = not read yet).
+inline cudaError_t device_sm_count(int* n) {
+  static std::atomic<int> count[256];
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev >= 0 && dev < 256 && (*n = count[dev].load(std::memory_order_relaxed)) > 0) return cudaSuccess;
+  e = cudaDeviceGetAttribute(n, cudaDevAttrMultiProcessorCount, dev);
+  if (e == cudaSuccess && dev >= 0 && dev < 256) count[dev].store(*n, std::memory_order_relaxed);
+  return e;
+}
+
 // Launch with programmatic dependent launch enabled (see pdl_wait / pdl_launch_dependents).
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,

@@ -82,7 +82,12 @@ struct Shapes {
         kv_heads = 1;
       } else {
         TORCH_CHECK(k.dim() == 4 && v.dim() == 4, "keys and values must be 3- or 4-dimensional");
-        kv_heads = H;
+        // grouped-query attention: query head h reads key/value head h / (H / kv_heads)
+        kv_heads = k.size(1);
+        TORCH_CHECK(v.size(1) == kv_heads, "keys and values must have the same number of heads (kv_heads ", kv_heads,
+                    " vs ", v.size(1), ")");
+        TORCH_CHECK(kv_heads > 0 && H % kv_heads == 0, "kv_heads (", kv_heads, ") must divide the query heads (", H,
+                    ")");
       }
     }
     Nk = k.size(-2);

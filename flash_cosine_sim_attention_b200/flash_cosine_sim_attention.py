@@ -65,6 +65,18 @@ def _kernel_supported(q, k, v, attn_bias):
             and q.shape[-1] in _KERNEL_HEAD_DIMS and not exists(attn_bias))
 
 
+def _check_kv_heads(q, k, v):
+    """4-D q, k, v: k and v have the same number of heads, and it divides q's (grouped-query attention)."""
+    if q.ndim != 4 or k.ndim != 4:
+        return
+    hk = k.shape[1]
+    if v.ndim != 4 or v.shape[1] != hk:
+        raise ValueError(f"keys and values must have the same number of heads (kv_heads {hk} vs "
+                         f"{v.shape[1] if v.ndim == 4 else 'a 3-D v'})")
+    if hk <= 0 or q.shape[1] % hk != 0:
+        raise ValueError(f"kv_heads ({hk}) must divide the query heads ({q.shape[1]})")
+
+
 class _Shapes:
     """Shape canonicalisation of the reference's host op (cu:1647-1660, cu:1679)."""
 
@@ -88,7 +100,9 @@ class _Shapes:
                 self.kv_heads = 1
                 self.kkind = "bnd"
             else:
-                self.kv_heads = self.H
+                # grouped-query attention: query head h reads key/value head h // (H // kv_heads)
+                _check_kv_heads(q, k, v)
+                self.kv_heads = k.shape[1]
                 self.kkind = "bhnd"
         self.Nk = k.shape[-2]
         assert k.shape[-1] == self.D and v.shape[-1] == self.D, "head dimensions of q, k, v must match"
@@ -335,21 +349,36 @@ def plain_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
             "have only 3 dimensions")
         attn_bias_batch_dim = True
         q = q.unsqueeze(1)
+    elif not single_head_kv:
+        _check_kv_heads(q, k, v)
+    # grouped-query attention: q viewed as (batch, kv_heads, group, seq, dim) against k, v unsqueezed at dim 2
+    # (autograd sums each group's gradients into its key/value head)
+    grouped = not merged and not single_head_kv and k.shape[1] != q.shape[1]
+    if grouped:
+        B, H = q.shape[:2]
+        Hk = k.shape[1]
+        q = q.unflatten(1, (Hk, H // Hk))
+        k, v = k.unsqueeze(2), v.unsqueeze(2)
+        if exists(attn_bias) and not attn_bias_batch_dim:
+            attn_bias = attn_bias.unflatten(0, (Hk, H // Hk))
     if l2norm_qk:
         q, k = (_l2norm_torch(t, groups) for t in (q, k))
     kk = k.unsqueeze(1) if single_head_kv else k
     vv = v.unsqueeze(1) if single_head_kv else v
     sim = torch.matmul(q, kk.transpose(-1, -2)) * scale
+    lead = (None,) * (sim.ndim - 3)             # the head dims between batch and (i, j)
     if exists(attn_bias):
-        sim = sim + attn_bias.unsqueeze(1 if attn_bias_batch_dim else 0)
+        sim = sim + (attn_bias[(slice(None),) + lead] if attn_bias_batch_dim else attn_bias)
     neg = -torch.finfo(sim.dtype).max
     if causal:
         i, j = sim.shape[-2:]
         future = torch.ones((i, j), device=q.device, dtype=torch.bool).triu(j - i + 1)
         sim = sim.masked_fill(future, neg)
     if exists(mask):
-        sim = sim.masked_fill(~mask[:, None, None, :], neg)
+        sim = sim.masked_fill(~mask[(slice(None),) + lead + (None, slice(None))], neg)
     out = torch.matmul(sim.softmax(dim=-1), vv)
+    if grouped:
+        out = out.flatten(1, 2)
     return out.squeeze(1) if merged else out
 
 
@@ -491,6 +520,7 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
     D = q.shape[-1]
     if not (k.dtype == q.dtype and v.dtype == q.dtype):
         raise TypeError("flash_cosine_sim_attention: q, k, v must share one dtype")
+    _check_kv_heads(q, k, v)
     if D > 128 or D % 8 != 0 or D % groups != 0:
         raise NotImplementedError(
             f"flash_cosine_sim_attention: head_dim {D} with groups {groups} has no sm_90a kernel (head dims: multiples "

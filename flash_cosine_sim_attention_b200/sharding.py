@@ -27,10 +27,14 @@ def shard_range(total, rank, world):
     return lo, lo + base + (1 if rank < rem else 0)
 
 
-def plan(batch, heads, world):
+def plan(batch, heads, world, kv_heads=None):
     """('batch' | 'heads', size of the sharded dim).  Batch is preferred (keeps single-head
-    keys/values local); heads are used when the batch does not divide evenly but heads do."""
+    keys/values local); heads are used when the batch does not divide evenly but heads do.
+    With grouped-query keys/values (1 < kv_heads < heads) heads are split only when the kv heads
+    divide over the ranks too, so that every query head's group stays on one rank."""
     if batch % world == 0 or heads % world != 0:
+        return "batch", batch
+    if kv_heads not in (None, 1, heads) and kv_heads % world != 0:
         return "batch", batch
     return "heads", heads
 
@@ -100,7 +104,7 @@ def sharded_flash_cosine_sim_attention(q, k, v, mask=None, *, gather=False, grou
         dim, total = 0, q.shape[0]                      # merged batch-heads: plain batch split
         kind = "batch"
     else:
-        kind, total = plan(q.shape[0], q.shape[1], world)
+        kind, total = plan(q.shape[0], q.shape[1], world, kv_heads=k.shape[1] if k.ndim == 4 else None)
         dim = 0 if kind == "batch" else 1
     lo, hi = shard_range(total, rank, world)
     sizes = [shard_range(total, r, world)[1] - shard_range(total, r, world)[0] for r in range(world)]
@@ -114,8 +118,11 @@ def sharded_flash_cosine_sim_attention(q, k, v, mask=None, *, gather=False, grou
         if k.ndim == 3:                                  # one kv head read by all ranks
             kl = _SharedAcrossRanks.apply(k, group) if world > 1 else k
             vl = _SharedAcrossRanks.apply(v, group) if world > 1 else v
-        else:
+        elif k.shape[1] == q.shape[1]:
             kl, vl = k.narrow(1, lo, hi - lo), v.narrow(1, lo, hi - lo)
+        else:                                            # grouped-query: this rank's whole groups
+            klo, khi = shard_range(k.shape[1], rank, world)
+            kl, vl = k.narrow(1, klo, khi - klo), v.narrow(1, klo, khi - klo)
     if hi - lo == 0:
         o = q.new_zeros(ql.shape)
     else:

@@ -48,22 +48,30 @@ def FeedForward(dim, mult=4, pre_norm=False):
 
 class Attention(nn.Module):
     def __init__(self, dim, dim_head=64, heads=8, scale=8, l2norm_groups=1, pre_norm=False,
-                 use_cuda_kernel=False, non_cosine_sim_attn=False, groups=None, **kwargs):
+                 use_cuda_kernel=False, non_cosine_sim_attn=False, groups=None, kv_heads=None, **kwargs):
         super().__init__()
+        # kv_heads: grouped-query attention - `kv_heads` key/value heads (dividing `heads`), each read by
+        # heads // kv_heads consecutive query heads.  None = one per query head (the reference's layout).
+        kv_heads = heads if kv_heads is None else kv_heads
+        assert heads % kv_heads == 0, f"kv_heads ({kv_heads}) must divide heads ({heads})"
         inner = dim_head * heads
         self.norm = nn.LayerNorm(dim) if pre_norm else nn.Identity()
         self.scale = scale
         self.heads = heads
+        self.kv_heads = kv_heads
         self.l2norm_groups = groups if groups is not None else l2norm_groups
         if non_cosine_sim_attn:
-            self.attn_fn = _softmax_attention
+            g = heads // kv_heads
+            self.attn_fn = (_softmax_attention if g == 1 else
+                            lambda q, k, v, **kw: _softmax_attention(q, k.repeat_interleave(g, dim=1),
+                                                                     v.repeat_interleave(g, dim=1)))
         elif use_cuda_kernel:
             self.attn_fn = (lambda q, k, v, **kw: flash_cosine_sim_attention(q, k, v, **{**kwargs, **kw}))
         else:
             self.attn_fn = plain_cosine_sim_attention
         self.to_q = nn.Linear(dim, inner, bias=False)
-        self.to_k = nn.Linear(dim, inner, bias=False)
-        self.to_v = nn.Linear(dim, inner, bias=False)
+        self.to_k = nn.Linear(dim, dim_head * kv_heads, bias=False)
+        self.to_v = nn.Linear(dim, dim_head * kv_heads, bias=False)
         self.to_out = nn.Linear(inner, dim, bias=False)
 
     def forward(self, x):
@@ -71,8 +79,9 @@ class Attention(nn.Module):
         x = self.norm(x)
         # (b, n, h*d) -> (b, h, n, d) views: strided, feature dim contiguous - the fused op reads
         # them through TMA tensor maps without a copy
-        split = lambda t: t.view(b, n, self.heads, -1).transpose(1, 2)
-        q, k, v = split(self.to_q(x)), split(self.to_k(x)), split(self.to_v(x))
+        split = lambda t, h: t.view(b, n, h, -1).transpose(1, 2)
+        q = split(self.to_q(x), self.heads)
+        k, v = split(self.to_k(x), self.kv_heads), split(self.to_v(x), self.kv_heads)
         o = self.attn_fn(q, k, v, causal=True, scale=self.scale, groups=self.l2norm_groups)
         return self.to_out(o.transpose(1, 2).reshape(b, n, -1))
 
@@ -80,7 +89,7 @@ class Attention(nn.Module):
 class CosineSimCausalTransformer(nn.Module):
     def __init__(self, *, num_tokens, dim, max_seq_len, depth, attn_scale=8, attn_l2norm_groups=1,
                  heads=8, dim_head=64, use_cuda_kernel=False, pre_norm=False, non_cosine_sim_attn=False,
-                 **kwargs):
+                 kv_heads=None, **kwargs):
         super().__init__()
         self.max_seq_len = max_seq_len
         self.token_emb = nn.Embedding(num_tokens, dim)
@@ -92,7 +101,7 @@ class CosineSimCausalTransformer(nn.Module):
             nn.ModuleList([
                 Attention(dim, dim_head=dim_head, heads=heads, use_cuda_kernel=use_cuda_kernel,
                           scale=attn_scale, groups=attn_l2norm_groups, pre_norm=pre_norm,
-                          non_cosine_sim_attn=non_cosine_sim_attn, **kwargs),
+                          non_cosine_sim_attn=non_cosine_sim_attn, kv_heads=kv_heads, **kwargs),
                 norm(),
                 FeedForward(dim, pre_norm=pre_norm),
                 norm(),

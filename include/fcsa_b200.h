@@ -57,12 +57,15 @@ typedef struct fcsa_tensor {
  * (cu:1630-1639, cu:1752-1764) after its shape canonicalisation (cu:1647-1660):
  *   - merged batch-heads (3-D q) is expressed as heads = 1
  *   - single-head keys/values (3-D k, v with 4-D q; cu:1679) is kv_heads = 1
+ *   - grouped-query attention (no reference counterpart): kv_heads divides heads and query head h reads
+ *     key/value head h / (heads / kv_heads); k, v (and dk, dv) then have kv_heads heads
  */
 typedef struct fcsa_problem {
   int32_t dtype;     /* FCSA_F16 | FCSA_BF16 (q, k, v, o, do, dq, dk, dv all share it)        */
   int32_t batch;
   int32_t heads;
-  int32_t kv_heads;  /* == heads, or 1 for keys/values shared across heads                   */
+  int32_t kv_heads;  /* divides heads: == heads (one per query head), 1 (shared by all), or a
+                        grouped-query count in between; anything else is FCSA_ERR_INVALID      */
   int32_t seq_q;
   int32_t seq_k;
   int32_t head_dim;  /* 64 or 128                                                             */
@@ -98,8 +101,9 @@ int64_t fcsa_debug(void);
 int fcsa_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
                  const fcsa_tensor* v, const fcsa_tensor* o, float* inv_l, void* stream);
 
-/* Bytes of SCRATCH fcsa_backward needs for this problem (per-row constants, shared-kv accumulators):
- * contents irrelevant on entry, garbage on exit. */
+/* Bytes of SCRATCH fcsa_backward needs for this problem (per-row constants; when kv_heads < heads also
+ * 2 * batch * kv_heads * seq_k * head_dim * 4 bytes of fp32 dk/dv accumulators): contents irrelevant on entry,
+ * garbage on exit.  A pure function of the problem. */
 size_t fcsa_backward_workspace_bytes(const fcsa_problem* p);
 
 /* Bytes of the ZEROED workspace of fcsa_backward (the fp32 dq accumulator tiles).
@@ -116,9 +120,14 @@ int fcsa_zeroed_init(void* zeroed, size_t bytes, void* stream);
 /*
  * Gradients of fcsa_forward w.r.t. q, k, v (the q, k given are the already-normalised ones,
  * exactly as in the reference: cu:1487-1626).  dq/dk/dv are caller-allocated in the problem
- * dtype; with kv_heads == 1, dk/dv have a single head and receive the sum over heads
- * (cu:1613-1619).  `workspace` must hold fcsa_backward_workspace_bytes(p) bytes, `zeroed`
- * fcsa_backward_zeroed_bytes(p) bytes that are all zero (see above).
+ * dtype; with kv_heads < heads, dk/dv have kv_heads heads and each receives the sum over the query
+ * heads that read it (cu:1613-1619 for kv_heads == 1).  `workspace` must hold
+ * fcsa_backward_workspace_bytes(p) bytes, `zeroed` fcsa_backward_zeroed_bytes(p) bytes that are all
+ * zero (see above).
+ * Reproducibility: o, dk, dv are bitwise reproducible from run to run when kv_heads == heads, and for
+ * grouped-query problems whose backward grid keeps each group in one CTA (enough batch * kv_heads *
+ * key tiles to fill the device, no bias).  Otherwise dk/dv are summed over CTAs with fp32 atomics and
+ * may differ in the last bits between runs, like dq always may.
  */
 int fcsa_backward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
                   const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o,
