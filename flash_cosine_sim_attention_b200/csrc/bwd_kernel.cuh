@@ -813,41 +813,6 @@ struct DqFinishArgs {
   int G;
 };
 
-// (dq_hat - q_hat <q_hat, dq_hat>_group) * rnorm_group on the 8 features one thread owns; the
-// `tpr` threads of a row are consecutive lanes, groups are aligned sub-blocks of them.
-template <typename T>
-__device__ __forceinline__ void finish_l2norm_bwd(float (&g)[8], const DqFinishArgs& a, bool ok, uint4 raw, int b,
-                                                  int h, int row, int c8) {
-  if (a.q_rnorm == nullptr) return;            // uniform across the grid
-  float y[8];
-  {
-    const float2 u0 = unpack2<T>(raw.x), u1 = unpack2<T>(raw.y), u2 = unpack2<T>(raw.z), u3 = unpack2<T>(raw.w);
-    y[0] = u0.x; y[1] = u0.y; y[2] = u1.x; y[3] = u1.y; y[4] = u2.x; y[5] = u2.y; y[6] = u3.x; y[7] = u3.y;
-  }
-  const int gs = a.D / a.G;
-  const long long rbase = (((long long)b * a.H + h) * a.Nq + row) * a.G;
-  if (gs >= 8) {
-    float dot = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) dot += y[i] * g[i];
-    const int tpg = gs >> 3;
-    for (int m = 1; m < tpg; m <<= 1) dot += __shfl_xor_sync(0xFFFFFFFFu, dot, m);
-    const float rn = ok ? a.q_rnorm[rbase + c8 / tpg] : 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) g[i] = (g[i] - y[i] * dot) * rn;
-  } else {
-    float pr[8], dot[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) pr[i] = y[i] * g[i];
-    subgroup_sums8(pr, gs, dot);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float rn = ok ? a.q_rnorm[rbase + (c8 * 8 + i) / gs] : 0.f;
-      g[i] = (g[i] - y[i] * dot[i]) * rn;
-    }
-  }
-}
-
 // dq conversion (reference: the fp32 -> scalar_t cast of dq after its atomics, cu:1904): TPR = D / 8 consecutive lanes
 // per query row, 8 features each.  The accumulator is read from L2 (the reductions of the main kernel have just
 // produced it there), converted, and written back as zeros: it is zero between launches.
@@ -873,24 +838,22 @@ __global__ void __launch_bounds__(256) bwd_dq_finish_kernel(const DqFinishArgs a
   }
   float g[8] = {lo.x * a.scale, lo.y * a.scale, lo.z * a.scale, lo.w * a.scale,
                 hi.x * a.scale, hi.y * a.scale, hi.z * a.scale, hi.w * a.scale};
-  uint4 qraw = make_uint4(0, 0, 0, 0);
-  if (ok && a.q_rnorm != nullptr)
-    qraw = ldg_stream128(reinterpret_cast<const T*>(a.q_hat) + b * a.q_sb + h * a.q_sh + (long long)row * a.q_sn +
-                         c8 * 8);
-  finish_l2norm_bwd<T>(g, a, ok, qraw, b, h, row, c8);
+  if (a.q_rnorm != nullptr) {                             // uniform across the grid
+    float y[8];
+    unpack16B<T>(ok ? ldg_stream128(reinterpret_cast<const T*>(a.q_hat) + b * a.q_sb + h * a.q_sh +
+                                    (long long)row * a.q_sn + c8 * 8)
+                    : make_uint4(0, 0, 0, 0), y);
+    l2norm_bwd_group<8>(g, y, D / a.G, c8, ok ? a.q_rnorm + (((long long)b * a.H + h) * a.Nq + row) * a.G : nullptr,
+                        1.f);
+  }
   if (!ok) return;
   if (a.out_f32) {
     float* dst = reinterpret_cast<float*>(a.dq) + b * a.sb + h * a.sh + (long long)row * a.sn + c8 * 8;
     *reinterpret_cast<float4*>(dst) = make_float4(g[0], g[1], g[2], g[3]);
     *reinterpret_cast<float4*>(dst + 4) = make_float4(g[4], g[5], g[6], g[7]);
   } else {
-    uint4 o4;
-    o4.x = pack2<T>(g[0], g[1]);
-    o4.y = pack2<T>(g[2], g[3]);
-    o4.z = pack2<T>(g[4], g[5]);
-    o4.w = pack2<T>(g[6], g[7]);
     T* dst = reinterpret_cast<T*>(a.dq) + b * a.sb + h * a.sh + (long long)row * a.sn + c8 * 8;
-    *reinterpret_cast<uint4*>(dst) = o4;
+    *reinterpret_cast<uint4*>(dst) = pack16B<T>(g);
   }
 }
 
@@ -1100,16 +1063,10 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
     if (h.k_rnorm != nullptr && to_acc) {
       // l2norm backward of dk (gradient w.r.t. the raw keys) as its own pass over the head-summed dk; otherwise
       // the main kernel's epilogue applies it
-      L2Args la;
-      la.B = h.B; la.H = h.kv_heads; la.N = h.Nk; la.D = D; la.G = h.groups;
-      la.x_sb = h.dk.sb; la.x_sh = h.dk.sh; la.x_sn = h.dk.sn;
-      la.y_sb = h.k.sb; la.y_sh = h.k.sh; la.y_sn = h.k.sn;
-      la.o_sb = h.dk.sb; la.o_sh = h.dk.sh; la.o_sn = h.dk.sn;
-      la.x = h.dk.ptr; la.y = h.k.ptr; la.dx = h.dk.ptr; la.rnorm = const_cast<float*>(h.k_rnorm);
-      const int rows_per_block = 256 / (D / 8);
-      const long long rows = (long long)la.B * la.H * la.N;
-      l2norm_bwd_kernel<T><<<(unsigned)((rows + rows_per_block - 1) / rows_per_block), 256, 0, stream>>>(la);
-      e = cudaGetLastError();
+      RowArgs la = {};
+      la.B = h.B; la.D = D; la.G = h.groups;
+      la.t[0] = {h.kv_heads, h.Nk, h.dk, h.k, h.dk, const_cast<float*>(h.k_rnorm)};
+      e = launch_row_bwd(la, h.dtype_bf16, false, stream);
       if (e != cudaSuccess) { *err = "l2norm backward (dk) launch"; *ce = e; return FCSA_ERR_CUDA; }
       ++*launches;
     }

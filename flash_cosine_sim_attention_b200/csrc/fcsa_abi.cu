@@ -138,41 +138,37 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
   return FCSA_OK;
 }
 
-template <typename T>
-int launch_l2norm_fwd(const fcsa::L2Args& a, cudaStream_t stream) {
-  const int tpr = a.D / 8;
-  const int rows_per_block = 256 / tpr;
-  const long long rows = (long long)a.B * a.H * a.N;
-  const long long grid = (rows + rows_per_block - 1) / rows_per_block;
-  fcsa::l2norm_fwd_kernel<T><<<(unsigned)grid, 256, 0, stream>>>(a);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "l2norm forward launch");
-  g_launches.fetch_add(1);
-  return FCSA_OK;
-}
-template <typename T>
-int launch_l2norm_bwd(const fcsa::L2Args& a, cudaStream_t stream) {
-  const int tpr = a.D / 8;
-  const int rows_per_block = 256 / tpr;
-  const long long rows = (long long)a.B * a.H * a.N;
-  const long long grid = (rows + rows_per_block - 1) / rows_per_block;
-  fcsa::l2norm_bwd_kernel<T><<<(unsigned)grid, 256, 0, stream>>>(a);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "l2norm backward launch");
+// error and launch count of one row pass
+int row_pass_launched(cudaError_t e, const char* what) {
+  if (e != cudaSuccess) return cuda_fail(e, what);
   g_launches.fetch_add(1);
   return FCSA_OK;
 }
 
-int check_l2(int32_t dtype, int32_t B, int32_t H, int32_t N, int32_t D, int32_t G) {
+// Shapes of the row passes.  The 16-bit l2norm takes head dims 32 to 256 and groups > 0; the float32 cast takes
+// head dims 16 to 128, and groups = 0 for a plain cast.  Head dims are powers of two, so every group size is too.
+int check_rows(bool f32, int32_t dtype, int32_t B, int32_t H, int32_t N, int32_t D, int32_t G) {
+  const char* what = f32 ? "f32 cast" : "l2norm";
   if (dtype != FCSA_F16 && dtype != FCSA_BF16)
-    return fail(FCSA_ERR_UNSUPPORTED, "l2norm: dtype %d not implemented", dtype);
-  if (B <= 0 || H <= 0 || N <= 0) return fail(FCSA_ERR_INVALID, "l2norm: empty tensor");
-  if (D != 32 && D != 64 && D != 128 && D != 256)
-    return fail(FCSA_ERR_UNSUPPORTED, "l2norm: head_dim %d not implemented", D);
-  if (G <= 0 || D % G != 0) return fail(FCSA_ERR_INVALID, "l2norm: groups %d does not divide %d", G, D);
-  const int gs = D / G;
-  if ((gs & (gs - 1)) != 0) return fail(FCSA_ERR_UNSUPPORTED, "l2norm: group size %d must be a power of two", gs);
+    return fail(FCSA_ERR_UNSUPPORTED, "%s: %sdtype %d not implemented", what, f32 ? "16-bit " : "", dtype);
+  if (B <= 0 || H <= 0 || N <= 0) return fail(FCSA_ERR_INVALID, "%s: empty tensor", what);
+  if (D < (f32 ? 16 : 32) || D > (f32 ? 128 : 256) || (D & (D - 1)) != 0)
+    return fail(FCSA_ERR_UNSUPPORTED, "%s: head_dim %d not implemented", what, D);
+  if (G < 0 || (G == 0 && !f32) || (G > 0 && D % G != 0))
+    return fail(FCSA_ERR_INVALID, f32 ? "f32 cast: groups %d must divide %d into power-of-two chunks"
+                                      : "l2norm: groups %d does not divide %d", G, D);
   return FCSA_OK;
+}
+
+// a float32 view whose rows start 16-byte aligned
+bool f32_rows(const fcsa_tensor* t) {
+  return t && t->ptr && aligned16(t->ptr) && t->sb % 4 == 0 && t->sh % 4 == 0 && t->sn % 4 == 0;
+}
+
+fcsa::RowArgs row_args(int32_t B, int32_t D, int32_t G, const float* mul = nullptr, int32_t mul_reciprocal = 0) {
+  fcsa::RowArgs a = {};
+  a.B = B; a.D = D; a.G = G; a.mul = mul; a.mul_reciprocal = mul_reciprocal;
+  return a;
 }
 
 }  // namespace
@@ -330,54 +326,19 @@ int fcsa_forward_fused(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_t
   int r;
   if ((r = check_problem(p))) return r;
   if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
-  if ((r = check_l2(p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, n->groups))) return r;
+  if ((r = check_rows(false, p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, n->groups))) return r;
   if ((r = check_tensor(q, "q")) || (r = check_tensor(k, "k")) || (r = check_tensor(&n->q_hat, "q_hat")) ||
       (r = check_tensor(&n->k_hat, "k_hat")))
     return r;
   if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
-  fcsa::L2PairArgs pa;
-  memset(&pa, 0, sizeof(pa));
-  const fcsa_tensor* src[2] = {q, k};
-  const fcsa_tensor* dst[2] = {&n->q_hat, &n->k_hat};
-  float* rn[2] = {n->q_rnorm, n->k_rnorm};
-  const int heads[2] = {p->heads, p->kv_heads};
-  const int rows[2] = {p->seq_q, p->seq_k};
-  int max_rows = 0;
-  for (int t = 0; t < 2; ++t) {
-    fcsa::L2Args& a = pa.t[t];
-    a.B = p->batch; a.H = heads[t]; a.N = rows[t]; a.D = p->head_dim; a.G = n->groups;
-    a.x_sb = src[t]->sb; a.x_sh = src[t]->sh; a.x_sn = src[t]->sn;
-    a.y_sb = dst[t]->sb; a.y_sh = dst[t]->sh; a.y_sn = dst[t]->sn;
-    a.x = src[t]->ptr; a.y = dst[t]->ptr; a.rnorm = rn[t];
-    if (a.N > max_rows) max_rows = a.N;
-  }
+  fcsa::RowArgs a = row_args(p->batch, p->head_dim, n->groups);
+  a.t[0] = {p->heads, p->seq_q, *q, n->q_hat, {}, n->q_rnorm};
+  a.t[1] = {p->kv_heads, p->seq_k, *k, n->k_hat, {}, n->k_rnorm};
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  constexpr int U = 2;                                       // rows per thread (16 features each)
-  const int rows_per_block = U * (256 / (p->head_dim / 16));
-  const long long bhs = (long long)pa.t[0].B * pa.t[0].H + (long long)pa.t[1].B * pa.t[1].H;
-  if (bhs > 65535) {
-    // more (batch, head) pairs than grid.y holds (merged batch-heads layouts): one 1-D-grid launch per tensor
-    const bool bf16 = p->dtype == FCSA_BF16;
-    for (int t = 0; t < 2; ++t)
-      if ((r = bf16 ? launch_l2norm_fwd<__nv_bfloat16>(pa.t[t], s) : launch_l2norm_fwd<__half>(pa.t[t], s))) return r;
-    return fcsa_forward(p, &n->q_hat, &n->k_hat, v, o, inv_l, stream);
-  }
-  dim3 grid((unsigned)((max_rows + rows_per_block - 1) / rows_per_block), (unsigned)bhs);
-  cudaError_t e;
-  const bool bf = p->dtype == FCSA_BF16;
   if (g_ev[2][0]) cudaEventRecord(g_ev[2][0], s);
-  if (p->head_dim == 64)
-    e = bf ? fcsa::launch_pdl(fcsa::l2norm_fwd_pair_kernel<__nv_bfloat16, 4, U>, grid, dim3(256), 0, s, pa)
-           : fcsa::launch_pdl(fcsa::l2norm_fwd_pair_kernel<__half, 4, U>, grid, dim3(256), 0, s, pa);
-  else if (p->head_dim == 128)
-    e = bf ? fcsa::launch_pdl(fcsa::l2norm_fwd_pair_kernel<__nv_bfloat16, 8, U>, grid, dim3(256), 0, s, pa)
-           : fcsa::launch_pdl(fcsa::l2norm_fwd_pair_kernel<__half, 8, U>, grid, dim3(256), 0, s, pa);
-  else
-    e = bf ? fcsa::launch_pdl(fcsa::l2norm_fwd_pair_kernel<__nv_bfloat16, 0, U>, grid, dim3(256), 0, s, pa)
-           : fcsa::launch_pdl(fcsa::l2norm_fwd_pair_kernel<__half, 0, U>, grid, dim3(256), 0, s, pa);
+  const cudaError_t e = fcsa::launch_row_fwd(a, p->dtype == FCSA_BF16, false, s);
   if (g_ev[2][1]) cudaEventRecord(g_ev[2][1], s);
-  if (e != cudaSuccess) return cuda_fail(e, "l2norm (q, k) launch");
-  g_launches.fetch_add(1);
+  if ((r = row_pass_launched(e, "l2norm (q, k) launch"))) return r;
   return fcsa_forward(p, &n->q_hat, &n->k_hat, v, o, inv_l, stream);
 }
 
@@ -389,88 +350,53 @@ int fcsa_backward_fused(const fcsa_problem* p, const fcsa_l2norm* n, const fcsa_
   if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
   int r;
   if ((r = check_problem(p))) return r;
-  if ((r = check_l2(p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, n->groups))) return r;
+  if ((r = check_rows(false, p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, n->groups))) return r;
   if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
   return backward_impl(p, &n->q_hat, &n->k_hat, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes,
                        zeroed, zeroed_bytes, stream, n->q_rnorm, n->k_rnorm, n->groups);
 }
 
-static int f32_cast_common(fcsa::F32CastArgs& a, int32_t dtype, int32_t B, int32_t H, int32_t N, int32_t D, int32_t G,
-                           const fcsa_tensor* x, const fcsa_tensor* y) {
-  if (dtype != FCSA_F16 && dtype != FCSA_BF16) return fail(FCSA_ERR_UNSUPPORTED, "f32 cast: 16-bit dtype %d not implemented", dtype);
-  if (B <= 0 || H <= 0 || N <= 0) return fail(FCSA_ERR_INVALID, "f32 cast: empty tensor");
-  if (D != 16 && D != 32 && D != 64 && D != 128) return fail(FCSA_ERR_UNSUPPORTED, "f32 cast: head_dim %d not implemented", D);
-  if (G < 0 || (G > 0 && (D % G != 0 || ((D / G) & (D / G - 1)) != 0)))
-    return fail(FCSA_ERR_INVALID, "f32 cast: groups %d must divide %d into power-of-two chunks", G, D);
-  if (!x || !x->ptr || !y) return fail(FCSA_ERR_INVALID, "f32 cast: null tensor");
-  if ((reinterpret_cast<uintptr_t>(x->ptr) & 15u) || (x->sb % 4) || (x->sh % 4) || (x->sn % 4))
-    return fail(FCSA_ERR_INVALID, "f32 cast: float32 rows must be 16-byte aligned");
-  memset(&a, 0, sizeof(a));
-  a.B = B; a.H = H; a.N = N; a.D = D; a.G = G;
-  a.x = reinterpret_cast<const float*>(x->ptr); a.x_sb = x->sb; a.x_sh = x->sh; a.x_sn = x->sn;
-  a.y = y->ptr; a.y_sb = y->sb; a.y_sh = y->sh; a.y_sn = y->sn;
-  return FCSA_OK;
-}
-
 int fcsa_f32_cast(int32_t dtype, int32_t batch, int32_t heads, int32_t rows, int32_t head_dim, int32_t groups,
                   const fcsa_tensor* x, const fcsa_tensor* y, float* rnorm, const float* mul, int32_t mul_reciprocal,
                   void* stream) {
-  fcsa::F32CastArgs a;
   int r;
-  if ((r = f32_cast_common(a, dtype, batch, heads, rows, head_dim, groups, x, y))) return r;
+  if ((r = check_rows(true, dtype, batch, heads, rows, head_dim, groups))) return r;
+  if (!x || !x->ptr || !y) return fail(FCSA_ERR_INVALID, "f32 cast: null tensor");
+  if (!f32_rows(x)) return fail(FCSA_ERR_INVALID, "f32 cast: float32 rows must be 16-byte aligned");
   if ((r = check_tensor(y, "y"))) return r;
   if (groups > 0 && !rnorm) return fail(FCSA_ERR_INVALID, "f32 cast: rnorm is null");
-  a.rnorm = rnorm; a.mul = mul; a.mul_reciprocal = mul_reciprocal;
-  const int rpb = 256 / (head_dim / 8);
-  const long long total = (long long)batch * heads * rows;
-  const unsigned grid = (unsigned)((total + rpb - 1) / rpb);
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  if (dtype == FCSA_BF16) fcsa::f32_cast_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(a);
-  else fcsa::f32_cast_kernel<__half><<<grid, 256, 0, s>>>(a);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "f32 cast launch");
-  g_launches.fetch_add(1);
-  return FCSA_OK;
+  fcsa::RowArgs a = row_args(batch, head_dim, groups, mul, mul_reciprocal);
+  a.t[0] = {heads, rows, *x, *y, {}, rnorm};
+  return row_pass_launched(fcsa::launch_row_fwd(a, dtype == FCSA_BF16, true, reinterpret_cast<cudaStream_t>(stream)),
+                           "f32 cast launch");
 }
 
 int fcsa_f32_cast_backward(int32_t dtype, int32_t batch, int32_t heads, int32_t rows, int32_t head_dim,
                            int32_t groups, const fcsa_tensor* dy, const fcsa_tensor* y, const float* rnorm,
                            const fcsa_tensor* dx, const float* mul, int32_t mul_reciprocal, void* stream) {
-  fcsa::F32CastArgs a;
   int r;
-  fcsa_tensor ynull = {nullptr, 0, 0, 0};
-  if ((r = f32_cast_common(a, dtype, batch, heads, rows, head_dim, groups, dy, groups > 0 ? y : &ynull))) return r;
-  if (groups > 0 && ((r = check_tensor(y, "y")) || !rnorm)) return r ? r : fail(FCSA_ERR_INVALID, "f32 cast backward: rnorm is null");
-  if (!dx || !dx->ptr || (reinterpret_cast<uintptr_t>(dx->ptr) & 15u) || (dx->sb % 4) || (dx->sh % 4) || (dx->sn % 4))
-    return fail(FCSA_ERR_INVALID, "f32 cast backward: dx rows must be 16-byte aligned float32");
-  a.dx = reinterpret_cast<float*>(dx->ptr); a.o_sb = dx->sb; a.o_sh = dx->sh; a.o_sn = dx->sn;
-  a.rnorm = const_cast<float*>(rnorm); a.mul = mul; a.mul_reciprocal = mul_reciprocal;
-  const int rpb = 256 / (head_dim / 8);
-  const long long total = (long long)batch * heads * rows;
-  const unsigned grid = (unsigned)((total + rpb - 1) / rpb);
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  if (dtype == FCSA_BF16) fcsa::f32_cast_bwd_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(a);
-  else fcsa::f32_cast_bwd_kernel<__half><<<grid, 256, 0, s>>>(a);
-  cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return cuda_fail(e, "f32 cast backward launch");
-  g_launches.fetch_add(1);
-  return FCSA_OK;
+  if ((r = check_rows(true, dtype, batch, heads, rows, head_dim, groups))) return r;
+  if (!dy || !dy->ptr || (groups > 0 && !y)) return fail(FCSA_ERR_INVALID, "f32 cast: null tensor");
+  if (!f32_rows(dy)) return fail(FCSA_ERR_INVALID, "f32 cast: float32 rows must be 16-byte aligned");
+  if (groups > 0 && (r = check_tensor(y, "y"))) return r;
+  if (groups > 0 && !rnorm) return fail(FCSA_ERR_INVALID, "f32 cast backward: rnorm is null");
+  if (!f32_rows(dx)) return fail(FCSA_ERR_INVALID, "f32 cast backward: dx rows must be 16-byte aligned float32");
+  fcsa::RowArgs a = row_args(batch, head_dim, groups, mul, mul_reciprocal);
+  a.t[0] = {heads, rows, *dy, groups > 0 ? *y : fcsa_tensor{}, *dx, const_cast<float*>(rnorm)};
+  return row_pass_launched(fcsa::launch_row_bwd(a, dtype == FCSA_BF16, true, reinterpret_cast<cudaStream_t>(stream)),
+                           "f32 cast backward launch");
 }
 
 int fcsa_l2norm_forward(int32_t dtype, int32_t batch, int32_t heads, int32_t rows, int32_t head_dim,
                         int32_t groups, const fcsa_tensor* x, const fcsa_tensor* y, float* rnorm,
                         void* stream) {
   int r;
-  if ((r = check_l2(dtype, batch, heads, rows, head_dim, groups))) return r;
+  if ((r = check_rows(false, dtype, batch, heads, rows, head_dim, groups))) return r;
   if ((r = check_tensor(x, "x")) || (r = check_tensor(y, "y"))) return r;
-  fcsa::L2Args a;
-  memset(&a, 0, sizeof(a));
-  a.B = batch; a.H = heads; a.N = rows; a.D = head_dim; a.G = groups;
-  a.x_sb = x->sb; a.x_sh = x->sh; a.x_sn = x->sn;
-  a.y_sb = y->sb; a.y_sh = y->sh; a.y_sn = y->sn;
-  a.x = x->ptr; a.y = y->ptr; a.rnorm = rnorm;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  return dtype == FCSA_BF16 ? launch_l2norm_fwd<__nv_bfloat16>(a, s) : launch_l2norm_fwd<__half>(a, s);
+  fcsa::RowArgs a = row_args(batch, head_dim, groups);
+  a.t[0] = {heads, rows, *x, *y, {}, rnorm};
+  return row_pass_launched(fcsa::launch_row_fwd(a, dtype == FCSA_BF16, false, reinterpret_cast<cudaStream_t>(stream)),
+                           "l2norm forward launch");
 }
 
 int fcsa_l2norm_backward(int32_t dtype, int32_t batch, int32_t heads, int32_t rows,
@@ -478,19 +404,14 @@ int fcsa_l2norm_backward(int32_t dtype, int32_t batch, int32_t heads, int32_t ro
                          const fcsa_tensor* y, const float* rnorm, const fcsa_tensor* dx,
                          void* stream) {
   int r;
-  if ((r = check_l2(dtype, batch, heads, rows, head_dim, groups))) return r;
+  if ((r = check_rows(false, dtype, batch, heads, rows, head_dim, groups))) return r;
   if ((r = check_tensor(dy, "dy")) || (r = check_tensor(y, "y")) || (r = check_tensor(dx, "dx")))
     return r;
   if (!rnorm) return fail(FCSA_ERR_INVALID, "rnorm: null");
-  fcsa::L2Args a;
-  memset(&a, 0, sizeof(a));
-  a.B = batch; a.H = heads; a.N = rows; a.D = head_dim; a.G = groups;
-  a.x_sb = dy->sb; a.x_sh = dy->sh; a.x_sn = dy->sn;
-  a.y_sb = y->sb; a.y_sh = y->sh; a.y_sn = y->sn;
-  a.o_sb = dx->sb; a.o_sh = dx->sh; a.o_sn = dx->sn;
-  a.x = dy->ptr; a.y = y->ptr; a.dx = dx->ptr; a.rnorm = const_cast<float*>(rnorm);
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  return dtype == FCSA_BF16 ? launch_l2norm_bwd<__nv_bfloat16>(a, s) : launch_l2norm_bwd<__half>(a, s);
+  fcsa::RowArgs a = row_args(batch, head_dim, groups);
+  a.t[0] = {heads, rows, *dy, *y, *dx, const_cast<float*>(rnorm)};
+  return row_pass_launched(fcsa::launch_row_bwd(a, dtype == FCSA_BF16, false, reinterpret_cast<cudaStream_t>(stream)),
+                           "l2norm backward launch");
 }
 
 }  // extern "C"

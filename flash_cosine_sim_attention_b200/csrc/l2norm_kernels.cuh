@@ -1,24 +1,41 @@
-// Grouped l2-normalisation of q / k rows and its backward.
+// Grouped l2-normalisation of q / k rows and its backward, and the float32 front end.
 //
 // Replaces the PyTorch ops the reference runs outside its kernels
 // (flash_cosine_sim_attention.py:38-65: F.normalize per `groups` chunk of the head dim, cast
 // back to the input dtype; backward left to autograd).  One pass each way, HBM-bound:
-// 16-byte vector loads, fp32 reduction with warp shuffles, one thread owns 8 features.
+// 16-byte vector loads, fp32 reduction with warp shuffles.
+//
+// float32 callers (reference: Float is dispatched in forward and backward, cu:1702-1703 / 1832-1834) run on the
+// 16-bit tensor-core kernels; the same two row kernels are the only extra work around them:
+//   row_fwd_kernel : y(16 bit) = round( x / max(||x||_group, 1e-12) * mul )   G > 0: l2norm over G groups
+//                                round( x * mul )                              G = 0: plain scaled cast
+//   row_bwd_kernel : dx = (dy - y <y, dy>_group) * rnorm_group * mul           G > 0   (dy: gradient w.r.t. y;
+//                         dy * mul                                             G = 0    y: 16 bit)
+// x / dy / dx are 16-bit or float32.  `mul` is an optional DEVICE scalar (the power-of-two range scale of v / dO,
+// chosen on the device - no host synchronisation) taken by the float32 passes; rnorm (fp32, per group) is kept for
+// the backward.
 #pragma once
 
+#include "../../include/fcsa_b200.h"
 #include "sm90_primitives.cuh"
+#include "tensor_map.h"
 
 namespace fcsa {
 
-struct L2Args {
-  int B, H, N, D, G;
-  long long x_sb, x_sh, x_sn;     // input  (x for forward, dy for backward)
-  long long y_sb, y_sh, y_sn;     // normalised tensor (output of forward, input of backward)
-  long long o_sb, o_sh, o_sn;     // dx (backward only)
-  const void* x;
-  void* y;
-  void* dx;
-  float* rnorm;                   // (B, H, N, G) fp32
+// One (B, H, N, D) tensor of a row pass; views with element strides and contiguous features.
+struct RowTensor {
+  int H, N;                       // heads (0: no tensor), rows
+  fcsa_tensor x;                  // forward: input; backward: dy (16-bit or float32)
+  fcsa_tensor y;                  // the 16-bit normalised tensor: output of forward, input of backward
+  fcsa_tensor dx;                 // backward only: output, the type of dy (may be dy itself: in-place passes)
+  float* rnorm;                   // (B, H, N, G) fp32; forward: nullptr = not kept
+};
+
+struct RowArgs {
+  int B, D, G;                    // G = 0: plain scaled cast (float32 passes)
+  const float* mul;               // device scalar or nullptr (= 1); read by the float32 passes only
+  int mul_reciprocal;             // 1: use 1 / *mul
+  RowTensor t[2];                 // forward: one or two tensors (t[1].H = 0 for one); backward: t[0]
 };
 
 // 1 / max(sqrt(ss), 1e-12)  (py:38-55: F.normalize's eps) = min(rsqrt(ss), 1e12): one MUFU.RSQ instead of an
@@ -36,9 +53,9 @@ __device__ __forceinline__ float group_reduce(float v, int tpg) {
   return v;
 }
 
-// Groups narrower than the 8 features one thread owns (group size gs = 1, 2 or 4): for every
-// feature, the sum of v over the aligned gs-wide block it belongs to.  Written with compile-time
-// register indices only - a `for (i < gs)` loop over the arrays would push them to local memory.
+// Groups narrower than 8 features (group size gs = 1, 2 or 4): for every feature, the sum of v over the aligned
+// gs-wide block it belongs to.  Written with compile-time register indices only - a `for (i < gs)` loop over the
+// arrays would push them to local memory.
 __device__ __forceinline__ void subgroup_sums8(const float (&v)[8], int gs, float (&out)[8]) {
   float p2[8], p4[8];
 #pragma unroll
@@ -49,40 +66,36 @@ __device__ __forceinline__ void subgroup_sums8(const float (&v)[8], int gs, floa
   for (int i = 0; i < 8; ++i) out[i] = gs == 1 ? v[i] : (gs == 2 ? p2[i] : p4[i]);
 }
 
-template <typename T>
-__global__ void __launch_bounds__(256) l2norm_fwd_kernel(const L2Args a) {
-  const int tpr = a.D >> 3;                       // threads per row (8 features each)
-  const int rows_per_block = 256 / tpr;
-  const long long row = (long long)blockIdx.x * rows_per_block + threadIdx.x / tpr;
-  const int tr = threadIdx.x % tpr;
-  const long long total_rows = (long long)a.B * a.H * a.N;
-  const bool ok = row < total_rows;
-  const long long rr = ok ? row : 0;
-  const int n = (int)(rr % a.N);
-  const int h = (int)((rr / a.N) % a.H);
-  const int b = (int)(rr / ((long long)a.N * a.H));
-  const T* xp = reinterpret_cast<const T*>(a.x) + b * a.x_sb + h * a.x_sh + n * a.x_sn + tr * 8;
-  uint4 raw = make_uint4(0, 0, 0, 0);
-  if (ok) raw = *reinterpret_cast<const uint4*>(xp);
-  float f[8];
-  {
-    float2 t0 = unpack2<T>(raw.x), t1 = unpack2<T>(raw.y), t2 = unpack2<T>(raw.z), t3 = unpack2<T>(raw.w);
-    f[0] = t0.x; f[1] = t0.y; f[2] = t1.x; f[3] = t1.y; f[4] = t2.x; f[5] = t2.y; f[6] = t3.x; f[7] = t3.y;
-  }
-  const int gs = a.D / a.G;                        // features per group
-  float rn[8];
-  if (gs >= 8) {
+// The group arithmetic of the F features (8 or 16) one thread owns.  The threads of a row are consecutive lanes,
+// tr is this thread's index in its row, gs the power-of-two group size; every lane of a row must take part (the
+// shuffles).  rnorm_row points at the row's G rnorm values, or is nullptr (forward: not kept; backward: a row past
+// the end, whose result is not stored).  A group of gs >= F features spans gs / F lanes; a 16-feature thread with
+// smaller groups works on each 8-feature half as a thread of its own.
+//
+// Forward: rn[i] = 1 / ||group of feature i||; the thread holding a group's first feature stores it.
+template <int F>
+__device__ __forceinline__ void l2norm_fwd_group(const float (&f)[F], int gs, int tr, float* rnorm_row,
+                                                 float (&rn)[F]) {
+  if (gs >= F) {
     float ss = 0.f;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) ss += f[i] * f[i];
-    const int tpg = gs >> 3;
-    ss = group_reduce(ss, tpg);
-    const float r = rnorm_of(ss);
+    for (int i = 0; i < F; ++i) ss += f[i] * f[i];
+    const int tpg = gs / F;                           // threads per group
+    const float r = rnorm_of(group_reduce(ss, tpg));
 #pragma unroll
-    for (int i = 0; i < 8; ++i) rn[i] = r;
-    if (ok && a.rnorm && (tr % tpg) == 0) a.rnorm[row * a.G + tr / tpg] = r;
+    for (int i = 0; i < F; ++i) rn[i] = r;
+    if (rnorm_row && (tr & (tpg - 1)) == 0) rnorm_row[tr / tpg] = r;
+  } else if constexpr (F == 16) {
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      float h[8], r8[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) h[i] = f[8 * s + i];
+      l2norm_fwd_group<8>(h, gs, 2 * tr + s, rnorm_row, r8);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) rn[8 * s + i] = r8[i];
+    }
   } else {
-    // several groups inside one thread's 8 features (gs = 1, 2 or 4)
     float sq[8], ss[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) sq[i] = f[i] * f[i];
@@ -90,332 +103,208 @@ __global__ void __launch_bounds__(256) l2norm_fwd_kernel(const L2Args a) {
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       rn[i] = rnorm_of(ss[i]);
-      if (ok && a.rnorm && (i & (gs - 1)) == 0) a.rnorm[row * a.G + (tr * 8 + i) / gs] = rn[i];
-    }
-  }
-  if (ok) {
-    uint4 w;
-    w.x = pack2<T>(f[0] * rn[0], f[1] * rn[1]);
-    w.y = pack2<T>(f[2] * rn[2], f[3] * rn[3]);
-    w.z = pack2<T>(f[4] * rn[4], f[5] * rn[5]);
-    w.w = pack2<T>(f[6] * rn[6], f[7] * rn[7]);
-    T* yp = reinterpret_cast<T*>(a.y) + b * a.y_sb + h * a.y_sh + n * a.y_sn + tr * 8;
-    *reinterpret_cast<uint4*>(yp) = w;
-  }
-}
-
-// q and k in one launch.  grid = (row blocks, batch*heads of q + batch*heads of k): blockIdx.y selects the
-// tensor and its (batch, head), so no thread divides 64-bit indices; one thread owns 16 features of U rows
-// and issues its 2 U 16-byte loads before the first reduction.  TPR = threads per row (D / 16) when known at
-// compile time (4 or 8), 0 = read it from the arguments (head dims 32 and 256: D must be a multiple of 16).
-struct L2PairArgs {
-  L2Args t[2];
-};
-
-template <typename T, int TPR, int U>
-__global__ void __launch_bounds__(256) l2norm_fwd_pair_kernel(const L2PairArgs pa) {
-  // TPR threads per row, SIXTEEN features per thread (two 16-byte loads): the pass is issue-bound before it is
-  // memory-bound (ncu: 84 % issue-slot utilisation with 8 features per thread), so the per-row bookkeeping
-  // (addresses, shuffle steps, predicates) is spread over twice the bytes.
-  pdl_launch_dependents();
-  pdl_wait();
-  const int bh0 = pa.t[0].B * pa.t[0].H;
-  const int which = blockIdx.y >= bh0;
-  const L2Args& a = pa.t[which];
-  const int bh = blockIdx.y - (which ? bh0 : 0);
-  const int tpr = TPR ? TPR : (a.D >> 4);
-  const int rpp = 256 / tpr;                          // rows per pass
-  const int tr = threadIdx.x % tpr;
-  const int r_in = threadIdx.x / tpr;
-  const int row0 = blockIdx.x * (U * rpp);
-  if (row0 >= a.N) return;                            // the grid is sized for the longer of the two tensors
-  const int b = bh / a.H, h = bh - b * a.H;
-  const T* xbase = reinterpret_cast<const T*>(a.x) + b * a.x_sb + h * a.x_sh + tr * 16;
-  T* ybase = reinterpret_cast<T*>(a.y) + b * a.y_sb + h * a.y_sh + tr * 16;
-  uint4 raw[U][2];
-#pragma unroll
-  for (int u = 0; u < U; ++u) {
-    const int n = row0 + u * rpp + r_in;
-    raw[u][0] = raw[u][1] = make_uint4(0, 0, 0, 0);
-    if (n < a.N) {
-      raw[u][0] = ldg_stream128(xbase + (long long)n * a.x_sn);
-      raw[u][1] = ldg_stream128(xbase + (long long)n * a.x_sn + 8);
-    }
-  }
-  const int gs = a.D / a.G;
-#pragma unroll
-  for (int u = 0; u < U; ++u) {
-    const int n = row0 + u * rpp + r_in;
-    const bool ok = n < a.N;
-    const long long row = (long long)bh * a.N + n;
-    float f[16];
-#pragma unroll
-    for (int s2 = 0; s2 < 2; ++s2) {
-      const float2 t0 = unpack2<T>(raw[u][s2].x), t1 = unpack2<T>(raw[u][s2].y), t2 = unpack2<T>(raw[u][s2].z),
-                   t3 = unpack2<T>(raw[u][s2].w);
-      f[8 * s2] = t0.x; f[8 * s2 + 1] = t0.y; f[8 * s2 + 2] = t1.x; f[8 * s2 + 3] = t1.y;
-      f[8 * s2 + 4] = t2.x; f[8 * s2 + 5] = t2.y; f[8 * s2 + 6] = t3.x; f[8 * s2 + 7] = t3.y;
-    }
-    float rn[16];
-    if (gs >= 16) {
-      float ss = 0.f;
-#pragma unroll
-      for (int i = 0; i < 16; ++i) ss += f[i] * f[i];
-      const int tpg = gs >> 4;                         // threads per group
-      ss = group_reduce(ss, tpg);
-      const float r = rnorm_of(ss);
-#pragma unroll
-      for (int i = 0; i < 16; ++i) rn[i] = r;
-      if (ok && a.rnorm && (tr & (tpg - 1)) == 0) a.rnorm[row * a.G + tr / tpg] = r;
-    } else if (gs == 8) {
-#pragma unroll
-      for (int s2 = 0; s2 < 2; ++s2) {
-        float ss = 0.f;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) ss += f[8 * s2 + i] * f[8 * s2 + i];
-        const float r = rnorm_of(ss);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) rn[8 * s2 + i] = r;
-        if (ok && a.rnorm) a.rnorm[row * a.G + 2 * tr + s2] = r;
-      }
-    } else {
-#pragma unroll
-      for (int s2 = 0; s2 < 2; ++s2) {
-        float sq[8], ss[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) sq[i] = f[8 * s2 + i] * f[8 * s2 + i];
-        subgroup_sums8(sq, gs, ss);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          rn[8 * s2 + i] = rnorm_of(ss[i]);
-          if (ok && a.rnorm && (i & (gs - 1)) == 0) a.rnorm[row * a.G + (tr * 16 + 8 * s2 + i) / gs] = rn[8 * s2 + i];
-        }
-      }
-    }
-    if (ok) {
-#pragma unroll
-      for (int s2 = 0; s2 < 2; ++s2) {
-        uint4 wv;
-        wv.x = pack2<T>(f[8 * s2 + 0] * rn[8 * s2 + 0], f[8 * s2 + 1] * rn[8 * s2 + 1]);
-        wv.y = pack2<T>(f[8 * s2 + 2] * rn[8 * s2 + 2], f[8 * s2 + 3] * rn[8 * s2 + 3]);
-        wv.z = pack2<T>(f[8 * s2 + 4] * rn[8 * s2 + 4], f[8 * s2 + 5] * rn[8 * s2 + 5]);
-        wv.w = pack2<T>(f[8 * s2 + 6] * rn[8 * s2 + 6], f[8 * s2 + 7] * rn[8 * s2 + 7]);
-        *reinterpret_cast<uint4*>(ybase + (long long)n * a.y_sn + 8 * s2) = wv;
-      }
+      if (rnorm_row && (i & (gs - 1)) == 0) rnorm_row[(tr * 8 + i) / gs] = rn[i];
     }
   }
 }
 
-// ------------------------------------------------------------------------------------------------
-// float32 front end (reference: Float is dispatched in forward and backward, cu:1702-1703 / 1832-1834).  float32
-// callers run on the 16-bit tensor-core kernels; these two passes are the only extra work around them:
-//   f32_cast_kernel     : y(16 bit) = round( x / max(||x||_group, 1e-12) * mul )   G > 0: l2norm over G groups
-//                                     round( x * mul )                              G = 0: plain scaled cast
-//                         `mul` is an optional DEVICE scalar (the power-of-two range scale of v / dO, chosen on
-//                         the device - no host synchronisation); rnorm (fp32, per group) is kept for the backward
-//   f32_cast_bwd_kernel : dx(f32) = (dy - y <y, dy>_group) * rnorm_group * mul      G > 0   (dy: f32 gradient
-//                                   dy * mul                                         G = 0    w.r.t. y; y: 16 bit)
-// One thread owns 8 features (two float4 loads); TPR threads per row.
-// ------------------------------------------------------------------------------------------------
-struct F32CastArgs {
-  int B, H, N, D, G;
-  long long x_sb, x_sh, x_sn;     // float32 tensor (x forward, dy / dx backward): element strides
-  long long y_sb, y_sh, y_sn;     // 16-bit tensor y
-  long long o_sb, o_sh, o_sn;     // backward only: dx (float32)
-  const float* x;
-  void* y;
-  float* dx;
-  float* rnorm;                   // (B, H, N, G) fp32 or nullptr (G = 0)
-  const float* mul;               // device scalar or nullptr (= 1)
-  int mul_reciprocal;             // 1: use 1 / *mul
-};
+// Backward, in place on g (dy in, dx out): g = (g - y <y, g>_group) * rnorm_group * mul.
+template <int F>
+__device__ __forceinline__ void l2norm_bwd_group(float (&g)[F], const float (&y)[F], int gs, int tr,
+                                                 const float* rnorm_row, float mul) {
+  if (gs >= F) {
+    float dot = 0.f;
+#pragma unroll
+    for (int i = 0; i < F; ++i) dot += y[i] * g[i];
+    const int tpg = gs / F;
+    dot = group_reduce(dot, tpg);
+    const float r = (rnorm_row ? rnorm_row[tr / tpg] : 0.f) * mul;
+#pragma unroll
+    for (int i = 0; i < F; ++i) g[i] = (g[i] - y[i] * dot) * r;
+  } else if constexpr (F == 16) {
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      float h[8], y8[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { h[i] = g[8 * s + i]; y8[i] = y[8 * s + i]; }
+      l2norm_bwd_group<8>(h, y8, gs, 2 * tr + s, rnorm_row, mul);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) g[8 * s + i] = h[i];
+    }
+  } else {
+    float pr[8], dot[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) pr[i] = y[i] * g[i];
+    subgroup_sums8(pr, gs, dot);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float r = (rnorm_row ? rnorm_row[(tr * 8 + i) / gs] : 0.f) * mul;
+      g[i] = (g[i] - y[i] * dot[i]) * r;
+    }
+  }
+}
 
-__device__ __forceinline__ float f32cast_mul(const F32CastArgs& a) {
-  if (a.mul == nullptr) return 1.f;
+// One 16-byte vector of X (16-bit: 8 elements, float: 4) to and from fp32.
+template <typename X>
+__device__ __forceinline__ void unpack16B(uint4 r, float* f) {
+  if constexpr (std::is_same<X, float>::value) {
+    f[0] = __uint_as_float(r.x); f[1] = __uint_as_float(r.y); f[2] = __uint_as_float(r.z); f[3] = __uint_as_float(r.w);
+  } else {
+    const float2 t0 = unpack2<X>(r.x), t1 = unpack2<X>(r.y), t2 = unpack2<X>(r.z), t3 = unpack2<X>(r.w);
+    f[0] = t0.x; f[1] = t0.y; f[2] = t1.x; f[3] = t1.y; f[4] = t2.x; f[5] = t2.y; f[6] = t3.x; f[7] = t3.y;
+  }
+}
+template <typename X>
+__device__ __forceinline__ uint4 pack16B(const float* f) {
+  if constexpr (std::is_same<X, float>::value)
+    return make_uint4(__float_as_uint(f[0]), __float_as_uint(f[1]), __float_as_uint(f[2]), __float_as_uint(f[3]));
+  else
+    return make_uint4(pack2<X>(f[0], f[1]), pack2<X>(f[2], f[3]), pack2<X>(f[4], f[5]), pack2<X>(f[6], f[7]));
+}
+
+// the scale of the float32 passes (1 without `mul`); the 16-bit passes take none
+template <typename X>
+__device__ __forceinline__ float row_mul(const RowArgs& a) {
+  if (!std::is_same<X, float>::value || a.mul == nullptr) return 1.f;
   const float m = __ldg(a.mul);
   return a.mul_reciprocal ? 1.f / m : m;
 }
 
-template <typename T>
-__global__ void __launch_bounds__(256) f32_cast_kernel(const F32CastArgs a) {
-  const int tpr = a.D >> 3;
-  const int rpb = 256 / tpr;
-  const long long row = (long long)blockIdx.x * rpb + threadIdx.x / tpr;
+// Forward: T is the 16-bit type of y, X the type of x (T or float).  grid = (row blocks, tensor): blockIdx.y
+// selects t[0] or t[1], and the blocks run over that tensor's (batch, head, row) rows as one flat sequence, so a
+// short sequence does not leave most of a block idle and any number of (batch, head) pairs fits.  Row indices are
+// 32-bit: 2^31 rows of at least 64 bytes do not fit in device memory.  One thread owns 16 features of U rows and
+// issues its loads of all U rows before the first reduction; TPR = threads per row (D / 16) when known at compile
+// time (4 or 8), 0 = read it from the arguments.  x is read with coherent loads: it may alias y.  The 16-bit passes
+// keep four blocks per SM (at most 64 registers).
+template <typename T, typename X, int TPR, int U>
+__global__ void __launch_bounds__(256, 8 / sizeof(X)) row_fwd_kernel(const RowArgs a) {
+  // SIXTEEN features per thread: the pass is issue-bound before it is memory-bound (ncu: 84 % issue-slot
+  // utilisation with 8 features per thread), so the per-row bookkeeping (addresses, shuffle steps, predicates) is
+  // spread over twice the bytes.
+  pdl_launch_dependents();
+  pdl_wait();
+  constexpr int E = 16 / sizeof(X);                   // elements of x per 16-byte vector
+  const RowTensor& t = a.t[blockIdx.y];
+  const int tpr = TPR ? TPR : (a.D >> 4);
+  const int rpp = 256 / tpr;                          // rows per pass
   const int tr = threadIdx.x % tpr;
-  const long long total = (long long)a.B * a.H * a.N;
-  const bool ok = row < total;
-  const long long rr = ok ? row : 0;
-  const int n = (int)(rr % a.N);
-  const int h = (int)((rr / a.N) % a.H);
-  const int b = (int)(rr / ((long long)a.N * a.H));
-  const float* xp = a.x + b * a.x_sb + h * a.x_sh + (long long)n * a.x_sn + tr * 8;
-  float4 lo = make_float4(0.f, 0.f, 0.f, 0.f), hi = lo;
-  if (ok) {
-    lo = __ldg(reinterpret_cast<const float4*>(xp));
-    hi = __ldg(reinterpret_cast<const float4*>(xp + 4));
+  const int rows = a.B * t.H * t.N;
+  if (blockIdx.x * (U * rpp) >= rows) return;         // the grid is sized for the longer of the two tensors
+  const int row0 = blockIdx.x * (U * rpp) + threadIdx.x / tpr;
+  const int gs = a.G ? a.D / a.G : 0;
+  const float mul = row_mul<X>(a);
+  uint4 raw[U][16 / E];
+  long long yoff[U];
+#pragma unroll
+  for (int u = 0; u < U; ++u) {
+    const int row = row0 + u * rpp;
+    const int bh = row / t.N, n = row - bh * t.N, b = bh / t.H, h = bh - b * t.H;
+    const X* xp = static_cast<const X*>(t.x.ptr) + b * t.x.sb + h * t.x.sh + (long long)n * t.x.sn + tr * 16;
+    yoff[u] = b * t.y.sb + h * t.y.sh + (long long)n * t.y.sn + tr * 16;
+#pragma unroll
+    for (int v = 0; v < 16 / E; ++v) raw[u][v] = row < rows ? ld_stream128(xp + v * E) : make_uint4(0, 0, 0, 0);
   }
-  float f[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-  const float mul = f32cast_mul(a);
-  float rn[8];
-  if (a.G == 0) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) rn[i] = mul;
-  } else {
-    const int gs = a.D / a.G;
-    if (gs >= 8) {
-      float ss = 0.f;
+  for (int u = 0; u < U; ++u) {
+    const int row = row0 + u * rpp;
+    const bool ok = row < rows;
+    float f[16], rn[16];
 #pragma unroll
-      for (int i = 0; i < 8; ++i) ss += f[i] * f[i];
-      const int tpg = gs >> 3;
-      ss = group_reduce(ss, tpg);
-      const float r = rnorm_of(ss);
+    for (int v = 0; v < 16 / E; ++v) unpack16B<X>(raw[u][v], f + v * E);
+    if (gs == 0) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) rn[i] = r * mul;
-      if (ok && a.rnorm && (tr & (tpg - 1)) == 0) a.rnorm[row * a.G + tr / tpg] = r;
+      for (int i = 0; i < 16; ++i) rn[i] = 1.f;
     } else {
-      float sq[8], ss[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) sq[i] = f[i] * f[i];
-      subgroup_sums8(sq, gs, ss);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float r = rnorm_of(ss[i]);
-        rn[i] = r * mul;
-        if (ok && a.rnorm && (i & (gs - 1)) == 0) a.rnorm[row * a.G + (tr * 8 + i) / gs] = r;
-      }
+      l2norm_fwd_group<16>(f, gs, tr, ok && t.rnorm ? t.rnorm + (long long)row * a.G : nullptr, rn);
     }
-  }
-  if (ok) {
-    uint4 w;
-    w.x = pack2<T>(f[0] * rn[0], f[1] * rn[1]);
-    w.y = pack2<T>(f[2] * rn[2], f[3] * rn[3]);
-    w.z = pack2<T>(f[4] * rn[4], f[5] * rn[5]);
-    w.w = pack2<T>(f[6] * rn[6], f[7] * rn[7]);
-    T* yp = reinterpret_cast<T*>(a.y) + b * a.y_sb + h * a.y_sh + (long long)n * a.y_sn + tr * 8;
-    *reinterpret_cast<uint4*>(yp) = w;
+#pragma unroll
+    for (int i = 0; i < 16; ++i) f[i] *= rn[i] * mul;
+    if (ok) {
+#pragma unroll
+      for (int s = 0; s < 2; ++s)
+        *reinterpret_cast<uint4*>(static_cast<T*>(t.y.ptr) + yoff[u] + 8 * s) = pack16B<T>(f + 8 * s);
+    }
   }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(256) f32_cast_bwd_kernel(const F32CastArgs a) {
+// Backward over a.t[0]: T is the 16-bit type of y, X the type of dy and dx (T or float).  One thread owns 8
+// features of one row, rows are flat over (batch, head, row).  dy is read with coherent loads: the dk pass of the
+// attention backward runs in place (dy == dx).
+template <typename T, typename X>
+__global__ void __launch_bounds__(256) row_bwd_kernel(const RowArgs a) {
+  constexpr int E = 16 / sizeof(X);                   // elements of dy / dx per 16-byte vector
+  const RowTensor& t = a.t[0];
   const int tpr = a.D >> 3;
-  const int rpb = 256 / tpr;
-  const long long row = (long long)blockIdx.x * rpb + threadIdx.x / tpr;
+  const long long row = (long long)blockIdx.x * (256 / tpr) + threadIdx.x / tpr;
   const int tr = threadIdx.x % tpr;
-  const long long total = (long long)a.B * a.H * a.N;
-  const bool ok = row < total;
+  const bool ok = row < (long long)a.B * t.H * t.N;
   const long long rr = ok ? row : 0;
-  const int n = (int)(rr % a.N);
-  const int h = (int)((rr / a.N) % a.H);
-  const int b = (int)(rr / ((long long)a.N * a.H));
-  const float* dyp = a.x + b * a.x_sb + h * a.x_sh + (long long)n * a.x_sn + tr * 8;
-  float4 lo = make_float4(0.f, 0.f, 0.f, 0.f), hi = lo;
-  uint4 ry = make_uint4(0, 0, 0, 0);
-  if (ok) {
-    lo = __ldg(reinterpret_cast<const float4*>(dyp));
-    hi = __ldg(reinterpret_cast<const float4*>(dyp + 4));
-    if (a.G > 0)
-      ry = ldg_stream128(reinterpret_cast<const T*>(a.y) + b * a.y_sb + h * a.y_sh + (long long)n * a.y_sn + tr * 8);
-  }
-  float dy[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-  const float mul = f32cast_mul(a);
-  float out[8];
+  const int n = (int)(rr % t.N);
+  const int h = (int)((rr / t.N) % t.H);
+  const int b = (int)(rr / ((long long)t.N * t.H));
+  const X* dyp = static_cast<const X*>(t.x.ptr) + b * t.x.sb + h * t.x.sh + (long long)n * t.x.sn + tr * 8;
+  uint4 rdy[8 / E], ry = make_uint4(0, 0, 0, 0);
+#pragma unroll
+  for (int v = 0; v < 8 / E; ++v) rdy[v] = ok ? ld_stream128(dyp + v * E) : make_uint4(0, 0, 0, 0);
+  if (ok && a.G > 0)
+    ry = ldg_stream128(static_cast<const T*>(t.y.ptr) + b * t.y.sb + h * t.y.sh + (long long)n * t.y.sn + tr * 8);
+  float g[8];
+#pragma unroll
+  for (int v = 0; v < 8 / E; ++v) unpack16B<X>(rdy[v], g + v * E);
+  const float mul = row_mul<X>(a);
   if (a.G == 0) {
 #pragma unroll
-    for (int i = 0; i < 8; ++i) out[i] = dy[i] * mul;
+    for (int i = 0; i < 8; ++i) g[i] *= mul;
   } else {
     float y[8];
-    {
-      const float2 u0 = unpack2<T>(ry.x), u1 = unpack2<T>(ry.y), u2 = unpack2<T>(ry.z), u3 = unpack2<T>(ry.w);
-      y[0] = u0.x; y[1] = u0.y; y[2] = u1.x; y[3] = u1.y; y[4] = u2.x; y[5] = u2.y; y[6] = u3.x; y[7] = u3.y;
-    }
-    const int gs = a.D / a.G;
-    if (gs >= 8) {
-      float dot = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) dot += y[i] * dy[i];
-      const int tpg = gs >> 3;
-      dot = group_reduce(dot, tpg);
-      const float r = (ok ? a.rnorm[row * a.G + tr / tpg] : 0.f) * mul;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) out[i] = (dy[i] - y[i] * dot) * r;
-    } else {
-      float pr[8], dot[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) pr[i] = y[i] * dy[i];
-      subgroup_sums8(pr, gs, dot);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float r = (ok ? a.rnorm[row * a.G + (tr * 8 + i) / gs] : 0.f) * mul;
-        out[i] = (dy[i] - y[i] * dot[i]) * r;
-      }
-    }
+    unpack16B<T>(ry, y);
+    l2norm_bwd_group<8>(g, y, a.D / a.G, tr, ok ? t.rnorm + row * a.G : nullptr, mul);
   }
-  if (ok) {
-    float* op = a.dx + b * a.o_sb + h * a.o_sh + (long long)n * a.o_sn + tr * 8;
-    *reinterpret_cast<float4*>(op) = make_float4(out[0], out[1], out[2], out[3]);
-    *reinterpret_cast<float4*>(op + 4) = make_float4(out[4], out[5], out[6], out[7]);
-  }
+  if (!ok) return;
+  X* dxp = static_cast<X*>(t.dx.ptr) + b * t.dx.sb + h * t.dx.sh + (long long)n * t.dx.sn + tr * 8;
+#pragma unroll
+  for (int v = 0; v < 8 / E; ++v) *reinterpret_cast<uint4*>(dxp + v * E) = pack16B<X>(g + v * E);
 }
 
-// dx = (dy - y * <y, dy>_group) * rnorm_group
-template <typename T>
-__global__ void __launch_bounds__(256) l2norm_bwd_kernel(const L2Args a) {
-  const int tpr = a.D >> 3;
-  const int rows_per_block = 256 / tpr;
-  const long long row = (long long)blockIdx.x * rows_per_block + threadIdx.x / tpr;
-  const int tr = threadIdx.x % tpr;
-  const long long total_rows = (long long)a.B * a.H * a.N;
-  const bool ok = row < total_rows;
-  const long long rr = ok ? row : 0;
-  const int n = (int)(rr % a.N);
-  const int h = (int)((rr / a.N) % a.H);
-  const int b = (int)(rr / ((long long)a.N * a.H));
-  const T* dyp = reinterpret_cast<const T*>(a.x) + b * a.x_sb + h * a.x_sh + n * a.x_sn + tr * 8;
-  const T* yp = reinterpret_cast<const T*>(a.y) + b * a.y_sb + h * a.y_sh + n * a.y_sn + tr * 8;
-  uint4 rdy = make_uint4(0, 0, 0, 0), ry = make_uint4(0, 0, 0, 0);
-  if (ok) {
-    rdy = *reinterpret_cast<const uint4*>(dyp);
-    ry = *reinterpret_cast<const uint4*>(yp);
-  }
-  float dy[8], y[8];
-  {
-    float2 t0 = unpack2<T>(rdy.x), t1 = unpack2<T>(rdy.y), t2 = unpack2<T>(rdy.z), t3 = unpack2<T>(rdy.w);
-    dy[0] = t0.x; dy[1] = t0.y; dy[2] = t1.x; dy[3] = t1.y; dy[4] = t2.x; dy[5] = t2.y; dy[6] = t3.x; dy[7] = t3.y;
-    float2 u0 = unpack2<T>(ry.x), u1 = unpack2<T>(ry.y), u2 = unpack2<T>(ry.z), u3 = unpack2<T>(ry.w);
-    y[0] = u0.x; y[1] = u0.y; y[2] = u1.x; y[3] = u1.y; y[4] = u2.x; y[5] = u2.y; y[6] = u3.x; y[7] = u3.y;
-  }
-  const int gs = a.D / a.G;
-  float out[8];
-  if (gs >= 8) {
-    float dot = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) dot += y[i] * dy[i];
-    const int tpg = gs >> 3;
-    dot = group_reduce(dot, tpg);
-    const float r = ok ? a.rnorm[row * a.G + tr / tpg] : 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) out[i] = (dy[i] - y[i] * dot) * r;
+// ------------------------------------------------------------------------------------------------
+// launchers: the grid, the instantiation and the launch error of each direction
+// ------------------------------------------------------------------------------------------------
+constexpr int kRowFwdU = 2;                           // forward: rows per thread (16 features each)
+
+template <typename T, typename X>
+cudaError_t launch_row_fwd_t(const RowArgs& a, dim3 grid, cudaStream_t stream) {
+  constexpr int U = kRowFwdU;
+  if (a.D == 64) return launch_pdl(row_fwd_kernel<T, X, 4, U>, grid, dim3(256), 0, stream, a);
+  if (a.D == 128) return launch_pdl(row_fwd_kernel<T, X, 8, U>, grid, dim3(256), 0, stream, a);
+  return launch_pdl(row_fwd_kernel<T, X, 0, U>, grid, dim3(256), 0, stream, a);
+}
+
+// forward over a.t[0] and, when a.t[1].H > 0, a.t[1]; x is float32 when f32_in, else of y's type
+inline cudaError_t launch_row_fwd(const RowArgs& a, bool bf16, bool f32_in, cudaStream_t stream) {
+  const int rows_per_block = kRowFwdU * (256 / (a.D / 16));
+  const long long rows = (long long)a.B * (a.t[0].H * a.t[0].N > a.t[1].H * a.t[1].N ? a.t[0].H * a.t[0].N
+                                                                                     : a.t[1].H * a.t[1].N);
+  const dim3 grid((unsigned)((rows + rows_per_block - 1) / rows_per_block), a.t[1].H ? 2 : 1);
+  if (bf16)
+    return f32_in ? launch_row_fwd_t<__nv_bfloat16, float>(a, grid, stream)
+                  : launch_row_fwd_t<__nv_bfloat16, __nv_bfloat16>(a, grid, stream);
+  return f32_in ? launch_row_fwd_t<__half, float>(a, grid, stream) : launch_row_fwd_t<__half, __half>(a, grid, stream);
+}
+
+// backward over a.t[0]; dy and dx are float32 when f32_grad, else of y's type
+inline cudaError_t launch_row_bwd(const RowArgs& a, bool bf16, bool f32_grad, cudaStream_t stream) {
+  const int rows_per_block = 256 / (a.D / 8);
+  const long long rows = (long long)a.B * a.t[0].H * a.t[0].N;
+  const unsigned grid = (unsigned)((rows + rows_per_block - 1) / rows_per_block);
+  if (bf16) {
+    if (f32_grad) row_bwd_kernel<__nv_bfloat16, float><<<grid, 256, 0, stream>>>(a);
+    else row_bwd_kernel<__nv_bfloat16, __nv_bfloat16><<<grid, 256, 0, stream>>>(a);
   } else {
-    float pr[8], dot[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) pr[i] = y[i] * dy[i];
-    subgroup_sums8(pr, gs, dot);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float r = ok ? a.rnorm[row * a.G + (tr * 8 + i) / gs] : 0.f;
-      out[i] = (dy[i] - y[i] * dot[i]) * r;
-    }
+    if (f32_grad) row_bwd_kernel<__half, float><<<grid, 256, 0, stream>>>(a);
+    else row_bwd_kernel<__half, __half><<<grid, 256, 0, stream>>>(a);
   }
-  if (ok) {
-    uint4 w;
-    w.x = pack2<T>(out[0], out[1]);
-    w.y = pack2<T>(out[2], out[3]);
-    w.z = pack2<T>(out[4], out[5]);
-    w.w = pack2<T>(out[6], out[7]);
-    T* op = reinterpret_cast<T*>(a.dx) + b * a.o_sb + h * a.o_sh + n * a.o_sn + tr * 8;
-    *reinterpret_cast<uint4*>(op) = w;
-  }
+  return cudaGetLastError();
 }
 
 }  // namespace fcsa

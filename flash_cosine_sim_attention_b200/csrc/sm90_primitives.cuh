@@ -100,6 +100,16 @@ __device__ __forceinline__ uint4 ldg_stream128(const void* p) {
   return v;
 }
 
+// 16-byte read of data that is touched once, with an ordinary (coherent) load: for data the same kernel may also
+// write, where the read-only path of ldg_stream128 is not allowed
+__device__ __forceinline__ uint4 ld_stream128(const void* p) {
+  uint4 v;
+  asm volatile("ld.global.L1::no_allocate.v4.u32 {%0, %1, %2, %3}, [%4];"
+               : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
+               : "l"(p));
+  return v;
+}
+
 // named barrier among a subset of the CTA's warps
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

@@ -100,3 +100,32 @@ def test_backward_rejects_missing_zeroed_workspace(lib):
     rc = lib.fcsa_backward(_abi.ref(p), *([_abi.ref(t)] * 5), 4096, *([_abi.ref(t)] * 3), 4096, need, None, 0, None)
     assert rc == _abi.FCSA_ERR_WORKSPACE and b"zeroed workspace" in lib.fcsa_last_error()
     assert lib.fcsa_zeroed_init(None, 0, None) == _abi.FCSA_ERR_INVALID
+
+
+def test_row_pass_shape_checks(lib):
+    """The 16-bit l2norm takes head dims 32 to 256 and groups > 0; the float32 cast takes 16 to 128 and groups >= 0
+    (0: a plain scaled cast).  Shapes that pass reach the null-tensor check, so nothing here is launched."""
+    t = _abi.FcsaTensor(None, 0, 0, 0)
+
+    def l2(D, G, dtype=_abi.FCSA_BF16, B=1):
+        rc = lib.fcsa_l2norm_forward(dtype, B, 1, 8, D, G, _abi.ref(t), _abi.ref(t), None, None)
+        return rc, lib.fcsa_last_error()
+
+    def f32(D, G, dtype=_abi.FCSA_BF16, B=1):
+        rc = lib.fcsa_f32_cast(dtype, B, 1, 8, D, G, _abi.ref(t), _abi.ref(t), None, None, 0, None)
+        return rc, lib.fcsa_last_error()
+
+    accepted = (_abi.FCSA_ERR_INVALID, b"null")
+    for fn, prefix in ((l2, b"l2norm: "), (f32, b"f32 cast: ")):
+        assert fn(64, 1, dtype=7)[0] == _abi.FCSA_ERR_UNSUPPORTED
+        assert fn(64, 1, B=0) == (_abi.FCSA_ERR_INVALID, prefix + b"empty tensor")
+        for D in (8, 48, 96, 512):
+            assert fn(D, 1) == (_abi.FCSA_ERR_UNSUPPORTED, prefix + b"head_dim %d not implemented" % D)
+        for G in (-1, 3, 128):
+            rc, msg = fn(64, G)
+            assert rc == _abi.FCSA_ERR_INVALID and msg.startswith(prefix + b"groups")
+        for G in (1, 2, 16, 64):
+            assert fn(64, G)[0] == accepted[0] and accepted[1] in fn(64, G)[1]
+    assert l2(16, 1)[0] == _abi.FCSA_ERR_UNSUPPORTED and accepted[1] in f32(16, 1)[1]
+    assert accepted[1] in l2(256, 1)[1] and f32(256, 1)[0] == _abi.FCSA_ERR_UNSUPPORTED
+    assert l2(64, 0)[1].startswith(b"l2norm: groups") and accepted[1] in f32(64, 0)[1]
