@@ -1,0 +1,265 @@
+"""CPU tests of the element-wise error bound (tests/elementwise_bounds.py), both ways: its reference part is the
+oracle, it accepts an emulation of the kernels' roundings with margin, and it rejects the tile-shaped mistakes that
+the relative-to-max metric of the GPU tests lets through."""
+import numpy as np
+import pytest
+import torch
+
+from elementwise_bounds import C, U, attention_bounds, check_bound, kernel_shift
+from gqa_reference import gqa_attention
+from oracle import cosine_sim_attention_oracle as oracle
+
+# (q shape, k shape, kwargs, bias planes or None): bias with d_bias, mask, causal Nq != Nk, groups, GQA, MQA,
+# merged batch-heads and l2norm_qk=False
+CASES = {
+    "bias_heads_mask_cross": ((2, 3, 70, 64), (2, 3, 90, 64), dict(mask_p=0.4), "heads"),
+    "bias_batch_causal": ((2, 2, 80, 64), (2, 2, 80, 64), dict(causal=True), "batch"),
+    "causal_q_lt_k": ((1, 2, 40, 64), (1, 2, 150, 64), dict(causal=True), None),
+    "causal_q_gt_k": ((1, 2, 150, 128), (1, 2, 40, 128), dict(causal=True), None),
+    "groups4_scale2": ((1, 2, 100, 64), (1, 2, 100, 64), dict(groups=4, scale=2), None),
+    "gqa_6_3": ((2, 6, 60, 64), (2, 3, 90, 64), dict(mask_p=0.3), None),
+    "gqa_bias_causal": ((1, 4, 64, 64), (1, 2, 64, 64), dict(causal=True), "heads"),
+    "mqa": ((2, 4, 70, 64), (2, 70, 64), dict(causal=True), None),
+    "merged": ((4, 90, 64), (4, 90, 64), dict(causal=True), None),
+    "no_l2norm": ((1, 2, 80, 64), (1, 2, 80, 64), dict(l2norm_qk=False, scale=1, amp=0.2), None),
+}
+
+
+def make_case(name, fmt, seed=0):
+    qs, ks, kw, bias_kind = CASES[name]
+    kw = dict(kw)
+    rng = np.random.default_rng(seed)
+    rnd = lambda shape, amp=1.0: oracle.round_to(rng.standard_normal(shape) * amp, fmt)
+    amp = kw.pop("amp", 1.0)
+    q, k, v, do = rnd(qs, amp), rnd(ks, amp), rnd(ks), rnd(qs)
+    mask_p = kw.pop("mask_p", None)
+    if mask_p is not None:
+        kw["mask"] = rng.random((qs[0], ks[-2])) > mask_p
+        kw["mask"][:, 0] = True
+    if bias_kind is not None:
+        planes = qs[0] if bias_kind == "batch" else qs[1]
+        kw["attn_bias"] = rnd((planes, qs[-2], ks[-2]))
+        kw["attn_bias_batch_dim"] = bias_kind == "batch"
+    return q, k, v, do, kw
+
+
+def reference(q, k, v, do, kw, fmt):
+    """oracle.attention (through gqa_attention for grouped keys/values) with the 16-bit q^, k^ of `fmt`."""
+    rq = fmt if kw.get("l2norm_qk", True) else None
+    f = gqa_attention if (k.ndim == 4 and q.ndim == 4 and k.shape[1] != q.shape[1]) else oracle.attention
+    return f(q, k, v, d_out=do, empty_rows="zero", round_qk=rq, **kw)
+
+
+@pytest.mark.parametrize("name", sorted(CASES))
+def test_reference_matches_oracle(name):
+    q, k, v, do, kw = make_case(name, "bf16")
+    want = reference(q, k, v, do, kw, "bf16")
+    ref, bound = attention_bounds(q, k, v, do, round_qk="bf16" if kw.get("l2norm_qk", True) else None, chunk=32,
+                                  **kw)
+    names = ("o", "dq", "dk", "dv", "d_bias")[:len(want)]
+    assert sorted(ref) == sorted(names)
+    for n, w in zip(names, want):
+        got = ref[n].numpy()
+        assert got.shape == w.shape, n
+        assert np.abs(got - w).max() <= 1e-12 * max(1.0, np.abs(w).max()), n
+        assert (bound[n].numpy() >= np.abs(w) - 1e-12).all(), n      # M is never below |ref| (it contains it)
+
+
+# ---- a numpy emulation of the kernels' rounding points ---------------------------------------------------------
+def emulate(q, k, v, do, fmt, mask=None, attn_bias=None, scale=8, groups=1, causal=False, l2norm_qk=True,
+            attn_bias_batch_dim=False):
+    """What the kernels compute, in float32 with every 16-bit rounding in its place: q^, k^ stored in T; S = q^ k^T
+    and p = exp(scale S + bias - shift) in fp32; p -> T before P V, l summed in fp32, o -> T; in the backward
+    delta from the stored o, P -> T before dV, dS -> T before dK / dQ, the l2norm backward on the stored q^, k^ with
+    fp32 1/||x||, outputs -> T (d_bias summed in fp32)."""
+    f32 = np.float32
+    T = lambda x: oracle.round_to(x, fmt).astype(f32)
+    shift = f32(kernel_shift(fmt, scale, groups, l2norm_qk, attn_bias))
+    merged, single = q.ndim == 3, k.ndim == 3
+    if merged:
+        q, k, v, do = q[:, None], k[:, None], v[:, None], do[:, None]
+        attn_bias_batch_dim = True
+    elif single:
+        k, v = k[:, None], v[:, None]
+    B, H, Nq, D = q.shape
+    Hk, Nk = k.shape[1], k.shape[2]
+    G = H // Hk
+    if l2norm_qk:
+        (qn, nq), (kn, nk) = oracle.l2norm(q, groups), oracle.l2norm(k, groups)
+        qn, kn = T(qn), T(kn)
+    else:
+        qn, kn = q.astype(f32), k.astype(f32)
+    v, do = v.astype(f32), do.astype(f32)
+    bias = None if attn_bias is None else attn_bias.astype(f32)
+    o = np.zeros(q.shape, f32)
+    dqn, dkn, dv = np.zeros(q.shape, f32), np.zeros(k.shape, f32), np.zeros(v.shape, f32)
+    db = None if bias is None else np.zeros(bias.shape, f32)
+    for b in range(B):
+        vis = oracle._visibility(b, Nq, Nk, mask, causal)
+        for h in range(H):
+            hk = h // G
+            logit = f32(scale) * (qn[b, h] @ kn[b, hk].T)
+            if bias is not None:
+                logit = logit + bias[b if attn_bias_batch_dim else h]
+            p = np.where(vis, np.exp(logit - shift), f32(0))
+            l = p.sum(-1, dtype=f32)
+            inv_l = f32(1) / np.maximum(l, f32(1e-37))
+            o[b, h] = T((T(p) @ v[b, hk]) * inv_l[:, None])
+            delta = (do[b, h] * o[b, h]).sum(-1, dtype=f32, keepdims=True)
+            with np.errstate(over="ignore"):         # rows without a visible key: 0 * (1 / 1e-37), then masked
+                P = np.where(vis, np.exp(logit - shift) * inv_l[:, None], f32(0))
+            dv[b, hk] += T(P).T @ do[b, h]
+            ds = P * (do[b, h] @ v[b, hk].T - delta)
+            dsr = T(ds)
+            dqn[b, h] = f32(scale) * (dsr @ kn[b, hk])
+            dkn[b, hk] += f32(scale) * (dsr.T @ qn[b, h])
+            if db is not None:
+                db[b if attn_bias_batch_dim else h] += ds
+
+    def l2bwd(dy, y, n):
+        g = y.reshape(*y.shape[:-1], groups, -1)
+        d = dy.reshape(g.shape)
+        return ((d - g * (g * d).sum(-1, keepdims=True)) * (f32(1) / n.astype(f32))[..., None]).reshape(y.shape)
+    dq, dk = (l2bwd(dqn, qn, nq), l2bwd(dkn, kn, nk)) if l2norm_qk else (dqn, dkn)
+    out = [T(o), T(dq), T(dk), T(dv)] + ([] if db is None else [T(db)])
+    if merged:
+        out[0], out[1], out[2], out[3] = out[0][:, 0], out[1][:, 0], out[2][:, 0], out[3][:, 0]
+    elif single:
+        out[2], out[3] = out[2][:, 0], out[3][:, 0]
+    return out
+
+
+EMULATION_WORST = {}
+
+
+@pytest.mark.parametrize("fmt", ["bf16", "f16"])
+@pytest.mark.parametrize("name", sorted(CASES) + ["long_causal"])
+def test_emulated_rounding_within_bound(name, fmt):
+    """The emulation stays within the bound with margin: its worst err / (u M) is at most C / 2."""
+    if name == "long_causal":
+        rng = np.random.default_rng(1)
+        q, k, v, do = (oracle.round_to(rng.standard_normal((1, 1, 2048, 64)), fmt) for _ in range(4))
+        kw = dict(causal=True)
+    else:
+        q, k, v, do, kw = make_case(name, fmt, seed=3)
+    got = emulate(q, k, v, do, fmt, **kw)
+    rq = fmt if kw.get("l2norm_qk", True) else None
+    shift = kernel_shift(fmt, kw.get("scale", 8), kw.get("groups", 1), kw.get("l2norm_qk", True),
+                         kw.get("attn_bias"))
+    ref, bound = attention_bounds(q, k, v, do, round_qk=rq, fmt=fmt, shift=shift, chunk=512, **kw)
+    for n, g in zip(("o", "dq", "dk", "dv", "d_bias"), got):
+        w = check_bound(n, torch.from_numpy(g), ref, bound, fmt, c=C / 2) * C / 2
+        EMULATION_WORST[f"{fmt}:{n}"] = max(EMULATION_WORST.get(f"{fmt}:{n}", 0.0), w)
+
+
+# ---- planted errors: kernel-shaped mistakes, built from float64 results, that the bound must reject --------------
+N = 2048
+
+
+def rel_err(got, ref):
+    return float(np.abs(got - ref).max() / np.abs(ref).max())
+
+
+@pytest.fixture(scope="module")
+def long_causal():
+    """(1, 1, 2048, 64) bf16 causal: float64 reference and bound.  The same problem with a per-head bias gives
+    d_bias ("biased")."""
+    rng = np.random.default_rng(0)
+    q, k, v, do = (oracle.round_to(rng.standard_normal((1, 1, N, 64)), "bf16") for _ in range(4))
+    bias = oracle.round_to(rng.standard_normal((1, N, N)) * 0.5, "bf16")
+    ref, bound = attention_bounds(q, k, v, do, causal=True, round_qk="bf16", fmt="bf16")
+    bref, bbound = attention_bounds(q, k, v, do, causal=True, attn_bias=bias, round_qk="bf16", fmt="bf16")
+    qn = oracle.round_to(oracle.l2norm(q)[0], "bf16")[0, 0]
+    kn = oracle.round_to(oracle.l2norm(k)[0], "bf16")[0, 0]
+    return dict(q=q, k=k, v=v, do=do, qn=qn, kn=kn, ref={n: t.numpy() for n, t in ref.items()}, tref=ref,
+                bound=bound, biased=(bref, bbound))
+
+
+def _rows(d, r0, r1, vis):
+    """o and dS of query rows [r0, r1) of the long causal problem under a visibility of their own."""
+    s = 8.0 * d["qn"][r0:r1] @ d["kn"].T
+    s = np.where(vis, s, -np.inf)
+    p = np.exp(s - s.max(-1, keepdims=True))
+    p /= p.sum(-1, keepdims=True)
+    v, do = d["v"][0, 0], d["do"][0, 0, r0:r1]
+    o = p @ v
+    ds = p * (do @ v.T - (do * o).sum(-1, keepdims=True))
+    return o, ds
+
+
+def _causal_vis(r0, r1, extra=0):
+    return np.arange(N)[None, :] <= np.arange(r0, r1)[:, None] + extra
+
+
+def _plant(d, what):
+    ref = d["ref"]
+    last_q, last_k = slice(N - 64, N), slice(N - 128, N)
+    if what == "dv_last_key_tile_zero":
+        g = ref["dv"].copy(); g[..., last_k, :] = 0
+        return "dv", g
+    if what == "dk_last_key_tile_x0.7":
+        g = ref["dk"].copy(); g[..., last_k, :] *= 0.7
+        return "dk", g
+    if what == "dq_last_query_tile_x0.7":
+        g = ref["dq"].copy(); g[..., last_q, :] *= 0.7
+        return "dq", g
+    if what == "o_last_query_tile_x0.7":
+        g = ref["o"].copy(); g[..., last_q, :] *= 0.7
+        return "o", g
+    if what == "o_late_tile_without_key_tile_3":
+        r0, r1 = N - 256, N - 128                      # forward query tile 14 drops keys 384..511
+        vis = _causal_vis(r0, r1)
+        vis[:, 384:512] = False
+        g = ref["o"].copy(); g[0, 0, r0:r1] = _rows(d, r0, r1, vis)[0]
+        return "o", g
+    if what == "o_causal_diagonal_off_by_one":
+        r0, r1 = N - 384, N - 256                      # forward query tile 13 sees one key past the diagonal
+        g = ref["o"].copy(); g[0, 0, r0:r1] = _rows(d, r0, r1, _causal_vis(r0, r1, extra=1))[0]
+        return "o", g
+    if what == "dq_tile_missing_64_keys":
+        r0, r1 = N - 128, N - 64                       # backward query tile 30 misses keys 1088..1151 (one half-tile)
+        _, ds = _rows(d, r0, r1, _causal_vis(r0, r1))
+        dqn = 8.0 * ds[:, 1088:1152] @ d["kn"][1088:1152]
+        g = ref["dq"].copy()
+        g[0, 0, r0:r1] -= oracle.l2norm_backward(dqn, d["q"][0, 0, r0:r1])
+        return "dq", g
+    if what == "d_bias_missing_query_tile":
+        g = d["biased"][0]["d_bias"].numpy().copy(); g[0, N - 64:] = 0
+        return "d_bias", g
+    raise ValueError(what)
+
+
+TOL = {"o": 1e-2, "dq": 2e-2, "dk": 2e-2, "dv": 2e-2, "d_bias": 2e-2}
+PLANTS = ["dv_last_key_tile_zero", "dk_last_key_tile_x0.7", "dq_last_query_tile_x0.7", "o_last_query_tile_x0.7",
+          "o_late_tile_without_key_tile_3", "o_causal_diagonal_off_by_one", "dq_tile_missing_64_keys",
+          "d_bias_missing_query_tile"]
+
+
+@pytest.mark.parametrize("what", PLANTS)
+def test_planted_error_fails_the_bound(long_causal, what, capsys):
+    name, got = _plant(long_causal, what)
+    ref, bound = long_causal["biased"] if name == "d_bias" else (long_causal["tref"], long_causal["bound"])
+    old = rel_err(got, ref[name].numpy())
+    with pytest.raises(AssertionError, match="element-wise bound") as e:
+        check_bound(name, torch.from_numpy(got), ref, bound, "bf16")
+    with capsys.disabled():
+        print(f"\n  planted {what}: rel_err {old:.3g} (tolerance {TOL[name]:g}: "
+              f"{'passes' if old <= TOL[name] else 'fails'}); bound: {str(e.value).split(' at ')[0]}")
+
+
+def test_bound_accepts_the_unplanted_reference(long_causal):
+    for ref, bound in ((long_causal["tref"], long_causal["bound"]), long_causal["biased"]):
+        for n, t in ref.items():
+            assert check_bound(n, t, ref, bound, "bf16") == 0.0
+
+
+def test_constants():
+    assert U["bf16"] == 2.0 ** -8 and U["f16"] == 2.0 ** -11 and C == 2.0
+
+
+def test_report_emulation_worst(capsys):
+    """Prints the emulation's worst err / (u M) per format and quantity (what C is chosen from) when the emulation
+    tests ran in the same session."""
+    with capsys.disabled():
+        for key in sorted(EMULATION_WORST):
+            print(f"\n  emulation worst {key}: {EMULATION_WORST[key]:.3f} u M", end="")

@@ -14,7 +14,7 @@ import pytest
 import torch
 
 from gqa_reference import gqa_attention
-from test_gpu_parity import ROUND, TOL_GRAD, TOL_OUT, fcsa, make_inputs, record, rel_err  # noqa: F401
+from test_gpu_parity import ROUND, TOL_GRAD, TOL_OUT, bound_check, fcsa, make_inputs, record, rel_err  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -73,6 +73,7 @@ def gqa_check(fcsa, qs, kvs, dtype, seed=0, mask_p=None, path=None, **kw):
         e = rel_err(t.grad, r)
         record(dtype, name, e, TOL_GRAD[dtype])
         assert e <= TOL_GRAD[dtype], name
+    bound_check(dtype, {"o": o, "dq": qd.grad, "dk": kd.grad, "dv": vd.grad}, q, k, v, do, mask=mask, **kw)
     return qd, kd, vd
 
 
@@ -175,6 +176,8 @@ def test_gqa_attn_bias(fcsa, batch_dim, dim_head, dtype):
         e = rel_err(t.grad, r)
         record(dtype, name, e, TOL_GRAD[dtype])
         assert e <= TOL_GRAD[dtype], name
+    bound_check(dtype, {"o": o, "dq": qd.grad, "dk": kd.grad, "dv": vd.grad, "d_bias": bd.grad}, q, k, v, do,
+                mask=m, attn_bias=bias, attn_bias_batch_dim=batch_dim)
 
 
 @pytest.mark.parametrize("causal", [False, True])

@@ -7,6 +7,8 @@ Tolerance policy (floating point; stated per test):
   max |got - ref| <= tol * max |ref|, tol = 1e-2 for bf16 and 2e-3 for f16 outputs, 2e-2 / 4e-3
   for gradients (they pass through two more 16-bit roundings: P/dS operands and the stored
   normalised q, k).  The reference's own tests allow 1e-1 absolute in f16 (tests/test.py:12-18,49).
+Next to it, element-wise: |got - ref| <= C u M for every element of every output, M modelling the kernels'
+roundings (tests/elementwise_bounds.py); the worst err / (C u M) is recorded under '<dtype>:<name>/bound'.
 """
 import ast
 import glob
@@ -16,6 +18,7 @@ import numpy as np
 import pytest
 import torch
 
+from elementwise_bounds import FMT, attention_bounds, check_bound, kernel_shift, round_to
 from oracle import cosine_sim_attention_oracle as oracle
 
 pytestmark = pytest.mark.gpu
@@ -58,6 +61,48 @@ def rel_err(got, ref):
     return np.abs(got - ref).max() / mag
 
 
+def float32_operands(q, k, v, do, attn_bias=None, scale=8, groups=1, l2norm_qk=True):
+    """What the float32 path hands the 16-bit kernels (_float32_on_half_kernels): the operand type, and v, dO
+    divided by their `_pow2_scale` factors, rounded and scaled back (exact), the bias rounded, q, k rounded when
+    they are not normalised inside the op.  Returns (fmt, q, k, v, do, bias) as float64 CPU tensors."""
+    from flash_cosine_sim_attention_b200.flash_cosine_sim_attention import _FP16_GROUPED_RANGE, _pow2_scale
+    fmt = "f16" if (l2norm_qk and scale * groups <= _FP16_GROUPED_RANGE) else "bf16"
+    t64 = lambda t: None if t is None else torch.as_tensor(t).detach().cpu().double()
+    q, k, v, do, attn_bias = (t64(t) for t in (q, k, v, do, attn_bias))
+
+    def scaled(t):
+        s = _pow2_scale(t.float(), 1).double()
+        return round_to(t / s, fmt) * s
+    if not l2norm_qk:
+        q, k = round_to(q, fmt), round_to(k, fmt)
+    return fmt, q, k, scaled(v), None if do is None else scaled(do), round_to(attn_bias, fmt)
+
+
+def bound_check(dtype, got, q, k, v, do=None, mask=None, **kw):
+    """The element-wise bound of every output in `got` ({name: tensor}) against the float64 reference of the same
+    inputs, computed on the GPU; records the worst err / (C u M) per dtype and quantity under '<name>/bound'.
+    float32 inputs are judged on the operands the 16-bit kernels really see (float32_operands)."""
+    l2 = kw.get("l2norm_qk", True)
+    bias = kw.get("attn_bias")
+    if dtype == torch.float32:
+        fmt, q, k, v, do, kw["attn_bias"] = float32_operands(q, k, v, do, bias, kw.get("scale", 8),
+                                                             kw.get("groups", 1), l2)
+    else:
+        fmt = FMT[dtype]
+    shift = kernel_shift(fmt, kw.get("scale", 8), kw.get("groups", 1), l2, bias)
+    ref, bound = attention_bounds(q, k, v, do, mask=mask, round_qk=fmt if l2 else None, fmt=fmt, shift=shift,
+                                  device="cuda", **kw)
+    worst = {}
+    for name, t in got.items():
+        try:
+            worst[name] = check_bound(name, t, ref, bound, fmt)
+        except AssertionError:
+            record(dtype, f"{name}/bound", float("inf"), 1.0)
+            raise
+        record(dtype, f"{name}/bound", worst[name], 1.0)
+    return worst
+
+
 def make_inputs(qs, kvs, dtype, seed, mask_p=None, amp=1.0):
     g = torch.Generator().manual_seed(seed)
     q = (torch.randn(qs, generator=g) * amp).to(dtype)
@@ -86,6 +131,7 @@ def check(fcsa, qs, kvs, dtype, seed=0, mask_p=None, grads=True, amp=1.0, **kw):
         e = rel_err(o, ref)
         record(dtype, "o", e, TOL_OUT[dtype])
         assert e <= TOL_OUT[dtype]
+        bound_check(dtype, {"o": o}, q, k, v, mask=mask, **kw)
         return
     o.backward(do.to(dev))
     e = rel_err(o, ref[0])
@@ -96,6 +142,7 @@ def check(fcsa, qs, kvs, dtype, seed=0, mask_p=None, grads=True, amp=1.0, **kw):
         e = rel_err(t.grad, r)
         record(dtype, name, e, TOL_GRAD[dtype])
         assert e <= TOL_GRAD[dtype], name
+    bound_check(dtype, {"o": o, "dq": qd.grad, "dk": kd.grad, "dv": vd.grad}, q, k, v, do, mask=mask, **kw)
 
 
 # ---- the reference's own test grid (tests/test.py:31-125), on the dtypes/head dims the kernels cover,
@@ -156,6 +203,8 @@ def test_attn_bias(fcsa, causal, mask, dim_head, dtype, batch_dim):
     for name, t, r in (("dq", qd, ref[1]), ("dk", kd, ref[2]), ("dv", vd, ref[3]), ("d_bias", bd, ref[4])):
         assert t.grad is not None and t.grad.shape == t.shape and t.grad.dtype == dtype, name
         assert rel_err(t.grad, r) <= TOL_GRAD[dtype], name
+    bound_check(dtype, {"o": o, "dq": qd.grad, "dk": kd.grad, "dv": vd.grad, "d_bias": bd.grad}, q, k, v, do,
+                mask=m, attn_bias=bias, causal=causal, attn_bias_batch_dim=batch_dim)
 
 
 def test_attn_bias_single_head_kv_grouped_l2norm(fcsa):
@@ -625,6 +674,11 @@ def _slice_check(fcsa, shape, dtype, slices, grads=True):
         if grads:
             for t, r in zip((qd, kd, vd), ref[1:]):
                 assert rel_err(t.grad[b:b + 1, h:h + 1], r) <= TOL_GRAD[dtype]
+        ts = lambda t: t[b:b + 1, h:h + 1]
+        got = {"o": ts(o)}
+        if grads:
+            got.update(dq=ts(qd.grad), dk=ts(kd.grad), dv=ts(vd.grad))
+        bound_check(dtype, got, ts(q), ts(k), ts(v), ts(do) if grads else None, causal=True)
     return qd, kd, vd, o
 
 
@@ -683,6 +737,8 @@ def test_config3_every_batch_head_against_float64_on_gpu(fcsa, dtype):
         tol = TOL_OUT[dtype] if name == "o" else TOL_GRAD[dtype]
         record(dtype, f"{name}@C3x32", err, tol)
         assert err <= tol, (name, err)
+    # every element of all 32 problems under the element-wise bound, its float64 reference computed on the GPU
+    bound_check(dtype, {"o": o, "dq": qd.grad, "dk": kd.grad, "dv": vd.grad}, q, k, v, do, causal=True)
 
 
 def test_config5_long_context_slice_16384x128(fcsa):
