@@ -7,6 +7,7 @@ from .flash_cosine_sim_attention import (  # noqa: F401
     debug,
     flash_cosine_sim_attention,
     flash_cosine_sim_attention_cuda,
+    flash_cosine_sim_attention_with_kv_cache,
     l2norm_tensors,
     plain_cosine_sim_attention,
     release_workspaces,

@@ -40,6 +40,8 @@ EXPORTED_SYMBOLS = (
     "fcsa_backward_bias",
     "fcsa_f32_cast",
     "fcsa_f32_cast_backward",
+    "fcsa_decode_workspace_bytes",
+    "fcsa_decode",
 )
 
 
@@ -134,6 +136,10 @@ def load():
     lib.fcsa_f32_cast.argtypes = [c_int32] * 6 + [PT, PT, c_void_p, c_void_p, c_int32, c_void_p]
     lib.fcsa_f32_cast_backward.restype = c_int32
     lib.fcsa_f32_cast_backward.argtypes = [c_int32] * 6 + [PT, PT, c_void_p, PT, c_void_p, c_int32, c_void_p]
+    lib.fcsa_decode_workspace_bytes.restype = c_size_t
+    lib.fcsa_decode_workspace_bytes.argtypes = [PP, c_int32]
+    lib.fcsa_decode.restype = c_int32
+    lib.fcsa_decode.argtypes = [PP, PT, PT, PT, c_void_p, PT, PT, c_int32, c_int32, PT, c_void_p, c_size_t, c_void_p]
     lib.fcsa_set_kernel_events.restype = c_int32
     lib.fcsa_set_kernel_events.argtypes = [c_int32, c_void_p, c_void_p]
     _lib = lib

@@ -18,6 +18,7 @@
 
 #include "../../include/fcsa_b200.h"
 #include "bwd_kernel.cuh"
+#include "decode_kernel.cuh"
 #include "fwd_kernel.cuh"
 #include "l2norm_kernels.cuh"
 #include "tensor_map.h"
@@ -169,6 +170,87 @@ fcsa::RowArgs row_args(int32_t B, int32_t D, int32_t G, const float* mul = nullp
   fcsa::RowArgs a = {};
   a.B = B; a.D = D; a.G = G; a.mul = mul; a.mul_reciprocal = mul_reciprocal;
   return a;
+}
+
+// ---- key/value-cache decode --------------------------------------------------------------------
+// The problem of a decode call: seq_q = new queries, seq_k = cache capacity; no key mask, 16-bit output.
+int check_decode_problem(const fcsa_problem* p, int32_t n_new) {
+  int r;
+  if ((r = check_problem(p))) return r;
+  if (p->key_mask) return fail(FCSA_ERR_UNSUPPORTED, "decode: no key mask (cache_seqlens gives the valid rows)");
+  if (p->out_f32) return fail(FCSA_ERR_UNSUPPORTED, "decode: out_f32 is not implemented");
+  if (n_new < 0) return fail(FCSA_ERR_INVALID, "decode: n_new %d < 0", n_new);
+  if ((long long)(p->heads / p->kv_heads) * p->seq_q > 0x7FFFFFFFLL - 64)
+    return fail(FCSA_ERR_INVALID, "decode: heads per kv head x seq_q too large");
+  return FCSA_OK;
+}
+
+struct DecodeShape {
+  int R, n_rb, n_split;
+  long long items;
+};
+
+// rows, row blocks, work items and splits of a decode problem on the current device
+int decode_shape(const fcsa_problem* p, DecodeShape* s) {
+  int sms = 0;
+  const cudaError_t e = fcsa::device_sm_count(&sms);
+  if (e != cudaSuccess) return cuda_fail(e, "cudaDeviceGetAttribute(multiProcessorCount)");
+  s->R = (p->heads / p->kv_heads) * p->seq_q;
+  s->n_rb = (s->R + 63) / 64;
+  s->items = (long long)p->batch * p->kv_heads * s->n_rb;
+  s->n_split = fcsa::decode_split(s->items, p->seq_k, sms);
+  return FCSA_OK;
+}
+
+size_t align16(size_t n) { return (n + 15) & ~size_t(15); }
+
+size_t decode_qhat_bytes(const fcsa_problem* p) {
+  return align16((size_t)p->batch * p->heads * p->seq_q * p->head_dim * 2);
+}
+
+template <typename T, int D>
+int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tensor* q, const fcsa_tensor* kc,
+                  const fcsa_tensor* vc, const int32_t* seqlens, int32_t n_new, const fcsa_tensor* o, float* part,
+                  cudaStream_t stream) {
+  using Cfg = fcsa::DecodeCfg<D>;
+  const bool bf = p->dtype == FCSA_BF16;
+  CUtensorMap tk, tv;
+  int r;
+  if ((r = fcsa::make_tensor_map_bhnd(&tk, kc->ptr, fcsa::tma_dtype16(bf), p->batch, p->kv_heads, p->seq_k, D, kc->sb,
+                                      kc->sh, kc->sn, 128)))
+    return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "k_cache: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map" : "cuTensorMapEncodeTiled failed", r);
+  if ((r = fcsa::make_tensor_map_bhnd(&tv, vc->ptr, fcsa::tma_dtype16(bf), p->batch, p->kv_heads, p->seq_k, D, vc->sb,
+                                      vc->sh, vc->sn, 128)))
+    return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "v_cache: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map" : "cuTensorMapEncodeTiled failed", r);
+  fcsa::DecodeArgs a;
+  a.B = p->batch; a.H = p->heads; a.KVH = p->kv_heads; a.G = p->heads / p->kv_heads;
+  a.Nq = p->seq_q; a.cap = p->seq_k; a.n_new = n_new;
+  a.causal = p->causal ? 1 : 0;
+  a.R = sh.R; a.n_rb = sh.n_rb; a.n_split = sh.n_split;
+  const float log2e = 1.4426950408889634f;
+  a.c1 = p->scale * log2e;
+  a.c2 = p->shift * log2e;
+  a.seqlens = seqlens;
+  a.q = q->ptr; a.q_sb = q->sb; a.q_sh = q->sh; a.q_sn = q->sn;
+  a.o = o->ptr; a.o_sb = o->sb; a.o_sh = o->sh; a.o_sn = o->sn;
+  a.part = part;
+  {
+    cudaError_t e = fcsa::ensure_dynamic_smem<fcsa::fcsa_decode_kernel<T, D>>(Cfg::kSmem);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(decode)");
+  }
+  const long long grid = sh.items * sh.n_split;
+  if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "decode: problem too large for one launch");
+  cudaError_t e = fcsa::launch_pdl(fcsa::fcsa_decode_kernel<T, D>, dim3((unsigned)grid), dim3(Cfg::kThreads),
+                                   Cfg::kSmem, stream, tk, tv, a);
+  if (e != cudaSuccess) return cuda_fail(e, "decode kernel launch");
+  g_launches.fetch_add(1);
+  if (sh.n_split == 1) return FCSA_OK;
+  const long long threads = sh.items * 64 * (D / 4);
+  e = fcsa::launch_pdl(fcsa::decode_combine_kernel<T, D>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0,
+                       stream, a);
+  if (e != cudaSuccess) return cuda_fail(e, "decode combine launch");
+  g_launches.fetch_add(1);
+  return FCSA_OK;
 }
 
 }  // namespace
@@ -412,6 +494,56 @@ int fcsa_l2norm_backward(int32_t dtype, int32_t batch, int32_t heads, int32_t ro
   a.t[0] = {heads, rows, *dy, *y, *dx, const_cast<float*>(rnorm)};
   return row_pass_launched(fcsa::launch_row_bwd(a, dtype == FCSA_BF16, false, reinterpret_cast<cudaStream_t>(stream)),
                            "l2norm backward launch");
+}
+
+size_t fcsa_decode_workspace_bytes(const fcsa_problem* p, int32_t n_new) {
+  DecodeShape sh;
+  if (check_decode_problem(p, n_new) || decode_shape(p, &sh)) return 0;
+  return decode_qhat_bytes(p) + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
+}
+
+int fcsa_decode(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k_cache, const fcsa_tensor* v_cache,
+                const int32_t* cache_seqlens, const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t n_new,
+                int32_t groups, const fcsa_tensor* o, void* workspace, size_t workspace_bytes, void* stream) {
+  int r;
+  if ((r = check_decode_problem(p, n_new))) return r;
+  if ((r = check_tensor(q, "q")) || (r = check_tensor(k_cache, "k_cache")) || (r = check_tensor(v_cache, "v_cache")) ||
+      (r = check_tensor(o, "o")))
+    return r;
+  if (n_new > 0 && ((r = check_tensor(k_new, "k")) || (r = check_tensor(v_new, "v")))) return r;
+  if (groups != 0 && (r = check_rows(false, p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, groups))) return r;
+  if (!cache_seqlens) return fail(FCSA_ERR_INVALID, "cache_seqlens: null");
+  DecodeShape sh;
+  if ((r = decode_shape(p, &sh))) return r;
+  const size_t qbytes = decode_qhat_bytes(p);
+  const size_t need = qbytes + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
+  if (!workspace || workspace_bytes < need)
+    return fail(FCSA_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need, workspace_bytes);
+  if (!aligned16(workspace)) return fail(FCSA_ERR_INVALID, "workspace not 16-byte aligned");
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+
+  // append pass: q_hat to the workspace (groups > 0), then k (normalised when groups > 0) and v into the caches at
+  // row cache_seqlens[b]
+  const int64_t H = p->heads, N = p->seq_q, D = p->head_dim;
+  const fcsa_tensor qhat = {workspace, H * N * D, N * D, D};
+  fcsa::RowArgs a = row_args(p->batch, p->head_dim, groups);
+  int n = 0;
+  if (groups > 0) a.t[n++] = {p->heads, p->seq_q, *q, qhat, {}, nullptr, nullptr, p->seq_q, 0};
+  if (n_new > 0) {
+    a.t[n++] = {p->kv_heads, n_new, *k_new, *k_cache, {}, nullptr, cache_seqlens, p->seq_k, groups == 0 ? 1 : 0};
+    a.t[n++] = {p->kv_heads, n_new, *v_new, *v_cache, {}, nullptr, cache_seqlens, p->seq_k, 1};
+  }
+  if (n > 0 && (r = row_pass_launched(fcsa::launch_row_append(a, n, p->dtype == FCSA_BF16, s), "append pass launch")))
+    return r;
+
+  const fcsa_tensor* qa = groups > 0 ? &qhat : q;
+  float* part = reinterpret_cast<float*>(static_cast<char*>(workspace) + qbytes);
+  if (p->dtype == FCSA_BF16) {
+    if (p->head_dim == 64) return launch_decode<__nv_bfloat16, 64>(p, sh, qa, k_cache, v_cache, cache_seqlens, n_new, o, part, s);
+    return launch_decode<__nv_bfloat16, 128>(p, sh, qa, k_cache, v_cache, cache_seqlens, n_new, o, part, s);
+  }
+  if (p->head_dim == 64) return launch_decode<__half, 64>(p, sh, qa, k_cache, v_cache, cache_seqlens, n_new, o, part, s);
+  return launch_decode<__half, 128>(p, sh, qa, k_cache, v_cache, cache_seqlens, n_new, o, part, s);
 }
 
 }  // extern "C"

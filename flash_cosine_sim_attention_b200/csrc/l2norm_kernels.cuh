@@ -29,13 +29,17 @@ struct RowTensor {
   fcsa_tensor y;                  // the 16-bit normalised tensor: output of forward, input of backward
   fcsa_tensor dx;                 // backward only: output, the type of dy (may be dy itself: in-place passes)
   float* rnorm;                   // (B, H, N, G) fp32; forward: nullptr = not kept
+  // read by the append pass only (row_fwd_kernel<..., APPEND = true>, the key/value-cache decode):
+  const int32_t* row0;            // device (B,): row n of x goes to row row0[b] + n of y; nullptr = row n
+  int rows_y;                     // rows of y: a destination row outside [0, rows_y) is not written
+  int raw;                        // 1: y = x, no l2norm whatever G (the values)
 };
 
 struct RowArgs {
   int B, D, G;                    // G = 0: plain scaled cast (float32 passes)
   const float* mul;               // device scalar or nullptr (= 1); read by the float32 passes only
   int mul_reciprocal;             // 1: use 1 / *mul
-  RowTensor t[2];                 // forward: one or two tensors (t[1].H = 0 for one); backward: t[0]
+  RowTensor t[3];                 // forward: one to three tensors (t[i].H = 0 ends the list); backward: t[0]
 };
 
 // 1 / max(sqrt(ss), 1e-12)  (py:38-55: F.normalize's eps) = min(rsqrt(ss), 1e12): one MUFU.RSQ instead of an
@@ -176,8 +180,9 @@ __device__ __forceinline__ float row_mul(const RowArgs& a) {
 // 32-bit: 2^31 rows of at least 64 bytes do not fit in device memory.  One thread owns 16 features of U rows and
 // issues its loads of all U rows before the first reduction; TPR = threads per row (D / 16) when known at compile
 // time (4 or 8), 0 = read it from the arguments.  x is read with coherent loads: it may alias y.  The 16-bit passes
-// keep four blocks per SM (at most 64 registers).
-template <typename T, typename X, int TPR, int U>
+// keep four blocks per SM (at most 64 registers).  APPEND (16-bit only): grid.y runs over up to three tensors, each
+// row lands at the per-batch offset row0[b] (rows falling outside y are skipped) and `raw` tensors are copied.
+template <typename T, typename X, int TPR, int U, bool APPEND = false>
 __global__ void __launch_bounds__(256, 8 / sizeof(X)) row_fwd_kernel(const RowArgs a) {
   // SIXTEEN features per thread: the pass is issue-bound before it is memory-bound (ncu: 84 % issue-slot
   // utilisation with 8 features per thread), so the per-row bookkeeping (addresses, shuffle steps, predicates) is
@@ -192,7 +197,7 @@ __global__ void __launch_bounds__(256, 8 / sizeof(X)) row_fwd_kernel(const RowAr
   const int rows = a.B * t.H * t.N;
   if (blockIdx.x * (U * rpp) >= rows) return;         // the grid is sized for the longer of the two tensors
   const int row0 = blockIdx.x * (U * rpp) + threadIdx.x / tpr;
-  const int gs = a.G ? a.D / a.G : 0;
+  const int gs = (a.G && !(APPEND && t.raw)) ? a.D / a.G : 0;
   const float mul = row_mul<X>(a);
   uint4 raw[U][16 / E];
   long long yoff[U];
@@ -201,7 +206,13 @@ __global__ void __launch_bounds__(256, 8 / sizeof(X)) row_fwd_kernel(const RowAr
     const int row = row0 + u * rpp;
     const int bh = row / t.N, n = row - bh * t.N, b = bh / t.H, h = bh - b * t.H;
     const X* xp = static_cast<const X*>(t.x.ptr) + b * t.x.sb + h * t.x.sh + (long long)n * t.x.sn + tr * 16;
-    yoff[u] = b * t.y.sb + h * t.y.sh + (long long)n * t.y.sn + tr * 16;
+    if constexpr (APPEND) {
+      long long ny = n;
+      if (t.row0 != nullptr && row < rows) ny += t.row0[b];
+      yoff[u] = (ny >= 0 && ny < t.rows_y) ? b * t.y.sb + h * t.y.sh + ny * t.y.sn + tr * 16 : -1;
+    } else {
+      yoff[u] = b * t.y.sb + h * t.y.sh + (long long)n * t.y.sn + tr * 16;
+    }
 #pragma unroll
     for (int v = 0; v < 16 / E; ++v) raw[u][v] = row < rows ? ld_stream128(xp + v * E) : make_uint4(0, 0, 0, 0);
   }
@@ -220,7 +231,7 @@ __global__ void __launch_bounds__(256, 8 / sizeof(X)) row_fwd_kernel(const RowAr
     }
 #pragma unroll
     for (int i = 0; i < 16; ++i) f[i] *= rn[i] * mul;
-    if (ok) {
+    if (ok && (!APPEND || yoff[u] >= 0)) {
 #pragma unroll
       for (int s = 0; s < 2; ++s)
         *reinterpret_cast<uint4*>(static_cast<T*>(t.y.ptr) + yoff[u] + 8 * s) = pack16B<T>(f + 8 * s);
@@ -290,6 +301,23 @@ inline cudaError_t launch_row_fwd(const RowArgs& a, bool bf16, bool f32_in, cuda
     return f32_in ? launch_row_fwd_t<__nv_bfloat16, float>(a, grid, stream)
                   : launch_row_fwd_t<__nv_bfloat16, __nv_bfloat16>(a, grid, stream);
   return f32_in ? launch_row_fwd_t<__half, float>(a, grid, stream) : launch_row_fwd_t<__half, __half>(a, grid, stream);
+}
+
+// the append pass of the key/value-cache decode over a.t[0 .. n): 16-bit x and y, head dim 64 or 128
+inline cudaError_t launch_row_append(const RowArgs& a, int n, bool bf16, cudaStream_t stream) {
+  constexpr int U = kRowFwdU;
+  const int rows_per_block = U * (256 / (a.D / 16));
+  long long rows = 0;
+  for (int i = 0; i < n; ++i) {
+    const long long r = (long long)a.B * a.t[i].H * a.t[i].N;
+    rows = r > rows ? r : rows;
+  }
+  const dim3 grid((unsigned)((rows + rows_per_block - 1) / rows_per_block), n);
+  if (bf16)
+    return a.D == 64 ? launch_pdl(row_fwd_kernel<__nv_bfloat16, __nv_bfloat16, 4, U, true>, grid, dim3(256), 0, stream, a)
+                     : launch_pdl(row_fwd_kernel<__nv_bfloat16, __nv_bfloat16, 8, U, true>, grid, dim3(256), 0, stream, a);
+  return a.D == 64 ? launch_pdl(row_fwd_kernel<__half, __half, 4, U, true>, grid, dim3(256), 0, stream, a)
+                   : launch_pdl(row_fwd_kernel<__half, __half, 8, U, true>, grid, dim3(256), 0, stream, a);
 }
 
 // backward over a.t[0]; dy and dx are float32 when f32_grad, else of y's type

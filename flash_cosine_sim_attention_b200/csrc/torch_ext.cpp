@@ -403,6 +403,81 @@ std::tuple<Tensor, Tensor, Tensor, optional<Tensor>> backward(
   return {std::get<0>(r), std::get<1>(r), std::get<2>(r), db};
 }
 
+// ------------------------------------------------------------------------------------------------
+// decode: new queries against a key/value cache, appending k / v at row cache_seqlens[b] (fcsa_decode).
+//   q (B, H, Nq, D); k_cache, v_cache (B, kv_heads, capacity, D), written in place, so they must be usable as they
+//   are (no copy); cache_seqlens int32 on q's device; k, v (B, kv_heads, n_new, D) or both None; groups > 0:
+//   l2-normalise q and k over that many groups.  Returns o (B, H, Nq, D).  Scratch comes from the per-(device,
+//   stream) workspace of the backward, whose contents are irrelevant on entry.
+// ------------------------------------------------------------------------------------------------
+Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
+              const optional<Tensor>& k_in, const optional<Tensor>& v_in, double scale, double shift, bool causal,
+              int64_t groups) {
+  TORCH_CHECK(q_in.dim() == 4 && k_cache.dim() == 4 && v_cache.dim() == 4,
+              "decode: q, k_cache, v_cache must be (batch, heads, seq, head_dim)");
+  TORCH_CHECK(q_in.is_cuda() && k_cache.is_cuda() && v_cache.is_cuda(), "decode: CUDA tensors required");
+  TORCH_CHECK(k_cache.scalar_type() == q_in.scalar_type() && v_cache.scalar_type() == q_in.scalar_type(),
+              "decode: q and the caches must share one dtype");
+  TORCH_CHECK(k_cache.sizes() == v_cache.sizes(), "decode: k_cache and v_cache must have the same shape");
+  const int64_t B = q_in.size(0), H = q_in.size(1), Nq = q_in.size(2), D = q_in.size(3);
+  const int64_t Hk = k_cache.size(1), cap = k_cache.size(2);
+  TORCH_CHECK(k_cache.size(0) == B && k_cache.size(3) == D, "decode: caches must be (", B, ", kv_heads, capacity, ", D,
+              ")");
+  TORCH_CHECK(Hk > 0 && H % Hk == 0, "decode: kv_heads (", Hk, ") must divide the query heads (", H, ")");
+  TORCH_CHECK(cache_seqlens.is_cuda() && cache_seqlens.get_device() == q_in.get_device() &&
+                  cache_seqlens.scalar_type() == at::kInt && cache_seqlens.dim() == 1 && cache_seqlens.size(0) == B,
+              "decode: cache_seqlens must be an int32 tensor of shape (", B, ") on q's device");
+  // the kernels index it as a dense array; a copy would also break graph capture (a replay must read the caller's
+  // buffer), so a strided or expanded view is refused
+  TORCH_CHECK(cache_seqlens.is_contiguous(), "decode: cache_seqlens must be contiguous (not a strided or expanded view)");
+  TORCH_CHECK(tma_ready(k_cache).data_ptr() == k_cache.data_ptr() && tma_ready(v_cache).data_ptr() == v_cache.data_ptr(),
+              "decode: the caches are written in place and must be usable as they are: contiguous head dim, "
+              "16-byte aligned base and strides, no expanded dimension");
+  const bool has_new = k_in.has_value() && k_in->defined();
+  TORCH_CHECK(has_new == (v_in.has_value() && v_in->defined()), "decode: pass both k and v, or neither");
+  int64_t n_new = 0;
+  Tensor k, v;
+  if (has_new) {
+    TORCH_CHECK(k_in->dim() == 4 && k_in->sizes() == v_in->sizes() && k_in->size(0) == B && k_in->size(1) == Hk &&
+                    k_in->size(3) == D,
+                "decode: k and v must be (", B, ", ", Hk, ", n_new, ", D, ")");
+    TORCH_CHECK(k_in->scalar_type() == q_in.scalar_type() && v_in->scalar_type() == q_in.scalar_type() &&
+                    k_in->is_cuda() && v_in->is_cuda(),
+                "decode: k and v must be CUDA tensors of q's dtype");
+    k = tma_ready(*k_in);
+    v = tma_ready(*v_in);
+    n_new = k.size(2);
+  }
+  const c10::cuda::CUDAGuard guard(q_in.device());
+  const Tensor q = tma_ready(q_in);
+  fcsa_problem p;
+  p.dtype = dtype_code(q);
+  p.batch = (int32_t)B; p.heads = (int32_t)H; p.kv_heads = (int32_t)Hk;
+  p.seq_q = (int32_t)Nq; p.seq_k = (int32_t)cap; p.head_dim = (int32_t)D;
+  p.causal = causal ? 1 : 0;
+  p.scale = (float)scale; p.shift = (float)shift;
+  p.key_mask = nullptr; p.key_mask_stride = 0;
+  p.out_f32 = 0; p.reserved_ = 0;
+  Tensor o = at::empty({B, H, Nq, D}, q.options());
+  cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
+  const size_t need = fcsa_decode_workspace_bytes(&p, (int32_t)n_new);
+  TORCH_CHECK(need > 0, "libfcsa_b200: ", fcsa_last_error());
+  Tensor scratch;
+  {
+    std::lock_guard<std::mutex> lock(g_ws_mutex);
+    Workspaces& w = g_ws[{(int)q.get_device(), (void*)stream}];
+    if (!w.scratch.defined() || (size_t)w.scratch.numel() < need)
+      w.scratch = at::empty({(int64_t)need}, q.options().dtype(at::kByte));
+    scratch = w.scratch;
+  }
+  const fcsa_tensor tq = view4(q), tkc = view4(k_cache), tvc = view4(v_cache), to = view4(o);
+  fcsa_tensor tk = {nullptr, 0, 0, 0}, tv = {nullptr, 0, 0, 0};
+  if (has_new) { tk = view4(k); tv = view4(v); }
+  FCSA_CHECK(fcsa_decode(&p, &tq, &tkc, &tvc, cache_seqlens.data_ptr<int32_t>(), &tk, &tv, (int32_t)n_new,
+                         (int32_t)groups, &to, scratch.data_ptr(), (size_t)scratch.numel(), stream));
+  return o;
+}
+
 // Drops the cached backward workspaces of every (device, stream) (they only ever grow: a long-context call leaves a
 // 1 GB accumulator behind).  Returns the number of bytes released to the caching allocator.  Safe at any time between
 // calls: buffers still referenced by enqueued kernels stay alive through the allocator's stream semantics.
@@ -439,6 +514,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("f32_cast_backward", &f32_cast_backward, "backward of f32_cast: float32 gradient w.r.t. the float32 input");
   m.def("l2norm_forward", &l2norm_forward, "grouped l2norm: x -> (y, 1/norm)");
   m.def("l2norm_backward", &l2norm_backward, "grouped l2norm backward from the normalised y");
+  m.def("decode", &decode, "new queries against a key/value cache, appending k / v at cache_seqlens");
   m.def("release_workspaces", &release_workspaces, "free the cached backward workspaces; returns the bytes released");
   m.def("abi_version", []() { return fcsa_version(); });
   m.def("_error_path_selftest", []() { FCSA_CHECK(fcsa_forward(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr)); },

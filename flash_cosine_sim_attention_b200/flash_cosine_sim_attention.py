@@ -5,6 +5,8 @@ flash_cosine_sim_attention/flash_cosine_sim_attention.py, kept name-for-name so 
     flash_cosine_sim_attention(q, k, v, mask, attn_bias, scale, groups, causal, l2norm_qk,
                                attn_bias_batch_dim)                     reference py:308-334
     l2norm_tensors(*tensors, groups)                                    reference py:57-65
+    flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens, k, v, ...)
+                                      decoding with a key/value cache (no reference counterpart)
     plain_cosine_sim_attention(...)   naive un-fused formulation        reference py:75-126
     FlashCosineSimAttention (autograd.Function) / forward / backward / debug   py:245-304, cu:1928-1933
 
@@ -28,6 +30,7 @@ from . import _abi
 
 __all__ = [
     "flash_cosine_sim_attention",
+    "flash_cosine_sim_attention_with_kv_cache",
     "plain_cosine_sim_attention",
     "l2norm_tensors",
     "FlashCosineSimAttention",
@@ -566,3 +569,79 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
     gs = q.shape[-1] // groups
     assert (gs & (gs - 1)) == 0, "groups must divide the head dim into power-of-two chunks"
     return _FusedCosineSimAttention.apply(q, k, v, mask, float(scale), bool(causal), int(groups), bool(l2norm_qk))
+
+
+def _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias):
+    """Everything flash_cosine_sim_attention_with_kv_cache rejects before touching a device."""
+    if exists(attn_bias):
+        raise NotImplementedError("flash_cosine_sim_attention_with_kv_cache: attn_bias is not supported")
+    if exists(mask):
+        raise NotImplementedError("flash_cosine_sim_attention_with_kv_cache: no key-padding mask - cache_seqlens "
+                                  "gives each batch element's valid cache rows")
+    if q.ndim != 4 or k_cache.ndim != 4 or v_cache.ndim != 4:
+        raise ValueError("flash_cosine_sim_attention_with_kv_cache: q must be (batch, heads, seq, head_dim) and the "
+                         "caches (batch, kv_heads, capacity, head_dim); merged batch-heads are not supported")
+    if exists(k) != exists(v):
+        raise ValueError("flash_cosine_sim_attention_with_kv_cache: pass both k and v, or neither")
+    if torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (q, k_cache, v_cache, k, v)):
+        raise RuntimeError("flash_cosine_sim_attention_with_kv_cache is inference-only (no autograd): call it under "
+                           "torch.no_grad() or with tensors that do not require grad")
+    if q.dtype == torch.float32:
+        raise TypeError("flash_cosine_sim_attention_with_kv_cache: float32 is not supported - use float16 or "
+                        "bfloat16 (run the model in 16-bit or under autocast)")
+    if q.dtype not in _KERNEL_DTYPES:
+        raise TypeError(f"flash_cosine_sim_attention_with_kv_cache: dtype {q.dtype} is not supported")
+    if any(t is not None and t.dtype != q.dtype for t in (k_cache, v_cache, k, v)):
+        raise TypeError("flash_cosine_sim_attention_with_kv_cache: q, the caches, k and v must share one dtype")
+    D = q.shape[-1]
+    if D not in _KERNEL_HEAD_DIMS:
+        raise NotImplementedError(f"flash_cosine_sim_attention_with_kv_cache: head_dim {D} (64 and 128 only)")
+    if k_cache.shape != v_cache.shape or k_cache.shape[0] != q.shape[0] or k_cache.shape[-1] != D:
+        raise ValueError(f"flash_cosine_sim_attention_with_kv_cache: caches of shape {tuple(k_cache.shape)} and "
+                         f"{tuple(v_cache.shape)} do not match q {tuple(q.shape)}")
+    hk = k_cache.shape[1]
+    if hk <= 0 or q.shape[1] % hk != 0:
+        raise ValueError(f"flash_cosine_sim_attention_with_kv_cache: kv_heads ({hk}) must divide the query heads "
+                         f"({q.shape[1]})")
+    if exists(k) and (k.shape != v.shape or k.ndim != 4 or k.shape[:2] != k_cache.shape[:2] or k.shape[-1] != D):
+        raise ValueError(f"flash_cosine_sim_attention_with_kv_cache: k and v must be (batch, kv_heads, n_new, {D}) "
+                         f"like the caches (got {tuple(k.shape)} and {tuple(v.shape)})")
+    if not torch.is_tensor(cache_seqlens) or cache_seqlens.dtype != torch.int32 or cache_seqlens.shape != (q.shape[0],):
+        raise TypeError("flash_cosine_sim_attention_with_kv_cache: cache_seqlens must be an int32 tensor of shape "
+                        f"({q.shape[0]},)")
+    if not cache_seqlens.is_contiguous():
+        raise ValueError("flash_cosine_sim_attention_with_kv_cache: cache_seqlens must be contiguous (the kernels read "
+                         "it as a dense array and a CUDA graph replay reads the caller's buffer; not a strided or "
+                         "expanded view)")
+    gs = D // groups if groups > 0 and D % groups == 0 else 0
+    if gs == 0 or (gs & (gs - 1)) != 0:
+        raise ValueError(f"flash_cosine_sim_attention_with_kv_cache: groups {groups} must divide head_dim {D} into "
+                         "power-of-two chunks")
+    if not (q.is_cuda and cache_seqlens.is_cuda):
+        raise RuntimeError("flash_cosine_sim_attention_with_kv_cache: CUDA tensors required (cache_seqlens included: "
+                           "the host never reads it) - this build has no CPU path")
+
+
+def flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens, k=None, v=None, scale=8, groups=1,
+                                             causal=True, l2norm_qk=True, mask=None, attn_bias=None):
+    """Cosine-sim attention of new queries against a key/value cache, for inference (generation).
+
+    q: (batch, heads, n_q, head_dim) new queries.  k_cache, v_cache: (batch, kv_heads, capacity, head_dim), kv_heads
+    dividing heads (query head h reads kv head h // (heads // kv_heads)).  cache_seqlens: int32 CUDA tensor (batch,)
+    of valid cache rows L_b; it is never read on the host, so a call does not synchronise and can be captured in a
+    CUDA graph.  k, v: optional (batch, kv_heads, n_new, head_dim), written into the caches at rows
+    [L_b, L_b + n_new) by this call.  cache_seqlens is NOT advanced: the caller adds n_new afterwards.
+
+    The cache holds keys in the form the kernel reads them: with l2norm_qk=True the appended rows are
+    l2norm(k, groups) rounded to the cache dtype (so the prefix is never renormalised), with l2norm_qk=False k as
+    given.  v is stored as given.  With T_b = L_b + n_new, new query i sees key j iff j < T_b and, with causal=True,
+    j <= i + T_b - n_q (the bottom-right rule of flash_cosine_sim_attention with n_k = T_b); rows that see no key
+    give 0.  scale, groups and the exponent shift are those of flash_cosine_sim_attention.
+
+    L_b + n_new must not exceed the capacity: rows that do not fit are not written, and T_b is clamped to the
+    capacity.  float16 / bfloat16 and head dims 64 and 128 only; no autograd, attn_bias, mask, float32 or merged
+    batch-heads.  Returns o (batch, heads, n_q, head_dim)."""
+    _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias)
+    shift = _choose_shift(q.dtype, scale, groups, l2norm_qk)
+    return _ext().decode(q, k_cache, v_cache, cache_seqlens, k, v, float(scale), float(shift), bool(causal),
+                         int(groups) if l2norm_qk else 0)

@@ -15,7 +15,8 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from .flash_cosine_sim_attention import flash_cosine_sim_attention, plain_cosine_sim_attention
+from .flash_cosine_sim_attention import (flash_cosine_sim_attention, flash_cosine_sim_attention_with_kv_cache,
+                                         plain_cosine_sim_attention)
 
 
 def _softmax_attention(q, k, v, **unused):
@@ -46,6 +47,20 @@ def FeedForward(dim, mult=4, pre_norm=False):
     )
 
 
+class KVCache:
+    """Keys and values of one attention layer, for decoding token after token (`forward(x, cache=...)`).
+
+    `k`, `v`: (batch, kv_heads, capacity, dim_head), allocated at the first call in the dtype of the keys.  With the
+    CUDA kernel they hold what flash_cosine_sim_attention_with_kv_cache stores (l2-normalised keys); with the plain
+    attention the raw keys.  `seqlens`: the valid rows per batch element on the device (int32), `length`: the same
+    count on the host (the batch elements advance together here)."""
+
+    def __init__(self, capacity):
+        self.capacity = capacity
+        self.k = self.v = self.seqlens = None
+        self.length = 0
+
+
 class Attention(nn.Module):
     def __init__(self, dim, dim_head=64, heads=8, scale=8, l2norm_groups=1, pre_norm=False,
                  use_cuda_kernel=False, non_cosine_sim_attn=False, groups=None, kv_heads=None, **kwargs):
@@ -60,6 +75,9 @@ class Attention(nn.Module):
         self.heads = heads
         self.kv_heads = kv_heads
         self.l2norm_groups = groups if groups is not None else l2norm_groups
+        self.use_cuda_kernel = use_cuda_kernel and not non_cosine_sim_attn
+        self.non_cosine_sim_attn = non_cosine_sim_attn
+        self.kernel_kwargs = kwargs         # extra keywords of flash_cosine_sim_attention (CUDA kernel only)
         if non_cosine_sim_attn:
             g = heads // kv_heads
             self.attn_fn = (_softmax_attention if g == 1 else
@@ -74,7 +92,7 @@ class Attention(nn.Module):
         self.to_v = nn.Linear(dim, dim_head * kv_heads, bias=False)
         self.to_out = nn.Linear(inner, dim, bias=False)
 
-    def forward(self, x):
+    def forward(self, x, cache=None):
         b, n, _ = x.shape
         x = self.norm(x)
         # (b, n, h*d) -> (b, h, n, d) views: strided, feature dim contiguous - the fused op reads
@@ -82,8 +100,44 @@ class Attention(nn.Module):
         split = lambda t, h: t.view(b, n, h, -1).transpose(1, 2)
         q = split(self.to_q(x), self.heads)
         k, v = split(self.to_k(x), self.kv_heads), split(self.to_v(x), self.kv_heads)
-        o = self.attn_fn(q, k, v, causal=True, scale=self.scale, groups=self.l2norm_groups)
+        if cache is None:
+            o = self.attn_fn(q, k, v, causal=True, scale=self.scale, groups=self.l2norm_groups)
+        else:
+            o = self._attend_cached(q, k, v, cache)
         return self.to_out(o.transpose(1, 2).reshape(b, n, -1))
+
+    def _attend_cached(self, q, k, v, cache):
+        """q, k, v of the next n tokens against the cached prefix; appends k, v to the cache."""
+        if self.non_cosine_sim_attn:
+            raise NotImplementedError("the key/value cache is implemented for cosine-sim attention only")
+        b, _, n, d = k.shape
+        L = cache.length
+        if L + n > cache.capacity:
+            raise ValueError(f"key/value cache full: {L} + {n} tokens exceed its capacity {cache.capacity}")
+        # the uncached CUDA path hands these keywords to flash_cosine_sim_attention; with a cache only l2norm_qk has a
+        # meaning, and a silently dropped one would make cached and uncached outputs differ
+        unsupported = sorted(set(self.kernel_kwargs) - {"l2norm_qk"}) if self.use_cuda_kernel else []
+        if unsupported:
+            raise NotImplementedError(f"the key/value cache does not support the attention keywords {unsupported}")
+        if self.use_cuda_kernel and k.dtype == torch.float32:
+            raise RuntimeError("the key/value cache with the CUDA kernel needs 16-bit activations: run the model in "
+                               "16-bit or under autocast")
+        if cache.k is None:
+            cache.k = torch.zeros(b, self.kv_heads, cache.capacity, d, dtype=k.dtype, device=k.device)
+            cache.v = torch.zeros_like(cache.k)
+            cache.seqlens = torch.zeros(b, dtype=torch.int32, device=k.device)
+        if self.use_cuda_kernel:
+            o = flash_cosine_sim_attention_with_kv_cache(q, cache.k, cache.v, cache.seqlens, k, v, scale=self.scale,
+                                                         groups=self.l2norm_groups, causal=True,
+                                                         l2norm_qk=self.kernel_kwargs.get("l2norm_qk", True))
+        else:
+            cache.k[:, :, L:L + n] = k
+            cache.v[:, :, L:L + n] = v
+            o = plain_cosine_sim_attention(q, cache.k[:, :, :L + n], cache.v[:, :, :L + n], causal=True,
+                                           scale=self.scale, groups=self.l2norm_groups)
+        cache.seqlens += n
+        cache.length += n
+        return o
 
 
 class CosineSimCausalTransformer(nn.Module):
@@ -124,25 +178,47 @@ class CosineSimCausalTransformer(nn.Module):
                 nn.init.xavier_normal_(lin.weight.data, gain=g)
         nn.init.xavier_normal_(self.to_logits[-1].weight.data, gain=1.0)
 
+    def new_cache(self):
+        """One empty KVCache per layer, holding up to max_seq_len tokens, for forward(x, cache=...)."""
+        return [KVCache(self.max_seq_len) for _ in self.layers]
+
     @torch.no_grad()
-    def generate(self, start_tokens, seq_len, temperature=1.0, filter_thres=0.9, **kwargs):
+    def generate(self, start_tokens, seq_len, temperature=1.0, filter_thres=0.9, kv_cache=False, **kwargs):
+        """kv_cache=True: one forward over the prompt, then one token per step against the cached keys / values.
+        Once the sequence is longer than max_seq_len, the window slides and its positions are re-encoded from 0, so
+        from then on each step re-fills a fresh cache with the window - the same computation as without the cache."""
         was_training = self.training
         self.eval()
         n0 = start_tokens.shape[1]
         out = start_tokens
+        cache = None
         for _ in range(seq_len):
-            logits = self.forward(out[:, -self.max_seq_len:], **kwargs)[:, -1, :]
+            if not kv_cache:
+                logits = self.forward(out[:, -self.max_seq_len:], **kwargs)[:, -1, :]
+            elif cache is None or out.shape[1] > self.max_seq_len:
+                cache = self.new_cache()
+                logits = self.forward(out[:, -self.max_seq_len:], cache=cache, **kwargs)[:, -1, :]
+            else:
+                logits = self.forward(out[:, -1:], cache=cache, **kwargs)[:, -1, :]
             probs = F.softmax(_keep_top_fraction(logits, filter_thres) / temperature, dim=-1)
             out = torch.cat((out, torch.multinomial(probs, 1)), dim=-1)
         self.train(was_training)
         return out[:, n0:]
 
-    def forward(self, x, return_loss=False):
+    def forward(self, x, return_loss=False, cache=None):
+        """cache: the list new_cache() returned - x are then the next tokens after the cached ones, and their
+        positions start at the cache's length."""
         if return_loss:
             x, labels = x[:, :-1], x[:, 1:]
-        x = self.token_emb(x) + self.pos_emb(torch.arange(x.shape[1], device=x.device))
-        for attn, attn_norm, ff, ff_norm in self.layers:
-            x = attn_norm(attn(x) + x * self.residual_scale)
+        start = 0 if cache is None else cache[0].length
+        if start + x.shape[1] > self.max_seq_len:
+            if cache is None:
+                raise ValueError(f"{x.shape[1]} tokens exceed max_seq_len {self.max_seq_len}")
+            raise ValueError(f"key/value cache full: {start} + {x.shape[1]} tokens exceed its capacity "
+                             f"{self.max_seq_len} (max_seq_len)")
+        x = self.token_emb(x) + self.pos_emb(torch.arange(start, start + x.shape[1], device=x.device))
+        for i, (attn, attn_norm, ff, ff_norm) in enumerate(self.layers):
+            x = attn_norm(attn(x, cache=None if cache is None else cache[i]) + x * self.residual_scale)
             x = ff_norm(ff(x) + x * self.residual_scale)
         logits = self.to_logits(x)
         if not return_loss:

@@ -246,6 +246,31 @@ int fcsa_backward_bias(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_t
  */
 int fcsa_set_kernel_events(int32_t which, void* start_event, void* stop_event);
 
+/* ---- key/value-cache decode (no reference counterpart: the reference has no inference path) ----------------------
+ * Attends seq_q >= 1 new queries per (batch, head) to a key/value cache and appends new keys / values to it, in at
+ * most three launches (append pass, attention, combine of the key splits) that never synchronise: a decode step can
+ * be captured in a CUDA graph.
+ *   p              : seq_q = new queries, seq_k = the cache CAPACITY, kv_heads as in fcsa_problem; no key_mask,
+ *                    out_f32 = 0.  scale / shift / causal as in fcsa_forward.
+ *   q, o           : (batch, heads, seq_q, head_dim)
+ *   k_cache,v_cache: (batch, kv_heads, capacity, head_dim), any TMA-legal strides; written in place
+ *   cache_seqlens  : DEVICE int32 (batch,): valid cache rows L_b before the call; never read by the host, never
+ *                    changed (the caller advances it by n_new afterwards)
+ *   k_new, v_new   : (batch, kv_heads, n_new, head_dim), appended at cache rows [L_b, L_b + n_new); ignored when
+ *                    n_new == 0
+ *   groups         : > 0: q and k_new are l2-normalised over `groups` chunks of the head dim (as fcsa_forward_fused)
+ *                    and the cache stores normalised keys rounded to the dtype; 0: q and k_new are used as given
+ * Visible length T_b = min(L_b + n_new, capacity).  Query i sees key j iff j < T_b and, causal, j <= i + T_b - seq_q
+ * (fcsa_forward's bottom-right rule with seq_k = T_b); rows with no visible key give o = 0.  Nothing is written
+ * outside the cache: appended rows at or past the capacity are dropped (L_b + n_new > capacity is a caller error).
+ * o is bitwise reproducible from run to run.  `workspace`: fcsa_decode_workspace_bytes(p, n_new) bytes of scratch,
+ * contents irrelevant on entry.
+ */
+size_t fcsa_decode_workspace_bytes(const fcsa_problem* p, int32_t n_new);
+int fcsa_decode(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k_cache, const fcsa_tensor* v_cache,
+                const int32_t* cache_seqlens, const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t n_new,
+                int32_t groups, const fcsa_tensor* o, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
