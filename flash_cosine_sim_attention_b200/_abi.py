@@ -42,6 +42,10 @@ EXPORTED_SYMBOLS = (
     "fcsa_f32_cast_backward",
     "fcsa_decode_workspace_bytes",
     "fcsa_decode",
+    "fcsa_forward_fused_varlen",
+    "fcsa_backward_fused_varlen_workspace_bytes",
+    "fcsa_backward_fused_varlen_zeroed_bytes",
+    "fcsa_backward_fused_varlen",
 )
 
 
@@ -75,6 +79,10 @@ class FcsaL2Norm(Structure):
 
 class FcsaBias(Structure):
     _fields_ = [("ptr", c_void_p), ("sb", c_int64), ("sh", c_int64), ("sn", c_int64), ("amax", c_void_p)]
+
+
+class FcsaVarlen(Structure):
+    _fields_ = [("cu_seqlens_q", c_void_p), ("cu_seqlens_k", c_void_p), ("total_q", c_int32), ("total_k", c_int32)]
 
 
 class FcsaError(RuntimeError):
@@ -140,6 +148,16 @@ def load():
     lib.fcsa_decode_workspace_bytes.argtypes = [PP, c_int32]
     lib.fcsa_decode.restype = c_int32
     lib.fcsa_decode.argtypes = [PP, PT, PT, PT, c_void_p, PT, PT, c_int32, c_int32, PT, c_void_p, c_size_t, c_void_p]
+    PV = POINTER(FcsaVarlen)
+    lib.fcsa_forward_fused_varlen.restype = c_int32
+    lib.fcsa_forward_fused_varlen.argtypes = [PP, PV, PT, PT, PT, PN, PT, c_void_p, c_void_p]
+    lib.fcsa_backward_fused_varlen_workspace_bytes.restype = c_size_t
+    lib.fcsa_backward_fused_varlen_workspace_bytes.argtypes = [PP, PV]
+    lib.fcsa_backward_fused_varlen_zeroed_bytes.restype = c_size_t
+    lib.fcsa_backward_fused_varlen_zeroed_bytes.argtypes = [PP, PV]
+    lib.fcsa_backward_fused_varlen.restype = c_int32
+    lib.fcsa_backward_fused_varlen.argtypes = [PP, PV, PN, PT, PT, PT, c_void_p, PT, PT, PT, c_void_p, c_size_t,
+                                               c_void_p, c_size_t, c_void_p]
     lib.fcsa_set_kernel_events.restype = c_int32
     lib.fcsa_set_kernel_events.argtypes = [c_int32, c_void_p, c_void_p]
     _lib = lib

@@ -111,6 +111,29 @@ inline BwdWorkspace bwd_workspace_layout(int B, int H, int kv_heads, int Nq, int
   return w;
 }
 
+// Packed sequences: the stats and the dq accumulator hold, per query head, `ntile` tiles of QT rows.  Sequence b starts
+// at tile base(b) = start_b / QT + b (start_b = its first query row), which needs no prefix sum on the device and leaves
+// room for ceil(len_b / QT) tiles before base(b + 1); every tile index stays below total_q / QT + B + 1.  dkv_acc is
+// [kv_heads][total_k][D] (dk, then dv).
+inline int varlen_tiles(int B, long long total_q) { return (int)(total_q / 64 + B + 1); }
+
+inline BwdWorkspace bwd_varlen_workspace_layout(int B, int H, int kv_heads, long long total_q, long long total_k,
+                                                int D) {
+  BwdWorkspace w;
+  w.QT = 64;
+  w.nqt = varlen_tiles(B, total_q);
+  size_t stats = (size_t)H * w.nqt * 2 * w.QT * 4;
+  size_t dq = (size_t)H * w.nqt * w.QT * D * 4;
+  size_t dkv = kv_heads < H ? (size_t)2 * kv_heads * total_k * D * 4 : 0;
+  auto up = [](size_t x) { return (x + 255) & ~size_t(255); };
+  w.stats_off = 0;
+  w.dkv_off = up(stats);
+  w.total = w.dkv_off + up(dkv);
+  w.dq_off = 0;
+  w.ztotal = up(dq);
+  return w;
+}
+
 inline size_t bwd_workspace_bytes(int B, int H, int kv_heads, int Nq, int Nk, int D) {
   return bwd_workspace_layout(B, H, kv_heads, Nq, Nk, D).total;
 }
@@ -133,6 +156,14 @@ struct PrepArgs {
   float* stats;
 };
 
+// Packed sequences: B sequences, Nq = the maximum length and nqt = ceil(Nq / QT) (the grid); o, d_o are
+// (total_q, H, D) (o_sb, do_sb unused), inv_l is (H, total_q) and the stats of head h, sequence b start at tile
+// h * ntile + base(b) (bwd_varlen_workspace_layout).
+struct PrepVarlenArgs : PrepArgs {
+  const int* cu_q;
+  int total_q, ntile;
+};
+
 __device__ __forceinline__ float lg2_approx(float x) {
   float y;
   asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -140,8 +171,8 @@ __device__ __forceinline__ float lg2_approx(float x) {
 }
 
 // TPR = threads per row = D / 8 (8 or 16); QT = 64.
-template <typename T, int TPR>
-__global__ void __launch_bounds__(256) bwd_prep_kernel(const PrepArgs a) {
+template <typename T, int TPR, bool VARLEN = false>
+__global__ void __launch_bounds__(256) bwd_prep_kernel(const std::conditional_t<VARLEN, PrepVarlenArgs, PrepArgs> a) {
   // 1-D grid = batch*heads x (row blocks of the padded sequence); TPR threads per row, two rows per
   // thread (four 16-byte loads in flight), shuffle reduce.  The pass must stay memory-bound: no
   // runtime-divisor divisions, MUFU log2.
@@ -153,12 +184,21 @@ __global__ void __launch_bounds__(256) bwd_prep_kernel(const PrepArgs a) {
   const int blk = blockIdx.x - bh * a.bpb;
   const int b = bh / a.H, h = bh - b * a.H;
   const int tr = threadIdx.x % TPR;
-  const int padded = a.nqt * QT;
+  int padded = a.nqt * QT, Nq = a.Nq;
+  long long tile0 = (long long)bh * a.nqt, row_off = 0;     // the stats tile of query row 0, o / d_o rows before it
+  if constexpr (VARLEN) {
+    // the sequence's rows, then zeros up to its last tile's end
+    const SeqSpan sq = seq_span(a.cu_q, b, a.Nq, a.total_q);
+    Nq = sq.len;
+    padded = (Nq + QT - 1) / QT * QT;
+    tile0 = (long long)h * a.ntile + sq.start / QT + b;
+    row_off = sq.start;
+  }
   const float c2 = a.c2 + (a.shift_extra != nullptr ? fmaxf(__ldg(a.shift_extra), 0.f) * 1.4426950408889634f : 0.f);
-  const long long o_off = b * a.o_sb + h * a.o_sh + tr * 8;
+  const long long o_off = (VARLEN ? 0 : b * a.o_sb) + h * a.o_sh + row_off * a.o_sn + tr * 8;
   const T* obase = reinterpret_cast<const T*>(a.o) + o_off;
   const float* obase32 = reinterpret_cast<const float*>(a.o) + o_off;
-  const T* dbase = reinterpret_cast<const T*>(a.d_o) + b * a.do_sb + h * a.do_sh + tr * 8;
+  const T* dbase = reinterpret_cast<const T*>(a.d_o) + (VARLEN ? 0 : b * a.do_sb) + h * a.do_sh + row_off * a.do_sn + tr * 8;
   int row[2];
   bool in[2], valid[2];
   uint4 ro[2], rd[2];
@@ -168,7 +208,7 @@ __global__ void __launch_bounds__(256) bwd_prep_kernel(const PrepArgs a) {
   for (int u = 0; u < 2; ++u) {
     row[u] = (blk * 2 + u) * RPB + threadIdx.x / TPR;     // row inside the padded (nqt*QT) range
     in[u] = row[u] < padded;
-    valid[u] = in[u] && row[u] < a.Nq;
+    valid[u] = in[u] && row[u] < Nq;
     ro[u] = rd[u] = make_uint4(0, 0, 0, 0);
     rof[u][0] = rof[u][1] = make_float4(0.f, 0.f, 0.f, 0.f);
     il[u] = 1.f;
@@ -180,7 +220,10 @@ __global__ void __launch_bounds__(256) bwd_prep_kernel(const PrepArgs a) {
         ro[u] = ldg_stream128(obase + (long long)row[u] * a.o_sn);
       }
       rd[u] = ldg_stream128(dbase + (long long)row[u] * a.do_sn);
-      if (tr == 0) il[u] = __ldg(a.inv_l + (long long)bh * a.Nq + row[u]);
+      if (tr == 0) {
+        if constexpr (VARLEN) il[u] = __ldg(a.inv_l + (long long)h * a.total_q + row_off + row[u]);
+        else il[u] = __ldg(a.inv_l + (long long)bh * a.Nq + row[u]);
+      }
     }
   }
 #pragma unroll
@@ -200,7 +243,7 @@ __global__ void __launch_bounds__(256) bwd_prep_kernel(const PrepArgs a) {
     const float ndl = valid[u] ? -dot : 0.f;      // stored negated: the dS stage computes P * (dP + (-delta))
     if (!in[u] || tr != 0) continue;
     const int qt = row[u] >> QSH, r = row[u] & (QT - 1);
-    float* st = a.stats + ((long long)bh * a.nqt + qt) * 2 * QT;
+    float* st = a.stats + (tile0 + qt) * 2 * QT;
     st[r] = c3;
     st[QT + r] = ndl;
   }
@@ -235,6 +278,17 @@ struct BwdArgs {
   int groups;
 };
 
+// Packed sequences (VARLEN instantiations): B sequences, Nq / Nk = the maximum lengths (nqt unused).  q, d_o are
+// (total_q, H, D), k, v, dk, dv (total_k, kv_heads, D), addressed at batch 0 of their maps (dk_sb, dv_sb unused);
+// sequence b owns query rows [cu_q[b], cu_q[b + 1]) and key rows [cu_k[b], cu_k[b + 1]).  The stats and the dq
+// accumulator of head h, sequence b start at tile h * ntile + base(b) (bwd_varlen_workspace_layout); dk_acc / dv_acc
+// and k_rnorm are [kv_heads][total_k][.].
+struct BwdVarlenArgs : BwdArgs {
+  const int* cu_q;
+  const int* cu_k;
+  int total_q, total_k, ntile;
+};
+
 // 16-bit global load through the read-only path (bias elements along the query axis are strided)
 __device__ __forceinline__ uint32_t ldg_u16(const void* p) {
   uint16_t v;
@@ -262,7 +316,7 @@ __device__ __forceinline__ float4 ldg_cg128f(const float* p) {
 // other three lanes of its quad.  k_hat comes from the resident K tile (row address sk_row, 128B swizzle, 64-feature
 // chunks 16 KB apart).  All lanes of the warp must call it (quad shuffles); `in` = the key exists.
 template <typename T, int D>
-__device__ __forceinline__ void l2norm_bwd_key_row(float (&g)[D / 4], const BwdArgs& a, uint32_t sk_row, int b, int hk,
+__device__ __forceinline__ void l2norm_bwd_key_row(float (&g)[D / 4], const BwdArgs& a, uint32_t sk_row, long long krow0,
                                                    int key, bool in) {
   const int lane = threadIdx.x & 31;
   const int r8 = (lane >> 2) & 7, cq = 2 * (lane & 3);
@@ -305,7 +359,7 @@ __device__ __forceinline__ void l2norm_bwd_key_row(float (&g)[D / 4], const BwdA
     for (int jb = 0; jb < D / 8; ++jb) dot[2 * jb] = dot[2 * jb + 1] = q[jb];
   }
   const int lg = __ffs(gs) - 1;
-  const float* rn = a.k_rnorm + (((long long)b * a.kv_heads + hk) * a.Nk + (in ? key : 0)) * a.groups;
+  const float* rn = a.k_rnorm + (krow0 + (in ? key : 0)) * a.groups;     // k_rnorm row krow0 + key
   // one load per feature pair (a pair shares its group unless gs = 1); the pairs of one group hit the same L1 line
 #pragma unroll
   for (int jb = 0; jb < D / 8; ++jb) {
@@ -319,13 +373,16 @@ __device__ __forceinline__ void l2norm_bwd_key_row(float (&g)[D / 4], const BwdA
 
 // HEAD_LOOP: the CTA works through several query heads (hpc > 1, grouped-query launches); otherwise hpc = 1 is a
 // compile-time constant and the loops below are those of one query head (MHA, MQA, BIAS and split groups of one head).
-template <typename T, int D, bool BIAS = false, bool HEAD_LOOP = false>
+// VARLEN: packed sequences (BwdVarlenArgs); `b` is then the sequence, and its lengths replace Nq / Nk.
+template <typename T, int D, bool BIAS = false, bool HEAD_LOOP = false, bool VARLEN = false>
 __global__ void __launch_bounds__(384, 1)
 fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                 const __grid_constant__ CUtensorMap tm_v, const __grid_constant__ CUtensorMap tm_do,
-                const __grid_constant__ CUtensorMap tm_dq, const BwdArgs a) {
+                const __grid_constant__ CUtensorMap tm_dq,
+                const std::conditional_t<VARLEN, BwdVarlenArgs, BwdArgs> a) {
   static_assert(D == 64 || D == 128, "head dim 64 or 128");
   static_assert(!(BIAS && HEAD_LOOP), "BIAS launches have one query head per CTA");
+  static_assert(!(BIAS && VARLEN), "packed sequences take no bias");
   using Cfg = BwdCfg<D>;
   constexpr bool STAGED = Cfg::kStaged;
   constexpr int QT = Cfg::QT;              // query rows per tile
@@ -368,15 +425,10 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int hpc = HEAD_LOOP ? a.hpc : 1;
   const int h0 = sl * hpc;                    // = hk * G + (slice within the group) * hpc
   const int key0 = jt * 128;
-  const int off = a.Nk - a.Nq;
-  int i_lo = 0;
-  if (a.causal) {
-    // first query tile with a row that can see key0: QT*i + QT-1 + off >= key0
-    const int x = key0 - off - (QT - 1);
-    i_lo = x <= 0 ? 0 : (x + QT - 1) / QT;
-  }
-  const int NI = max(0, a.nqt - i_lo);        // number of query tiles to visit per query head
-  const int NT = hpc * NI;                    // flat tile index i: head h0 + i / NI, query tile i_lo + i % NI
+  // packed sequences: the tensor maps' batch coordinate is 0, the sequence starts at query row q_row0 and key row
+  // k_row0, and its stats / dq accumulator at tile qbase of each head; the lengths are read after pdl_wait
+  const int tb = VARLEN ? 0 : b;
+  int Nq = a.Nq, Nk = a.Nk, nqt = a.nqt, q_row0 = 0, k_row0 = 0, qbase = 0;
 
   if (threadIdx.x == 0) {
     mbar_init(BAR(KV_FULL), 1);
@@ -396,6 +448,22 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   }
   __syncthreads();
   pdl_wait();          // stats come from the preprocess kernel; the dq accumulator is zero on entry
+  if constexpr (VARLEN) {
+    const SeqSpan sq = seq_span(a.cu_q, b, a.Nq, a.total_q), sk = seq_span(a.cu_k, b, a.Nk, a.total_k);
+    Nq = sq.len; Nk = sk.len; q_row0 = sq.start; k_row0 = sk.start;
+    nqt = (Nq + QT - 1) / QT;
+    qbase = q_row0 / QT + b;
+    if (key0 >= Nk) return;                   // a key tile past the end of its sequence
+  }
+  const int off = Nk - Nq;
+  int i_lo = 0;
+  if (a.causal) {
+    // first query tile with a row that can see key0: QT*i + QT-1 + off >= key0
+    const int x = key0 - off - (QT - 1);
+    i_lo = x <= 0 ? 0 : (x + QT - 1) / QT;
+  }
+  const int NI = max(0, nqt - i_lo);          // number of query tiles to visit per query head
+  const int NT = hpc * NI;                    // flat tile index i: head h0 + i / NI, query tile i_lo + i % NI
 
   if (wg == 0) {
     // =============================== TMA producer ===============================
@@ -408,19 +476,21 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       mbar_expect_tx(BAR(KV_FULL), 2 * Cfg::kKV);
 #pragma unroll
       for (int ch = 0; ch < KCH; ++ch) {
-        tma_load_4d(sK + ch * 16384, &tm_k, BAR(KV_FULL), ch * 64, key0, hk, b);
-        tma_load_4d(sV + ch * 16384, &tm_v, BAR(KV_FULL), ch * 64, key0, hk, b);
+        tma_load_4d(sK + ch * 16384, &tm_k, BAR(KV_FULL), ch * 64, k_row0 + key0, hk, tb);
+        tma_load_4d(sV + ch * 16384, &tm_v, BAR(KV_FULL), ch * 64, k_row0 + key0, hk, tb);
       }
       for (int i = 0, h = h0; h < h0 + hpc; ++h) {
-        const float* stats_h = a.stats + ((long long)b * a.H + h) * a.nqt * 2 * QT;
-        for (int qt = i_lo; qt < a.nqt; ++qt, ++i) {
+        long long tile0 = ((long long)b * a.H + h) * a.nqt;     // the stats tile of query tile 0
+        if constexpr (VARLEN) tile0 = (long long)h * a.ntile + qbase;
+        const float* stats_h = a.stats + tile0 * 2 * QT;
+        for (int qt = i_lo; qt < nqt; ++qt, ++i) {
           const int st = i % NST;
           mbar_wait(BAR(EMPTY + st), ((i / NST) & 1) ^ 1);
           mbar_expect_tx(BAR(FULL + st), 2 * Cfg::kQ + 8 * QT);
 #pragma unroll
           for (int ch = 0; ch < KCH; ++ch) {
-            tma_load_4d(sQ + st * Cfg::kQ + ch * QCHUNK, &tm_q, BAR(FULL + st), ch * 64, qt * QT, h, b);
-            tma_load_4d(sDO + st * Cfg::kQ + ch * QCHUNK, &tm_do, BAR(FULL + st), ch * 64, qt * QT, h, b);
+            tma_load_4d(sQ + st * Cfg::kQ + ch * QCHUNK, &tm_q, BAR(FULL + st), ch * 64, q_row0 + qt * QT, h, tb);
+            tma_load_4d(sDO + st * Cfg::kQ + ch * QCHUNK, &tm_do, BAR(FULL + st), ch * 64, q_row0 + qt * QT, h, tb);
           }
           bulk_load_1d(sStats + st * 8 * QT, stats_h + (long long)qt * 2 * QT, 8 * QT, BAR(FULL + st));
         }
@@ -428,7 +498,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     } else if (STAGED && (warp == 1 || warp == 2) && elect_one()) {
       // dQ reducer of consumer warpgroup warp - 1, which owns the query tiles i = warp - 1 (mod 2): each staged
       // 64 x D fp32 tile is added into the accumulator by TMA (rows at or beyond Nq lie outside the tensor map
-      // and are not written)
+      // and are not written; with packed sequences the rows of a tail tile past the sequence's end are inside it,
+      // and the dq finish kernel clears them)
       const int rw = warp - 1;
       if (rw == 0) tma_prefetch_desc(&tm_dq);
       for (int i = rw; i < NT; i += 2) {
@@ -437,7 +508,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         const uint32_t src = sDQ + (NDQ * rw + sb) * Cfg::kDQ;
         mbar_wait(BAR(DQ_FULL + NDQ * rw + sb), (n / NDQ) & 1);
 #pragma unroll
-        for (int c = 0; c < D / 32; ++c) tma_reduce_add_4d(&tm_dq, src + c * (QT * 128), c * 32, qt * QT, h0 + hh, b);
+        for (int c = 0; c < D / 32; ++c)
+          tma_reduce_add_4d(&tm_dq, src + c * (QT * 128), c * 32, (qbase + qt) * QT, h0 + hh, tb);
         bulk_commit();
         bulk_wait_read<0>();
         mbar_arrive(BAR(DQ_EMPTY + NDQ * rw + sb));
@@ -460,13 +532,13 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     key_g[hf] = key0 + 64 * w + kr + 8 * hf;
-    bool ok = key_g[hf] < a.Nk;
+    bool ok = key_g[hf] < Nk;
     if (a.has_mask && ok) ok = a.mask[(long long)b * a.mask_sb + key_g[hf]] != 0;
-    key_lo[hf] = !ok ? a.Nq + QT : (a.causal ? key_g[hf] - off : 0);
+    key_lo[hf] = !ok ? Nq + QT : (a.causal ? key_g[hf] - off : 0);
   }
   // the warpgroup's keys are all real and unmasked: only query tiles crossing the causal diagonal or the end
   // of the sequence need per-element selects
-  const bool keys_full = !a.has_mask && key0 + 64 * w + 64 <= a.Nk;
+  const bool keys_full = !a.has_mask && key0 + 64 * w + 64 <= Nk;
   const uint32_t sKw = sK + w * 64 * 128, sVw = sV + w * 64 * 128;    // the warpgroup's 64 rows of every chunk
   const uint32_t ds_thr = kr * 128 + cq * 2;  // the thread's dS^T words: + 1024 hf + 16 (column block ^ r8)
   const float c1 = a.c1;
@@ -496,7 +568,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
                          uint32_t (&pf)[QT / 4], uint32_t (&dsf)[QT / 4], int row0, uint32_t stc3, uint32_t dsbuf) {
     int hi = QT - 1, lo[2] = {0, 0};
     if (MASKED) {
-      hi = min(QT - 1, a.Nq - 1 - row0);                      // last valid query column of the tile
+      hi = min(QT - 1, Nq - 1 - row0);                        // last valid query column of the tile
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {                        // first visible query column of each key row
         lo[hf] = max(0, key_lo[hf] - row0);
@@ -552,7 +624,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   auto elementwise_tile = [&](const float (&s)[QT / 2], const float (&dp)[QT / 2], uint32_t (&pf)[QT / 4],
                               uint32_t (&dsf)[QT / 4], int row0, uint32_t stc3, uint32_t dsbuf) {
     // interior tile: every key of the warpgroup sees every query row (no causal diagonal, no ragged end)
-    const bool interior = keys_full && row0 + QT <= a.Nq && (!a.causal || key0 + 64 * w + 63 - off <= row0);
+    const bool interior = keys_full && row0 + QT <= Nq && (!a.causal || key0 + 64 * w + 63 - off <= row0);
     if (!BIAS && interior) elementwise(false, s, dp, pf, dsf, row0, stc3, dsbuf);
     else elementwise(true, s, dp, pf, dsf, row0, stc3, dsbuf);
     fence_proxy_async_smem();
@@ -596,6 +668,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   float dv[D / 2], dk[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) dv[i] = dk[i] = 0.f;
+  // (packed sequences: a head's last tile ends at ceil(Nq / QT) * QT, so row0 + QT < Nq says whether row0 is before it)
   // the producer loads K and V whatever NI; the epilogue reads K (l2norm backward) even when no query tile is visited
   mbar_wait(BAR(KV_FULL), 0);
 
@@ -655,7 +728,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       mbar_wait(BAR(FULL), 0);
       issue_s_dp(s, dp, sQ, sDO);
       // i runs over the flat (head, query tile) sequence; row0 restarts at i_lo * QT with every head
-      for (int i = 0, row0 = i_lo * QT; i < NT; ++i, row0 = (!HEAD_LOOP || row0 + QT < a.nqt * QT) ? row0 + QT : i_lo * QT) {
+      for (int i = 0, row0 = i_lo * QT; i < NT; ++i, row0 = (!HEAD_LOOP || row0 + QT < (VARLEN ? Nq : a.nqt * QT)) ? row0 + QT : i_lo * QT) {
         const int st = i % NST;
         const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
         wgmma_wait<0>();                        // S^T, dP^T of tile i; dV, dK of tile i - 1; dQ of tile i - 2
@@ -731,11 +804,13 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       mbar_arrive(BAR(EMPTY + st));             // Q, dO and the stats of this stage are no longer read
 
       // ---- dQ partial tile -> fp32 accumulator (rows = queries, columns = features) ----
-      float* acc = a.dq_acc + (((long long)b * a.H + h0 + hh) * a.nqt * QT + row0) * D + cq;
+      long long tile0 = ((long long)b * a.H + h0 + hh) * a.nqt;     // the accumulator tile of query tile 0
+      if constexpr (VARLEN) tile0 = (long long)(h0 + hh) * a.ntile + qbase;
+      float* acc = a.dq_acc + (tile0 * QT + row0) * D + cq;
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {
         const int q = 16 * wl + r8 + 8 * hf;
-        if (row0 + q < a.Nq) {
+        if (row0 + q < Nq) {
 #pragma unroll
           for (int jb = 0; jb < D / 8; ++jb)
             red_add_f32x2(acc + (long long)q * D + 8 * jb, dq[4 * jb + 2 * hf], dq[4 * jb + 2 * hf + 1]);
@@ -747,14 +822,22 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   // ---- epilogue: dV and dK * scale of the warpgroup's 64 keys ---------------------------------
   // (no early exit for keys at or beyond Nk: the l2norm backward below shuffles within the quad of a key row)
   const bool to_acc = a.split > 1;
+  long long krow0 = ((long long)b * a.kv_heads + hk) * a.Nk;     // the row of key 0 in k_rnorm and dk_acc / dv_acc
+  if constexpr (VARLEN) {
+    // the key span is read again rather than kept in registers through the main loop
+    const SeqSpan sk = seq_span(a.cu_k, b, a.Nk, a.total_k);
+    Nk = sk.len;
+    k_row0 = sk.start;
+    krow0 = (long long)hk * a.total_k + k_row0;
+  }
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     const int key = key_g[hf];
-    const bool in = key < a.Nk;
+    const bool in = key < Nk;
     if (to_acc) {
       // the group's heads are split over several CTAs: sum over them in fp32 (reference: cu:1613-1619)
-      float* pv = a.dv_acc + (((long long)b * a.kv_heads + hk) * a.Nk + key) * D + cq;
-      float* pk = a.dk_acc + (((long long)b * a.kv_heads + hk) * a.Nk + key) * D + cq;
+      float* pv = a.dv_acc + (krow0 + key) * D + cq;
+      float* pk = a.dk_acc + (krow0 + key) * D + cq;
       if (in) {
 #pragma unroll
         for (int jb = 0; jb < D / 8; ++jb) {
@@ -762,7 +845,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           red_add_f32x2(pk + 8 * jb, dk[4 * jb + 2 * hf] * a.scale, dk[4 * jb + 2 * hf + 1] * a.scale);
         }
       }
-    } else if (a.out_f32) {
+    } else if (!VARLEN && a.out_f32) {
       float* pv = reinterpret_cast<float*>(a.dv) + b * a.dv_sb + hk * a.dv_sh + (long long)key * a.dv_sn + cq;
       float* pk = reinterpret_cast<float*>(a.dk) + b * a.dk_sb + hk * a.dk_sh + (long long)key * a.dk_sn + cq;
       if (in) {
@@ -774,8 +857,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         }
       }
     } else {
-      T* pv = reinterpret_cast<T*>(a.dv) + b * a.dv_sb + hk * a.dv_sh + (long long)key * a.dv_sn + cq;
-      T* pk = reinterpret_cast<T*>(a.dk) + b * a.dk_sb + hk * a.dk_sh + (long long)key * a.dk_sn + cq;
+      T* pv = reinterpret_cast<T*>(a.dv) + tb * a.dv_sb + hk * a.dv_sh + (long long)(k_row0 + key) * a.dv_sn + cq;
+      T* pk = reinterpret_cast<T*>(a.dk) + tb * a.dk_sb + hk * a.dk_sh + (long long)(k_row0 + key) * a.dk_sn + cq;
       if (in) {
 #pragma unroll
         for (int jb = 0; jb < D / 8; ++jb)
@@ -788,7 +871,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         g[2 * jb] = dk[4 * jb + 2 * hf] * a.scale;
         g[2 * jb + 1] = dk[4 * jb + 2 * hf + 1] * a.scale;
       }
-      if (a.k_rnorm != nullptr) l2norm_bwd_key_row<T, D>(g, a, sK + (64 * w + kr + 8 * hf) * 128, b, hk, key, in);
+      if (a.k_rnorm != nullptr) l2norm_bwd_key_row<T, D>(g, a, sK + (64 * w + kr + 8 * hf) * 128, krow0, key, in);
       if (in) {
 #pragma unroll
         for (int jb = 0; jb < D / 8; ++jb)
@@ -813,15 +896,60 @@ struct DqFinishArgs {
   int G;
 };
 
+// Packed sequences: B sequences, Nq = the maximum length, padded = ceil(Nq / QT) * QT (the grid covers that many rows
+// of every (sequence, head)); dq, q_hat are (total_q, H, D) (sb, q_sb unused), q_rnorm is (H, total_q, G) and the
+// accumulator of head h, sequence b starts at tile h * ntile + base(b).
+struct DqFinishVarlenArgs : DqFinishArgs {
+  const int* cu_q;
+  int total_q, ntile;
+};
+
 // dq conversion (reference: the fp32 -> scalar_t cast of dq after its atomics, cu:1904): TPR = D / 8 consecutive lanes
 // per query row, 8 features each.  The accumulator is read from L2 (the reductions of the main kernel have just
 // produced it there), converted, and written back as zeros: it is zero between launches.
-template <typename T, int D>
-__global__ void __launch_bounds__(256) bwd_dq_finish_kernel(const DqFinishArgs a) {
+// VARLEN: every row of a sequence's tiles is cleared, the padding rows past its end included.  Those lie inside the
+// accumulator's tensor map and receive dS K for masked queries: exact zeros for finite K, NaN when the neighbouring rows
+// the tail tile reads hold non-finite values - cleared here, so the zeroed workspace stays zero for every later call.
+template <typename T, int D, bool VARLEN = false>
+__global__ void __launch_bounds__(256)
+bwd_dq_finish_kernel(const std::conditional_t<VARLEN, DqFinishVarlenArgs, DqFinishArgs> a) {
   pdl_launch_dependents();
   pdl_wait();
   constexpr int TPR = D / 8;
   const long long t = (long long)blockIdx.x * 256 + threadIdx.x;
+  if constexpr (VARLEN) {
+    constexpr int QT = 64;
+    const long long rowid = t / TPR;                       // over (sequences*heads) x padded
+    const int c8 = (int)(t % TPR);
+    const bool in_grid = rowid < (long long)a.B * a.H * a.padded;
+    const long long bh = in_grid ? rowid / a.padded : 0;
+    const int r = (int)(rowid - bh * a.padded);
+    const int b = (int)(bh / a.H), h = (int)(bh % a.H);
+    const SeqSpan sq = seq_span(a.cu_q, b, a.Nq, a.total_q);
+    const bool own = in_grid && r < (sq.len + QT - 1) / QT * QT;    // a row of the sequence's tiles
+    const bool ok = in_grid && r < sq.len;                          // ... and of the sequence (whole rows of lanes)
+    float* src = a.dq_acc + (((long long)h * a.ntile + sq.start / QT + b) * QT + r) * D + c8 * 8;
+    const long long row = (long long)sq.start + r;                  // the packed row
+    float4 lo = make_float4(0.f, 0.f, 0.f, 0.f), hi = lo;
+    if (own) {
+      lo = ldg_cg128f(src);
+      hi = ldg_cg128f(src + 4);
+      *reinterpret_cast<float4*>(src) = make_float4(0.f, 0.f, 0.f, 0.f);
+      *reinterpret_cast<float4*>(src + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    float g[8] = {lo.x * a.scale, lo.y * a.scale, lo.z * a.scale, lo.w * a.scale,
+                  hi.x * a.scale, hi.y * a.scale, hi.z * a.scale, hi.w * a.scale};
+    if (a.q_rnorm != nullptr) {
+      float y[8];
+      unpack16B<T>(ok ? ldg_stream128(reinterpret_cast<const T*>(a.q_hat) + h * a.q_sh + row * a.q_sn + c8 * 8)
+                      : make_uint4(0, 0, 0, 0), y);
+      l2norm_bwd_group<8>(g, y, D / a.G, c8, ok ? a.q_rnorm + ((long long)h * a.total_q + row) * a.G : nullptr, 1.f);
+    }
+    if (!ok) return;
+    T* dst = reinterpret_cast<T*>(a.dq) + h * a.sh + row * a.sn + c8 * 8;
+    *reinterpret_cast<uint4*>(dst) = pack16B<T>(g);
+    return;
+  }
   const long long rowid = t / TPR;                         // over (batch*heads) x Nq
   const int c8 = (int)(t % TPR);
   const bool ok = rowid < (long long)a.B * a.H * a.Nq;     // whole rows of TPR lanes (shuffles stay in them)
@@ -916,6 +1044,11 @@ struct BwdHostArgs {
   const void* bias = nullptr; long long bias_sb = 0, bias_sh = 0, bias_sn = 0;
   const float* bias_amax = nullptr;           // optional device scalar added (if positive) to the shift
   float* dbias = nullptr; long long dbias_sb = 0, dbias_sh = 0;
+  // packed sequences (run_backward_varlen): B sequences, Nq / Nk the maximum lengths, q, d_o, o, dq (total_q, H, D)
+  // and k, v, dk, dv (total_k, kv_heads, D) with sb unused, inv_l (H, total_q), the rnorms [heads][total][groups]
+  const int* cu_q = nullptr;
+  const int* cu_k = nullptr;
+  int total_q = 0, total_k = 0;
 };
 
 // Slices per key/value-head group (query heads per CTA = G / split).  One CTA per group keeps dk / dv in registers
@@ -933,11 +1066,15 @@ inline int bwd_group_split(int B, int H, int kv_heads, int Nk, bool bias, int sm
   return G;
 }
 
-template <typename T, int D, bool BIAS = false>
+template <typename T, int D, bool BIAS = false, bool VARLEN = false>
 int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, const char** err,
                    cudaError_t* ce) {
   using Cfg = BwdCfg<D>;
-  const BwdWorkspace w = bwd_workspace_layout(h.B, h.H, h.kv_heads, h.Nq, h.Nk, D);
+  const BwdWorkspace w = VARLEN ? bwd_varlen_workspace_layout(h.B, h.H, h.kv_heads, h.total_q, h.total_k, D)
+                                : bwd_workspace_layout(h.B, h.H, h.kv_heads, h.Nq, h.Nk, D);
+  // the batch, key rows and query tiles of the tensors as addressed: packed sequences are one batch of total rows
+  const int tB = VARLEN ? 1 : h.B, tNq = VARLEN ? h.total_q : h.Nq, tNk = VARLEN ? h.total_k : h.Nk;
+  const int nqt = (h.Nq + Cfg::QT - 1) / Cfg::QT;     // query tiles of the longest sequence
   uint8_t* ws = reinterpret_cast<uint8_t*>(h.workspace);
   uint8_t* zs = reinterpret_cast<uint8_t*>(h.zeroed);
   float* stats = reinterpret_cast<float*>(ws + w.stats_off);
@@ -953,7 +1090,7 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
     split = bwd_group_split(h.B, h.H, h.kv_heads, h.Nk, BIAS, sms);
   }
   const bool to_acc = split > 1;
-  const size_t dkv_elems = (size_t)h.B * h.kv_heads * h.Nk * D;
+  const size_t dkv_elems = (size_t)tB * h.kv_heads * tNk * D;
 
   // dk/dv accumulators of split groups are per call (the dq accumulator is self-cleaning)
   if (to_acc) {
@@ -963,8 +1100,9 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
 
   // 1. preprocess
   {
-    PrepArgs pa;
-    pa.B = h.B; pa.H = h.H; pa.Nq = h.Nq; pa.Nk = h.Nk; pa.D = D; pa.nqt = w.nqt; pa.QT = Cfg::QT; pa.causal = h.causal;
+    std::conditional_t<VARLEN, PrepVarlenArgs, PrepArgs> pa;
+    pa.B = h.B; pa.H = h.H; pa.Nq = h.Nq; pa.Nk = h.Nk; pa.D = D; pa.nqt = nqt; pa.QT = Cfg::QT; pa.causal = h.causal;
+    if constexpr (VARLEN) { pa.cu_q = h.cu_q; pa.total_q = h.total_q; pa.ntile = w.nqt; }
     pa.c2 = h.shift * log2e;
     pa.shift_extra = h.bias_amax;
     pa.o_f32 = h.out_f32 ? 1 : 0;
@@ -972,12 +1110,12 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
     pa.d_o = h.d_o.ptr; pa.do_sb = h.d_o.sb; pa.do_sh = h.d_o.sh; pa.do_sn = h.d_o.sn;
     pa.inv_l = h.inv_l; pa.stats = stats;
     const int rows_per_block = 2 * (256 / (D / 8));
-    const int padded = w.nqt * Cfg::QT;
+    const int padded = nqt * Cfg::QT;
     pa.bpb = (padded + rows_per_block - 1) / rows_per_block;
     const long long grid = (long long)pa.bpb * h.B * h.H;
     if (grid > 0x7FFFFFFFLL) { *err = "problem too large for one launch"; return FCSA_ERR_INVALID; }
     if (h.ev_prep[0]) cudaEventRecord(h.ev_prep[0], stream);
-    e = launch_pdl(bwd_prep_kernel<T, D / 8>, dim3((unsigned)grid), dim3(256), 0, stream, pa);
+    e = launch_pdl(bwd_prep_kernel<T, D / 8, VARLEN>, dim3((unsigned)grid), dim3(256), 0, stream, pa);
     if (h.ev_prep[1]) cudaEventRecord(h.ev_prep[1], stream);
     if (e != cudaSuccess) { *err = "backward preprocess launch"; *ce = e; return FCSA_ERR_CUDA; }
     ++*launches;
@@ -986,26 +1124,30 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
   {
     CUtensorMap tq, tk, tv, tdo, tdq;
     const CUtensorMapDataType dt = tma_dtype16(h.dtype_bf16);
-    if (make_tensor_map_bhnd(&tq, h.q.ptr, dt, h.B, h.H, h.Nq, D, h.q.sb, h.q.sh, h.q.sn, Cfg::QT) ||
-        make_tensor_map_bhnd(&tk, h.k.ptr, dt, h.B, h.kv_heads, h.Nk, D, h.k.sb, h.k.sh, h.k.sn, 128) ||
-        make_tensor_map_bhnd(&tv, h.v.ptr, dt, h.B, h.kv_heads, h.Nk, D, h.v.sb, h.v.sh, h.v.sn, 128) ||
-        make_tensor_map_bhnd(&tdo, h.d_o.ptr, dt, h.B, h.H, h.Nq, D, h.d_o.sb, h.d_o.sh, h.d_o.sn, Cfg::QT)) {
+    if (make_tensor_map_bhnd(&tq, h.q.ptr, dt, tB, h.H, tNq, D, h.q.sb, h.q.sh, h.q.sn, Cfg::QT) ||
+        make_tensor_map_bhnd(&tk, h.k.ptr, dt, tB, h.kv_heads, tNk, D, h.k.sb, h.k.sh, h.k.sn, 128) ||
+        make_tensor_map_bhnd(&tv, h.v.ptr, dt, tB, h.kv_heads, tNk, D, h.v.sb, h.v.sh, h.v.sn, 128) ||
+        make_tensor_map_bhnd(&tdo, h.d_o.ptr, dt, tB, h.H, tNq, D, h.d_o.sb, h.d_o.sh, h.d_o.sn, Cfg::QT)) {
       *err = "cuTensorMapEncodeTiled failed (backward): q, k, v, d_o must be views a TMA tensor map can express "
              "(positive strides, 16-byte aligned)";
       return FCSA_ERR_INVALID;
     }
-    // the dq accumulator as [B][H][Nq][D] fp32 over its padded rows: boxes of 32 features x QT rows
+    // the dq accumulator as [B][H][Nq][D] fp32 over its padded rows: boxes of 32 features x QT rows (packed
+    // sequences: [1][H][ntile * QT][D], every tile inside the map)
     memset(&tdq, 0, sizeof(tdq));
     const long long acc_sh = (long long)w.nqt * Cfg::QT * D;
     if (Cfg::kStaged &&
-        make_tensor_map_bhnd(&tdq, dq_acc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, h.B, h.H, h.Nq, D, h.H * acc_sh, acc_sh, D,
-                             Cfg::QT, 32)) {
+        make_tensor_map_bhnd(&tdq, dq_acc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, tB, h.H, VARLEN ? w.nqt * Cfg::QT : h.Nq, D,
+                             h.H * acc_sh, acc_sh, D, Cfg::QT, 32)) {
       *err = "cuTensorMapEncodeTiled failed (backward dq accumulator)";
       return FCSA_ERR_CUDA;
     }
-    BwdArgs a;
+    std::conditional_t<VARLEN, BwdVarlenArgs, BwdArgs> a;
     a.B = h.B; a.H = h.H; a.Nq = h.Nq; a.Nk = h.Nk; a.kv_heads = h.kv_heads; a.causal = h.causal;
     a.has_mask = h.mask ? 1 : 0; a.nqt = w.nqt;
+    if constexpr (VARLEN) {
+      a.cu_q = h.cu_q; a.cu_k = h.cu_k; a.total_q = h.total_q; a.total_k = h.total_k; a.ntile = w.nqt;
+    }
     a.split = split; a.hpc = h.H / h.kv_heads / split;
     a.c1 = h.scale * log2e; a.scale = h.scale;
     a.mask = h.mask; a.mask_sb = h.mask_sb;
@@ -1018,11 +1160,11 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
     a.out_f32 = h.out_f32 ? 1 : 0;
     a.k_rnorm = h.k_rnorm; a.groups = h.groups;
     constexpr bool kLoop = !BIAS;
-    auto kern = a.hpc > 1 ? fcsa_bwd_kernel<T, D, BIAS, kLoop> : fcsa_bwd_kernel<T, D, BIAS>;
-    e = a.hpc > 1 ? ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS, kLoop>>(Cfg::kSmem)
-                  : ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS>>(Cfg::kSmem);
+    auto kern = a.hpc > 1 ? fcsa_bwd_kernel<T, D, BIAS, kLoop, VARLEN> : fcsa_bwd_kernel<T, D, BIAS, false, VARLEN>;
+    e = a.hpc > 1 ? ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS, kLoop, VARLEN>>(Cfg::kSmem)
+                  : ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS, false, VARLEN>>(Cfg::kSmem);
     if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(bwd)"; *ce = e; return FCSA_ERR_CUDA; }
-    // one CTA per (key tile, batch, kv head, slice of its group)
+    // one CTA per (key tile, batch, kv head, slice of its group); packed sequences: key tiles of the longest one
     const long long items = (long long)((h.Nk + 127) / 128) * h.B * h.kv_heads * split;
     if (items > 0x7FFFFFFFLL) { *err = "problem too large for one launch"; return FCSA_ERR_INVALID; }
     if (h.ev_start) cudaEventRecord(h.ev_start, stream);
@@ -1033,23 +1175,24 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
   }
   // 3. finish
   {
-    DqFinishArgs fa;
+    std::conditional_t<VARLEN, DqFinishVarlenArgs, DqFinishArgs> fa;
     fa.B = h.B; fa.H = h.H; fa.Nq = h.Nq; fa.D = D; fa.nqt = w.nqt; fa.padded = w.nqt * Cfg::QT; fa.scale = h.scale;
+    if constexpr (VARLEN) { fa.padded = nqt * Cfg::QT; fa.cu_q = h.cu_q; fa.total_q = h.total_q; fa.ntile = w.nqt; }
     fa.dq_acc = dq_acc; fa.dq = h.dq.ptr; fa.sb = h.dq.sb; fa.sh = h.dq.sh; fa.sn = h.dq.sn;
     fa.q_hat = h.q.ptr; fa.q_sb = h.q.sb; fa.q_sh = h.q.sh; fa.q_sn = h.q.sn;
     fa.q_rnorm = h.q_rnorm; fa.G = h.groups; fa.out_f32 = h.out_f32 ? 1 : 0;
-    const long long threads = (long long)h.B * h.H * h.Nq * (D / 8);
+    const long long threads = (long long)h.B * h.H * (VARLEN ? fa.padded : h.Nq) * (D / 8);
     const long long blocks = (threads + 255) / 256;
     if (blocks > 0x7FFFFFFFLL) { *err = "problem too large for one launch"; return FCSA_ERR_INVALID; }
     if (h.ev_finish[0]) cudaEventRecord(h.ev_finish[0], stream);
-    e = launch_pdl(bwd_dq_finish_kernel<T, D>, dim3((unsigned)blocks), dim3(256), 0, stream, fa);
+    e = launch_pdl(bwd_dq_finish_kernel<T, D, VARLEN>, dim3((unsigned)blocks), dim3(256), 0, stream, fa);
     if (h.ev_finish[1]) cudaEventRecord(h.ev_finish[1], stream);
     if (e != cudaSuccess) { *err = "dq finish launch"; *ce = e; return FCSA_ERR_CUDA; }
     ++*launches;
     if (to_acc) {
       for (int which = 0; which < 2; ++which) {
         KvFinishArgs ka;
-        ka.B = h.B; ka.Hk = h.kv_heads; ka.Nk = h.Nk; ka.D = D; ka.out_f32 = h.out_f32 ? 1 : 0;
+        ka.B = tB; ka.Hk = h.kv_heads; ka.Nk = tNk; ka.D = D; ka.out_f32 = h.out_f32 ? 1 : 0;
         ka.acc = dkv_acc + (which ? dkv_elems : 0);
         const fcsa_tensor& t = which ? h.dv : h.dk;
         ka.out = t.ptr; ka.sb = t.sb; ka.sh = t.sh; ka.sn = t.sn;
@@ -1064,14 +1207,25 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
       // l2norm backward of dk (gradient w.r.t. the raw keys) as its own pass over the head-summed dk; otherwise
       // the main kernel's epilogue applies it
       RowArgs la = {};
-      la.B = h.B; la.D = D; la.G = h.groups;
-      la.t[0] = {h.kv_heads, h.Nk, h.dk, h.k, h.dk, const_cast<float*>(h.k_rnorm)};
+      la.B = tB; la.D = D; la.G = h.groups;
+      la.t[0] = {h.kv_heads, tNk, h.dk, h.k, h.dk, const_cast<float*>(h.k_rnorm)};
       e = launch_row_bwd(la, h.dtype_bf16, false, stream);
       if (e != cudaSuccess) { *err = "l2norm backward (dk) launch"; *ce = e; return FCSA_ERR_CUDA; }
       ++*launches;
     }
   }
   return FCSA_OK;
+}
+
+// packed sequences (h.cu_q, h.cu_k set); no bias, no mask, 16-bit outputs
+inline int run_backward_varlen(const BwdHostArgs& h, cudaStream_t stream, int* launches, const char** err,
+                               cudaError_t* ce) {
+  if (h.D == 64) {
+    if (h.dtype_bf16) return run_backward_t<__nv_bfloat16, 64, false, true>(h, stream, launches, err, ce);
+    return run_backward_t<__half, 64, false, true>(h, stream, launches, err, ce);
+  }
+  if (h.dtype_bf16) return run_backward_t<__nv_bfloat16, 128, false, true>(h, stream, launches, err, ce);
+  return run_backward_t<__half, 128, false, true>(h, stream, launches, err, ce);
 }
 
 inline int run_backward(const BwdHostArgs& h, cudaStream_t stream, int* launches, const char** err,

@@ -79,25 +79,30 @@ int check_bias(const fcsa_problem* p, const fcsa_bias* bias) {
   return FCSA_OK;
 }
 
-template <typename T, int D, bool BIAS = false>
+// VARLEN: packed sequences (vl); q, k, v, o are then one batch of total_q / total_k rows
+template <typename T, int D, bool BIAS = false, bool VARLEN = false>
 int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
                    const fcsa_tensor* v, const fcsa_tensor* o, float* inv_l, cudaStream_t stream,
-                   const fcsa_bias* bias = nullptr) {
+                   const fcsa_bias* bias = nullptr, const fcsa_varlen* vl = nullptr) {
   using Cfg = fcsa::FwdCfg<D>;
   const bool bf = p->dtype == FCSA_BF16;
+  const int tB = VARLEN ? 1 : p->batch, tNq = VARLEN ? vl->total_q : p->seq_q, tNk = VARLEN ? vl->total_k : p->seq_k;
   CUtensorMap tq, tk, tv;
   int r;
-  if ((r = fcsa::make_tensor_map_bhnd(&tq, q->ptr, fcsa::tma_dtype16(bf), p->batch, p->heads, p->seq_q, D, q->sb, q->sh,
+  if ((r = fcsa::make_tensor_map_bhnd(&tq, q->ptr, fcsa::tma_dtype16(bf), tB, p->heads, tNq, D, q->sb, q->sh,
                                       q->sn, 128)))
     return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "q: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - make the tensor contiguous" : "cuTensorMapEncodeTiled failed", r);
-  if ((r = fcsa::make_tensor_map_bhnd(&tk, k->ptr, fcsa::tma_dtype16(bf), p->batch, p->kv_heads, p->seq_k, D, k->sb,
+  if ((r = fcsa::make_tensor_map_bhnd(&tk, k->ptr, fcsa::tma_dtype16(bf), tB, p->kv_heads, tNk, D, k->sb,
                                       k->sh, k->sn, 128)))
     return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "k: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - make the tensor contiguous" : "cuTensorMapEncodeTiled failed", r);
-  if ((r = fcsa::make_tensor_map_bhnd(&tv, v->ptr, fcsa::tma_dtype16(bf), p->batch, p->kv_heads, p->seq_k, D, v->sb,
+  if ((r = fcsa::make_tensor_map_bhnd(&tv, v->ptr, fcsa::tma_dtype16(bf), tB, p->kv_heads, tNk, D, v->sb,
                                       v->sh, v->sn, 128)))
     return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "v: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - make the tensor contiguous" : "cuTensorMapEncodeTiled failed", r);
 
-  fcsa::FwdArgs a;
+  std::conditional_t<VARLEN, fcsa::FwdVarlenArgs, fcsa::FwdArgs> a;
+  if constexpr (VARLEN) {
+    a.cu_q = vl->cu_seqlens_q; a.cu_k = vl->cu_seqlens_k; a.total_q = vl->total_q; a.total_k = vl->total_k;
+  }
   a.B = p->batch;
   a.H = p->heads;
   a.Nq = p->seq_q;
@@ -123,12 +128,12 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
   a.bias_sn = BIAS ? bias->sn : 0;
   a.bias_amax = BIAS ? bias->amax : nullptr;
 
-  auto kern = fcsa::fcsa_fwd_kernel<T, D, BIAS>;
+  auto kern = fcsa::fcsa_fwd_kernel<T, D, BIAS, VARLEN>;
   {
-    cudaError_t e = fcsa::ensure_dynamic_smem<fcsa::fcsa_fwd_kernel<T, D, BIAS>>(Cfg::kSmem);
+    cudaError_t e = fcsa::ensure_dynamic_smem<fcsa::fcsa_fwd_kernel<T, D, BIAS, VARLEN>>(Cfg::kSmem);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(fwd)");
   }
-  // one CTA per (query block of 128 rows, batch, head)
+  // one CTA per (query block of 128 rows, batch, head); packed sequences: blocks of the longest sequence
   const long long grid = (long long)a.n_qblk * p->batch * p->heads;
   if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
   if (g_ev[0][0]) cudaEventRecord(g_ev[0][0], stream);
@@ -251,6 +256,43 @@ int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tenso
   if (e != cudaSuccess) return cuda_fail(e, "decode combine launch");
   g_launches.fetch_add(1);
   return FCSA_OK;
+}
+
+// ---- packed sequences ----------------------------------------------------------------------------
+// The problem of a varlen call: batch = sequences, seq_q / seq_k = the maximum lengths; no key mask, 16-bit outputs.
+int check_varlen(const fcsa_problem* p, const fcsa_varlen* vl) {
+  int r;
+  if ((r = check_problem(p))) return r;
+  if (p->key_mask) return fail(FCSA_ERR_UNSUPPORTED, "varlen: no key mask (cu_seqlens give the valid rows)");
+  if (p->out_f32) return fail(FCSA_ERR_UNSUPPORTED, "varlen: out_f32 is not implemented");
+  if (!vl) return fail(FCSA_ERR_INVALID, "varlen: null fcsa_varlen");
+  if (!vl->cu_seqlens_q || !vl->cu_seqlens_k) return fail(FCSA_ERR_INVALID, "varlen: null cu_seqlens");
+  if ((reinterpret_cast<uintptr_t>(vl->cu_seqlens_q) & 3) || (reinterpret_cast<uintptr_t>(vl->cu_seqlens_k) & 3))
+    return fail(FCSA_ERR_INVALID, "varlen: cu_seqlens must be 4-byte aligned int32 arrays");
+  if (vl->total_q <= 0 || vl->total_k <= 0)
+    return fail(FCSA_ERR_INVALID, "varlen: empty packed tensors (total_q %d total_k %d)", vl->total_q, vl->total_k);
+  if ((long long)vl->total_q / 64 + p->batch + 1 > 0x7FFFFFFFLL / 64)
+    return fail(FCSA_ERR_INVALID, "varlen: too many query rows and sequences for one call");
+  return FCSA_OK;
+}
+
+// Zero the rows of up to three packed outputs that belong to no sequence (fcsa::varlen_tail_kernel), after the
+// attention kernels on the same stream.  t[i].cu / total say which cumulative lengths each tensor follows.
+int launch_varlen_tail(const fcsa_problem* p, fcsa::TailArgs a, int n, cudaStream_t stream) {
+  a.B = p->batch;
+  a.D = p->head_dim;
+  long long vecs = 0;
+  for (int i = 0; i < n; ++i) vecs = std::max(vecs, (long long)a.t[i].total * a.t[i].H * (p->head_dim / 8));
+  // a grid-stride loop: a few waves of blocks at most, whatever the tail's length
+  const unsigned blocks = (unsigned)std::max(1LL, std::min((vecs + 255) / 256, 1024LL));
+  const cudaError_t e = fcsa::launch_pdl(fcsa::varlen_tail_kernel, dim3(blocks, n), dim3(256), 0, stream, a);
+  if (e != cudaSuccess) return cuda_fail(e, "varlen tail launch");
+  g_launches.fetch_add(1);
+  return FCSA_OK;
+}
+
+fcsa::BwdWorkspace varlen_layout(const fcsa_problem* p, const fcsa_varlen* vl) {
+  return fcsa::bwd_varlen_workspace_layout(p->batch, p->heads, p->kv_heads, vl->total_q, vl->total_k, p->head_dim);
 }
 
 }  // namespace
@@ -544,6 +586,113 @@ int fcsa_decode(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* 
   }
   if (p->head_dim == 64) return launch_decode<__half, 64>(p, sh, qa, k_cache, v_cache, cache_seqlens, n_new, o, part, s);
   return launch_decode<__half, 128>(p, sh, qa, k_cache, v_cache, cache_seqlens, n_new, o, part, s);
+}
+
+int fcsa_forward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_tensor* q, const fcsa_tensor* k,
+                              const fcsa_tensor* v, const fcsa_l2norm* n, const fcsa_tensor* o, float* inv_l,
+                              void* stream) {
+  int r;
+  if ((r = check_varlen(p, vl))) return r;
+  if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
+  if ((r = check_tensor(q, "q")) || (r = check_tensor(k, "k")) || (r = check_tensor(v, "v")) ||
+      (r = check_tensor(o, "o")))
+    return r;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  const fcsa_tensor *qa = q, *ka = k;
+  if (n->groups != 0) {
+    // the row pass runs over the packed rows as one batch: rnorm is [heads][total][groups]
+    if ((r = check_rows(false, p->dtype, 1, p->heads, vl->total_q, p->head_dim, n->groups))) return r;
+    if ((r = check_tensor(&n->q_hat, "q_hat")) || (r = check_tensor(&n->k_hat, "k_hat"))) return r;
+    if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
+    fcsa::RowArgs a = row_args(1, p->head_dim, n->groups);
+    a.t[0] = {p->heads, vl->total_q, *q, n->q_hat, {}, n->q_rnorm};
+    a.t[1] = {p->kv_heads, vl->total_k, *k, n->k_hat, {}, n->k_rnorm};
+    if (g_ev[2][0]) cudaEventRecord(g_ev[2][0], s);
+    const cudaError_t e = fcsa::launch_row_fwd(a, p->dtype == FCSA_BF16, false, s);
+    if (g_ev[2][1]) cudaEventRecord(g_ev[2][1], s);
+    if ((r = row_pass_launched(e, "l2norm (q, k) launch"))) return r;
+    qa = &n->q_hat;
+    ka = &n->k_hat;
+  }
+  if (p->dtype == FCSA_BF16) {
+    if (p->head_dim == 64) r = launch_forward<__nv_bfloat16, 64, false, true>(p, qa, ka, v, o, inv_l, s, nullptr, vl);
+    else r = launch_forward<__nv_bfloat16, 128, false, true>(p, qa, ka, v, o, inv_l, s, nullptr, vl);
+  } else {
+    if (p->head_dim == 64) r = launch_forward<__half, 64, false, true>(p, qa, ka, v, o, inv_l, s, nullptr, vl);
+    else r = launch_forward<__half, 128, false, true>(p, qa, ka, v, o, inv_l, s, nullptr, vl);
+  }
+  if (r) return r;
+  // o = 0 in the rows outside every sequence
+  fcsa::TailArgs ta = {};
+  ta.t[0] = {o->ptr, o->sh, o->sn, p->heads, vl->total_q, vl->cu_seqlens_q};
+  return launch_varlen_tail(p, ta, 1, s);
+}
+
+size_t fcsa_backward_fused_varlen_workspace_bytes(const fcsa_problem* p, const fcsa_varlen* vl) {
+  if (check_varlen(p, vl)) return 0;
+  return varlen_layout(p, vl).total;
+}
+
+size_t fcsa_backward_fused_varlen_zeroed_bytes(const fcsa_problem* p, const fcsa_varlen* vl) {
+  if (check_varlen(p, vl)) return 0;
+  return varlen_layout(p, vl).ztotal;
+}
+
+int fcsa_backward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_l2norm* n,
+                               const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
+                               const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv, void* workspace,
+                               size_t workspace_bytes, void* zeroed, size_t zeroed_bytes, void* stream) {
+  int r;
+  if ((r = check_varlen(p, vl))) return r;
+  if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
+  if (n->groups != 0) {
+    if ((r = check_rows(false, p->dtype, 1, p->heads, vl->total_q, p->head_dim, n->groups))) return r;
+    if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
+  }
+  if ((r = check_tensor(&n->q_hat, "q")) || (r = check_tensor(&n->k_hat, "k")) || (r = check_tensor(v, "v")) ||
+      (r = check_tensor(o, "o")) || (r = check_tensor(d_o, "d_o")) || (r = check_tensor(dq, "dq")) ||
+      (r = check_tensor(dk, "dk")) || (r = check_tensor(dv, "dv")))
+    return r;
+  if (!inv_l) return fail(FCSA_ERR_INVALID, "inv_l: null");
+  const fcsa::BwdWorkspace w = varlen_layout(p, vl);
+  if (!workspace || workspace_bytes < w.total)
+    return fail(FCSA_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w.total, workspace_bytes);
+  if (!aligned16(workspace)) return fail(FCSA_ERR_INVALID, "workspace not 16-byte aligned");
+  if (!zeroed || zeroed_bytes < w.ztotal)
+    return fail(FCSA_ERR_WORKSPACE, "zeroed workspace too small: need %zu bytes, got %zu", w.ztotal, zeroed_bytes);
+  if (!aligned16(zeroed)) return fail(FCSA_ERR_INVALID, "zeroed workspace not 16-byte aligned");
+  fcsa::BwdHostArgs h;
+  h.dtype_bf16 = p->dtype == FCSA_BF16;
+  h.B = p->batch; h.H = p->heads; h.kv_heads = p->kv_heads; h.Nq = p->seq_q; h.Nk = p->seq_k;
+  h.D = p->head_dim; h.causal = p->causal ? 1 : 0;
+  h.scale = p->scale; h.shift = p->shift;
+  h.mask = nullptr; h.mask_sb = 0;
+  h.q = n->q_hat; h.k = n->k_hat; h.v = *v; h.o = *o; h.d_o = *d_o; h.dq = *dq; h.dk = *dk; h.dv = *dv;
+  h.inv_l = inv_l;
+  h.workspace = workspace;
+  h.zeroed = zeroed;
+  h.ev_start = g_ev[1][0];
+  h.ev_stop = g_ev[1][1];
+  h.ev_prep[0] = g_ev[3][0]; h.ev_prep[1] = g_ev[3][1];
+  h.ev_finish[0] = g_ev[4][0]; h.ev_finish[1] = g_ev[4][1];
+  h.q_rnorm = n->groups != 0 ? n->q_rnorm : nullptr;
+  h.k_rnorm = n->groups != 0 ? n->k_rnorm : nullptr;
+  h.groups = n->groups != 0 ? n->groups : 1;
+  h.cu_q = vl->cu_seqlens_q; h.cu_k = vl->cu_seqlens_k;
+  h.total_q = vl->total_q; h.total_k = vl->total_k;
+  int launches = 0;
+  const char* err = nullptr;
+  cudaError_t ce = cudaSuccess;
+  r = fcsa::run_backward_varlen(h, reinterpret_cast<cudaStream_t>(stream), &launches, &err, &ce);
+  g_launches.fetch_add(launches);
+  if (r == FCSA_ERR_CUDA) return fail(r, "%s: %s", err ? err : "backward", cudaGetErrorString(ce));
+  if (r != FCSA_OK) return fail(r, "%s", err ? err : "backward failed");
+  // zero gradients in the rows outside every sequence
+  fcsa::TailArgs ta = {};
+  ta.t[0] = {dq->ptr, dq->sh, dq->sn, p->heads, vl->total_q, vl->cu_seqlens_q};
+  ta.t[1] = {dk->ptr, dk->sh, dk->sn, p->kv_heads, vl->total_k, vl->cu_seqlens_k};
+  ta.t[2] = {dv->ptr, dv->sh, dv->sn, p->kv_heads, vl->total_k, vl->cu_seqlens_k};
+  return launch_varlen_tail(p, ta, 3, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

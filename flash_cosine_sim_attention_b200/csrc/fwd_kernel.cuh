@@ -42,6 +42,16 @@ struct FwdArgs {
   const float* bias_amax;       // optional device scalar: shift += max(*bias_amax, 0)  (fp16 range guard)
 };
 
+// Packed sequences (VARLEN instantiation): B sequences, Nq / Nk = the maximum lengths (they size the grid and clamp
+// the device lengths).  q is (total_q, H, D) and k, v (total_k, kv_heads, D), addressed by tensor maps of batch extent
+// 1; sequence b owns query rows [cu_q[b], cu_q[b + 1]) and key rows [cu_k[b], cu_k[b + 1]).  o has q's layout (o_sb is
+// unused) and inv_l is (H, total_q).
+struct FwdVarlenArgs : FwdArgs {
+  const int* cu_q;
+  const int* cu_k;
+  int total_q, total_k;
+};
+
 template <int D>
 struct FwdCfg {
   static constexpr int kTile = 128 * D * 2;          // bytes of one 128-row operand tile
@@ -55,10 +65,12 @@ struct FwdCfg {
   static_assert(kSmem <= 232448, "forward kernel shared memory");
 };
 
-template <typename T, int D, bool BIAS = false>
+template <typename T, int D, bool BIAS = false, bool VARLEN = false>
 __global__ void __launch_bounds__(384, 1)
 fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
-                const __grid_constant__ CUtensorMap tm_v, const FwdArgs a) {
+                const __grid_constant__ CUtensorMap tm_v,
+                const std::conditional_t<VARLEN, FwdVarlenArgs, FwdArgs> a) {
+  static_assert(!(BIAS && VARLEN), "packed sequences take no bias");
   using Cfg = FwdCfg<D>;
   constexpr int S = Cfg::kStages, TILE = Cfg::kTile, DCH = D / 64;
 
@@ -88,12 +100,10 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int b = bh / a.H, h = bh - b * a.H;
   const int hk = h / a.group;
   const int m0 = qblk * 128;
-  const int off = a.Nk - a.Nq;
-  int NT = (a.Nk + 127) >> 7;                                 // key tiles this block visits
-  if (a.causal) {
-    const int last_col = min(m0 + 127, a.Nq - 1) + off;
-    NT = last_col < 0 ? 0 : min(NT, (last_col >> 7) + 1);
-  }
+  // the (batch) coordinate of the tensor maps and the first query / key row of the sequence: packed sequences are
+  // row offsets into maps of batch extent 1; their lengths are read after pdl_wait (a previous kernel may write them)
+  const int tb = VARLEN ? 0 : b;
+  int Nq = a.Nq, Nk = a.Nk, q_row0 = 0, k_row0 = 0;
 
   if (threadIdx.x == 0) {
     mbar_init(BAR(Q_FULL), 1);
@@ -107,6 +117,17 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   }
   __syncthreads();
   pdl_wait();          // q, k (normalised by the previous kernel), v, mask are read from here on
+  if constexpr (VARLEN) {
+    const SeqSpan sq = seq_span(a.cu_q, b, a.Nq, a.total_q), sk = seq_span(a.cu_k, b, a.Nk, a.total_k);
+    Nq = sq.len; Nk = sk.len; q_row0 = sq.start; k_row0 = sk.start;
+    if (m0 >= Nq) return;                                     // a query block past the end of its sequence
+  }
+  const int off = Nk - Nq;
+  int NT = (Nk + 127) >> 7;                                   // key tiles this block visits
+  if (a.causal) {
+    const int last_col = min(m0 + 127, Nq - 1) + off;
+    NT = last_col < 0 ? 0 : min(NT, (last_col >> 7) + 1);
+  }
 
   if (wg == 0) {
     // =============================== TMA producer ===============================
@@ -117,7 +138,7 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       tma_prefetch_desc(&tm_v);
       mbar_expect_tx(BAR(Q_FULL), TILE);
 #pragma unroll
-      for (int ch = 0; ch < DCH; ++ch) tma_load_4d(sQ + ch * 16384, &tm_q, BAR(Q_FULL), ch * 64, m0, h, b);
+      for (int ch = 0; ch < DCH; ++ch) tma_load_4d(sQ + ch * 16384, &tm_q, BAR(Q_FULL), ch * 64, q_row0 + m0, h, tb);
       for (int j = 0; j < NT; ++j) {
         const int s = j % S;
         const uint32_t par = ((j / S) & 1) ^ 1;
@@ -125,12 +146,12 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         mbar_expect_tx(BAR(K_FULL + s), TILE);
 #pragma unroll
         for (int ch = 0; ch < DCH; ++ch)
-          tma_load_4d(sK + s * TILE + ch * 16384, &tm_k, BAR(K_FULL + s), ch * 64, j * 128, hk, b);
+          tma_load_4d(sK + s * TILE + ch * 16384, &tm_k, BAR(K_FULL + s), ch * 64, k_row0 + j * 128, hk, tb);
         mbar_wait(BAR(V_EMPTY + s), par);
         mbar_expect_tx(BAR(V_FULL + s), TILE);
 #pragma unroll
         for (int ch = 0; ch < DCH; ++ch)
-          tma_load_4d(sV + s * TILE + ch * 16384, &tm_v, BAR(V_FULL + s), ch * 64, j * 128, hk, b);
+          tma_load_4d(sV + s * TILE + ch * 16384, &tm_v, BAR(V_FULL + s), ch * 64, k_row0 + j * 128, hk, tb);
       }
     }
     return;
@@ -158,7 +179,7 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   // last visible column of each row (causal / ragged end)
   int lim[2];
 #pragma unroll
-  for (int hf = 0; hf < 2; ++hf) lim[hf] = a.causal ? min(a.Nk - 1, row_a + 8 * hf + off) : a.Nk - 1;
+  for (int hf = 0; hf < 2; ++hf) lim[hf] = a.causal ? min(Nk - 1, row_a + 8 * hf + off) : Nk - 1;
 
   float o[D / 2];
 #pragma unroll
@@ -187,7 +208,7 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
     // ---- P = exp2(S*c1 - c2 [+ bias*log2e]), masked; row sums in fp32; 16-bit P as A fragments ----
     const int col0 = j * 128;
-    const bool need_mask = a.has_mask || (col0 + 127 >= a.Nk) || (a.causal && col0 + 127 > m0 + 64 * w + off);
+    const bool need_mask = a.has_mask || (col0 + 127 >= Nk) || (a.causal && col0 + 127 > m0 + 64 * w + off);
     uint32_t pf[32];
     auto exp_tile = [&](auto masked_tag) {
       constexpr bool MASKED = decltype(masked_tag)::value;
@@ -253,8 +274,8 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     const int row = row_a + 8 * hf;
-    if (row >= a.Nq) continue;
-    const long long o_off = (long long)b * a.o_sb + (long long)h * a.o_sh + (long long)row * a.o_sn;
+    if (row >= Nq) continue;
+    const long long o_off = (long long)tb * a.o_sb + (long long)h * a.o_sh + (long long)(q_row0 + row) * a.o_sn;
     if (a.o_f32) {
       float* orow = reinterpret_cast<float*>(a.o) + o_off;
 #pragma unroll
@@ -268,7 +289,45 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         *reinterpret_cast<uint32_t*>(orow + 8 * jb + cq) =
             pack2<T>(o[4 * jb + 2 * hf] * inv[hf], o[4 * jb + 2 * hf + 1] * inv[hf]);
     }
-    if ((lane & 3) == 0 && a.inv_l != nullptr) a.inv_l[((long long)b * a.H + h) * a.Nq + row] = inv[hf];
+    if ((lane & 3) == 0 && a.inv_l != nullptr) {
+      if constexpr (VARLEN) a.inv_l[(long long)h * a.total_q + q_row0 + row] = inv[hf];
+      else a.inv_l[((long long)b * a.H + h) * a.Nq + row] = inv[hf];
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// Packed sequences: the rows that belong to no sequence
+// ------------------------------------------------------------------------------------------
+// With cumulative lengths cu[0 .. B] the sequences own rows [cu[0], cu[B]) of a packed tensor; rows [0, cu[0]) and
+// [cu[B], total) belong to none (e.g. a fixed-size packing buffer that is not full).  The attention kernels never
+// write them, so this pass sets them to zero in the outputs: o = 0 there, and zero gradients.  The bounds are read on
+// the device (clamped to [0, total]); when the sequences fill the tensor every block exits after two loads.
+struct TailArgs {
+  struct Tensor {
+    void* ptr;               // 16-bit (total, H, D) tensor, element strides sh, sn, features contiguous
+    long long sh, sn;
+    int H, total;
+    const int* cu;           // its cumulative lengths (B + 1 entries)
+  } t[3];
+  int B, D;
+};
+
+__global__ void __launch_bounds__(256) varlen_tail_kernel(const __grid_constant__ TailArgs a) {
+  pdl_launch_dependents();
+  pdl_wait();                          // the lengths may come from a previous kernel; the outputs are written after it
+  const TailArgs::Tensor& t = a.t[blockIdx.y];
+  const int lo = min(max(ld_cu(t.cu), 0), t.total);                  // rows [0, lo) and [hi, total) are cleared
+  const int hi = max(min(max(ld_cu(t.cu + a.B), 0), t.total), lo);
+  const int vpr = a.D / 8;                                           // 16-byte vectors per row
+  const long long n = (long long)(lo + t.total - hi) * t.H * vpr;
+  for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n; i += (long long)gridDim.x * 256) {
+    const int c = (int)(i % vpr);
+    const long long rh = i / vpr;
+    const int h = (int)(rh % t.H);
+    long long r = rh / t.H;
+    if (r >= lo) r += hi - lo;
+    *reinterpret_cast<uint4*>(static_cast<uint16_t*>(t.ptr) + h * t.sh + r * t.sn + c * 8) = make_uint4(0, 0, 0, 0);
   }
 }
 

@@ -370,4 +370,21 @@ __device__ __forceinline__ float2 lds64f(uint32_t addr) {
   return v;
 }
 
+// Rows [start, start + len) of sequence b of a packed tensor, from its cumulative lengths on the device.  Out-of-
+// contract lengths are clamped: the rows stay inside [0, total) and len <= max_len.
+struct SeqSpan {
+  int start, len;
+};
+// (volatile loads: a kernel that needs the span again late re-reads it instead of keeping it in registers)
+__device__ __forceinline__ int ld_cu(const int* p) {
+  int v;
+  asm volatile("ld.global.nc.s32 %0, [%1];" : "=r"(v) : "l"(p));
+  return v;
+}
+__device__ __forceinline__ SeqSpan seq_span(const int* cu, int b, int max_len, int total) {
+  const int s = min(max(ld_cu(cu + b), 0), total);
+  const int e = min(max(ld_cu(cu + b + 1), s), total);
+  return {s, min(e - s, max_len)};
+}
+
 }  // namespace fcsa

@@ -162,8 +162,7 @@ struct Workspaces {
 std::mutex g_ws_mutex;
 std::map<std::pair<int, void*>, Workspaces> g_ws;
 
-Workspaces backward_workspaces(const fcsa_problem& p, const Tensor& like, cudaStream_t stream) {
-  const size_t need_s = fcsa_backward_workspace_bytes(&p), need_z = fcsa_backward_zeroed_bytes(&p);
+Workspaces workspaces_of_size(size_t need_s, size_t need_z, const Tensor& like, cudaStream_t stream) {
   TORCH_CHECK(need_s > 0 && need_z > 0, "libfcsa_b200: ", fcsa_last_error());
   std::lock_guard<std::mutex> lock(g_ws_mutex);
   Workspaces& w = g_ws[{(int)like.get_device(), (void*)stream}];
@@ -174,6 +173,10 @@ Workspaces backward_workspaces(const fcsa_problem& p, const Tensor& like, cudaSt
     FCSA_CHECK(fcsa_zeroed_init(w.zeroed.data_ptr(), need_z, stream));
   }
   return w;
+}
+
+Workspaces backward_workspaces(const fcsa_problem& p, const Tensor& like, cudaStream_t stream) {
+  return workspaces_of_size(fcsa_backward_workspace_bytes(&p), fcsa_backward_zeroed_bytes(&p), like, stream);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -478,6 +481,128 @@ Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, 
   return o;
 }
 
+// ------------------------------------------------------------------------------------------------
+// packed variable-length sequences (fcsa_forward_fused_varlen / fcsa_backward_fused_varlen)
+//   q (total_q, H, D), k, v (total_k, kv_heads, D); cu_q, cu_k int32 (B + 1) on q's device, read by the kernels
+//   only (never copied: a CUDA graph replay must read the caller's buffers); max_q, max_k >= every length.
+// ------------------------------------------------------------------------------------------------
+// (total, heads, feature) -> the (batch, head, row) addressing of the ABI: one batch, rows = the packed rows
+fcsa_tensor view_packed(const Tensor& t) {
+  fcsa_tensor v;
+  v.ptr = t.data_ptr();
+  v.sb = 0; v.sh = t.stride(1); v.sn = t.stride(0);
+  return v;
+}
+
+struct Varlen {
+  fcsa_problem p;
+  fcsa_varlen vl;
+};
+
+Varlen varlen_problem(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& cu_q, const Tensor& cu_k,
+                      int64_t max_q, int64_t max_k, double scale, double shift, bool causal) {
+  TORCH_CHECK(q.dim() == 3 && k.dim() == 3 && v.dim() == 3,
+              "varlen: q must be (total_q, heads, head_dim) and k, v (total_k, kv_heads, head_dim)");
+  TORCH_CHECK(q.is_cuda() && k.is_cuda() && v.is_cuda(), "varlen: CUDA tensors required - this build has no CPU path");
+  TORCH_CHECK(k.scalar_type() == q.scalar_type() && v.scalar_type() == q.scalar_type(), "varlen: q, k, v must share one dtype");
+  TORCH_CHECK(k.sizes() == v.sizes(), "varlen: k and v must have the same shape");
+  const int64_t H = q.size(1), Hk = k.size(1), D = q.size(2);
+  TORCH_CHECK(k.size(2) == D, "varlen: head dimensions of q, k, v must match");
+  TORCH_CHECK(Hk > 0 && H % Hk == 0, "varlen: kv_heads (", Hk, ") must divide the query heads (", H, ")");
+  for (const Tensor* c : {&cu_q, &cu_k}) {
+    TORCH_CHECK(c->is_cuda() && c->get_device() == q.get_device() && c->scalar_type() == at::kInt && c->dim() == 1 &&
+                    c->size(0) >= 2,
+                "varlen: cu_seqlens must be int32 tensors of shape (batch + 1,) on q's device");
+    TORCH_CHECK(c->is_contiguous(), "varlen: cu_seqlens must be contiguous (not a strided or expanded view)");
+  }
+  TORCH_CHECK(cu_q.size(0) == cu_k.size(0), "varlen: cu_seqlens_q and cu_seqlens_k must have the same length");
+  TORCH_CHECK(max_q >= 1 && max_k >= 1 && max_q <= 0x7FFFFFFF && max_k <= 0x7FFFFFFF,
+              "varlen: max_seqlen_q / max_seqlen_k must be positive int32 values");
+  TORCH_CHECK(q.size(0) <= 0x7FFFFFFF && k.size(0) <= 0x7FFFFFFF, "varlen: too many packed rows");
+  Varlen r;
+  fcsa_problem& p = r.p;
+  p.dtype = dtype_code(q);
+  p.batch = (int32_t)(cu_q.size(0) - 1); p.heads = (int32_t)H; p.kv_heads = (int32_t)Hk;
+  p.seq_q = (int32_t)max_q; p.seq_k = (int32_t)max_k; p.head_dim = (int32_t)D;
+  p.causal = causal ? 1 : 0;
+  p.scale = (float)scale; p.shift = (float)shift;
+  p.key_mask = nullptr; p.key_mask_stride = 0;
+  p.out_f32 = 0; p.reserved_ = 0;
+  r.vl.cu_seqlens_q = cu_q.data_ptr<int32_t>();
+  r.vl.cu_seqlens_k = cu_k.data_ptr<int32_t>();
+  r.vl.total_q = (int32_t)q.size(0);
+  r.vl.total_k = (int32_t)k.size(0);
+  return r;
+}
+
+// groups > 0: q, k are RAW and l2-normalised inside; returns (o, inv_l, q_hat, k_hat, q_rnorm, k_rnorm), the last four
+// undefined when groups == 0, inv_l undefined unless need_inv_l
+std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> forward_varlen(
+    const Tensor& q_in, const Tensor& k_in, const Tensor& v_in, const Tensor& cu_q, const Tensor& cu_k, int64_t max_q,
+    int64_t max_k, double scale, double shift, bool causal, int64_t groups, bool need_inv_l) {
+  const c10::cuda::CUDAGuard guard(q_in.device());
+  const Tensor q = tma_ready(q_in), k = tma_ready(k_in), v = tma_ready(v_in);
+  const Varlen vr = varlen_problem(q, k, v, cu_q, cu_k, max_q, max_k, scale, shift, causal);
+  const int64_t H = q.size(1), Hk = k.size(1), Tq = q.size(0), Tk = k.size(0);
+  Tensor o = at::empty(q.sizes(), q.options());
+  Tensor inv_l;
+  if (need_inv_l) inv_l = at::empty({H, Tq}, q.options().dtype(at::kFloat));
+  Tensor qn, kn, rq, rk;
+  fcsa_l2norm n;
+  n.groups = (int32_t)groups;
+  n.q_hat = n.k_hat = fcsa_tensor{nullptr, 0, 0, 0};
+  n.q_rnorm = n.k_rnorm = nullptr;
+  if (groups > 0) {
+    qn = at::empty(q.sizes(), q.options());
+    kn = at::empty(k.sizes(), k.options());
+    rq = at::empty({H, Tq, groups}, q.options().dtype(at::kFloat));
+    rk = at::empty({Hk, Tk, groups}, q.options().dtype(at::kFloat));
+    n.q_hat = view_packed(qn); n.k_hat = view_packed(kn);
+    n.q_rnorm = rq.data_ptr<float>(); n.k_rnorm = rk.data_ptr<float>();
+  }
+  const fcsa_tensor tq = view_packed(q), tk = view_packed(k), tv = view_packed(v), to = view_packed(o);
+  FCSA_CHECK(fcsa_forward_fused_varlen(&vr.p, &vr.vl, &tq, &tk, &tv, &n, &to, need_inv_l ? inv_l.data_ptr<float>() : nullptr,
+                                       at::cuda::getCurrentCUDAStream().stream()));
+  return {o, inv_l, qn, kn, rq, rk};
+}
+
+// gradients of forward_varlen w.r.t. the raw q, k (groups > 0: q, k are the normalised tensors it returned) and v
+std::tuple<Tensor, Tensor, Tensor> backward_varlen(
+    const Tensor& d_out, const Tensor& o_in, const Tensor& inv_l, const Tensor& q_in, const Tensor& k_in,
+    const Tensor& v_in, const optional<Tensor>& q_rnorm, const optional<Tensor>& k_rnorm, const Tensor& cu_q,
+    const Tensor& cu_k, int64_t max_q, int64_t max_k, double scale, double shift, bool causal, int64_t groups) {
+  const c10::cuda::CUDAGuard guard(q_in.device());
+  const Tensor q = tma_ready(q_in), k = tma_ready(k_in), v = tma_ready(v_in), o = tma_ready(o_in),
+               d_o = tma_ready(d_out);
+  const Varlen vr = varlen_problem(q, k, v, cu_q, cu_k, max_q, max_k, scale, shift, causal);
+  TORCH_CHECK(d_o.sizes() == q.sizes() && d_o.scalar_type() == q.scalar_type() && o.sizes() == q.sizes() &&
+                  o.scalar_type() == q.scalar_type(),
+              "backward_varlen: o and d_out must have the shape and dtype of the queries");
+  TORCH_CHECK(inv_l.scalar_type() == at::kFloat && inv_l.is_contiguous() && inv_l.numel() == q.size(0) * q.size(1),
+              "backward_varlen: inv_l must be the (heads, total_q) float32 tensor of the forward");
+  Tensor dq = at::empty(q.sizes(), q.options());
+  Tensor dk = at::empty(k.sizes(), k.options());
+  Tensor dv = at::empty(v.sizes(), v.options());
+  cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
+  const Workspaces ws = workspaces_of_size(fcsa_backward_fused_varlen_workspace_bytes(&vr.p, &vr.vl),
+                                           fcsa_backward_fused_varlen_zeroed_bytes(&vr.p, &vr.vl), q, stream);
+  fcsa_l2norm n;
+  n.groups = (int32_t)groups;
+  n.q_hat = view_packed(q); n.k_hat = view_packed(k);
+  n.q_rnorm = n.k_rnorm = nullptr;
+  if (groups > 0) {
+    TORCH_CHECK(q_rnorm.has_value() && q_rnorm->defined() && k_rnorm.has_value() && k_rnorm->defined(),
+                "backward_varlen: q_rnorm and k_rnorm are needed with groups > 0");
+    n.q_rnorm = q_rnorm->data_ptr<float>(); n.k_rnorm = k_rnorm->data_ptr<float>();
+  }
+  const fcsa_tensor tv = view_packed(v), to = view_packed(o), tdo = view_packed(d_o), tdq = view_packed(dq),
+                    tdk = view_packed(dk), tdv = view_packed(dv);
+  FCSA_CHECK(fcsa_backward_fused_varlen(&vr.p, &vr.vl, &n, &tv, &to, &tdo, inv_l.data_ptr<float>(), &tdq, &tdk, &tdv,
+                                        ws.scratch.data_ptr(), (size_t)ws.scratch.numel(), ws.zeroed.data_ptr(),
+                                        (size_t)ws.zeroed.numel(), stream));
+  return {dq, dk, dv};
+}
+
 // Drops the cached backward workspaces of every (device, stream) (they only ever grow: a long-context call leaves a
 // 1 GB accumulator behind).  Returns the number of bytes released to the caching allocator.  Safe at any time between
 // calls: buffers still referenced by enqueued kernels stay alive through the allocator's stream semantics.
@@ -514,6 +639,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("f32_cast_backward", &f32_cast_backward, "backward of f32_cast: float32 gradient w.r.t. the float32 input");
   m.def("l2norm_forward", &l2norm_forward, "grouped l2norm: x -> (y, 1/norm)");
   m.def("l2norm_backward", &l2norm_backward, "grouped l2norm backward from the normalised y");
+  m.def("forward_varlen", &forward_varlen, "packed variable-length sequences: forward (fused l2norm when groups > 0)");
+  m.def("backward_varlen", &backward_varlen, "backward of forward_varlen");
   m.def("decode", &decode, "new queries against a key/value cache, appending k / v at cache_seqlens");
   m.def("release_workspaces", &release_workspaces, "free the cached backward workspaces; returns the bytes released");
   m.def("abi_version", []() { return fcsa_version(); });

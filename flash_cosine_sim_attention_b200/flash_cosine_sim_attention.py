@@ -7,6 +7,8 @@ flash_cosine_sim_attention/flash_cosine_sim_attention.py, kept name-for-name so 
     l2norm_tensors(*tensors, groups)                                    reference py:57-65
     flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens, k, v, ...)
                                       decoding with a key/value cache (no reference counterpart)
+    flash_cosine_sim_attention_varlen(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, ...)
+                                      packed variable-length sequences (no reference counterpart)
     plain_cosine_sim_attention(...)   naive un-fused formulation        reference py:75-126
     FlashCosineSimAttention (autograd.Function) / forward / backward / debug   py:245-304, cu:1928-1933
 
@@ -31,6 +33,7 @@ from . import _abi
 __all__ = [
     "flash_cosine_sim_attention",
     "flash_cosine_sim_attention_with_kv_cache",
+    "flash_cosine_sim_attention_varlen",
     "plain_cosine_sim_attention",
     "l2norm_tensors",
     "FlashCosineSimAttention",
@@ -645,3 +648,115 @@ def flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens,
     shift = _choose_shift(q.dtype, scale, groups, l2norm_qk)
     return _ext().decode(q, k_cache, v_cache, cache_seqlens, k, v, float(scale), float(shift), bool(causal),
                          int(groups) if l2norm_qk else 0)
+
+
+class _FusedVarlenAttention(Function):
+    """One autograd node for packed sequences: l2norm(q), l2norm(k) -> attention, all in CUDA kernels."""
+
+    @staticmethod
+    def forward(ctx, q, k, v, cu_q, cu_k, max_q, max_k, scale, causal, groups, l2norm_qk):
+        shift = _choose_shift(q.dtype, scale, groups, l2norm_qk)
+        g = groups if l2norm_qk else 0
+        needs_grad = any(ctx.needs_input_grad[:3])
+        o, inv_l, qn, kn, rq, rk = _ext().forward_varlen(q, k, v, cu_q, cu_k, max_q, max_k, scale, shift, causal, g,
+                                                         needs_grad)
+        if needs_grad:
+            if not l2norm_qk:
+                qn, kn = q, k
+            ctx.save_for_backward(o, inv_l, qn, kn, v, rq, rk, cu_q, cu_k)
+            ctx.params = (max_q, max_k, scale, shift, causal, g)
+        return o
+
+    @staticmethod
+    def backward(ctx, do):
+        o, inv_l, qn, kn, v, rq, rk, cu_q, cu_k = ctx.saved_tensors
+        max_q, max_k, scale, shift, causal, g = ctx.params
+        dq, dk, dv = _ext().backward_varlen(do, o, inv_l, qn, kn, v, rq, rk, cu_q, cu_k, max_q, max_k, scale, shift,
+                                            causal, g)
+        return (dq, dk, dv) + (None,) * 8
+
+
+class _EmptyVarlenAttention(Function):
+    """Packed tensors with no query or no key rows: o = 0 and zero gradients, with no kernel launch."""
+
+    @staticmethod
+    def forward(ctx, q, k, v):
+        ctx.kv = (k.shape, v.shape, k.dtype, k.device)
+        return q.new_zeros(q.shape)
+
+    @staticmethod
+    def backward(ctx, do):
+        ks, vs, dtype, device = ctx.kv
+        return (torch.zeros_like(do), torch.zeros(ks, dtype=dtype, device=device),
+                torch.zeros(vs, dtype=dtype, device=device))
+
+
+def _check_varlen_args(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, groups, mask, attn_bias):
+    """Everything flash_cosine_sim_attention_varlen rejects before touching a device."""
+    name = "flash_cosine_sim_attention_varlen"
+    if exists(attn_bias):
+        raise NotImplementedError(f"{name}: attn_bias is not supported")
+    if exists(mask):
+        raise NotImplementedError(f"{name}: no key-padding mask - cu_seqlens_k gives each sequence's keys")
+    if q.ndim != 3 or k.ndim != 3 or v.ndim != 3:
+        raise ValueError(f"{name}: q must be (total_q, heads, head_dim) and k, v (total_k, kv_heads, head_dim)")
+    if q.dtype == torch.float32:
+        raise TypeError(f"{name}: float32 is not supported - use float16 or bfloat16")
+    if q.dtype not in _KERNEL_DTYPES:
+        raise TypeError(f"{name}: dtype {q.dtype} is not supported (float16, bfloat16)")
+    if k.dtype != q.dtype or v.dtype != q.dtype:
+        raise TypeError(f"{name}: q, k, v must share one dtype")
+    D = q.shape[-1]
+    if D not in _KERNEL_HEAD_DIMS:
+        raise NotImplementedError(f"{name}: head_dim {D} (64 and 128 only)")
+    if k.shape != v.shape or k.shape[-1] != D:
+        raise ValueError(f"{name}: k and v must both be (total_k, kv_heads, {D}) (got {tuple(k.shape)} and "
+                         f"{tuple(v.shape)})")
+    hk = k.shape[1]
+    if hk <= 0 or q.shape[1] % hk != 0:
+        raise ValueError(f"{name}: kv_heads ({hk}) must divide the query heads ({q.shape[1]})")
+    for t in (cu_seqlens_q, cu_seqlens_k):
+        if not torch.is_tensor(t) or t.dtype != torch.int32 or t.ndim != 1 or t.shape[0] < 2:
+            raise TypeError(f"{name}: cu_seqlens_q and cu_seqlens_k must be int32 tensors of shape (batch + 1,)")
+        if not t.is_contiguous():
+            raise ValueError(f"{name}: cu_seqlens must be contiguous (the kernels read them as dense arrays and a CUDA "
+                             "graph replay reads the caller's buffer; not a strided or expanded view)")
+    if cu_seqlens_q.shape != cu_seqlens_k.shape:
+        raise ValueError(f"{name}: cu_seqlens_q and cu_seqlens_k must have the same length")
+    for m in (max_seqlen_q, max_seqlen_k):
+        if isinstance(m, bool) or not isinstance(m, int) or m < 0:
+            raise TypeError(f"{name}: max_seqlen_q and max_seqlen_k must be non-negative Python ints")
+    gs = D // groups if groups > 0 and D % groups == 0 else 0
+    if gs == 0 or (gs & (gs - 1)) != 0:
+        raise ValueError(f"{name}: groups {groups} must divide head_dim {D} into power-of-two chunks")
+    if not (q.is_cuda and k.is_cuda and v.is_cuda):
+        raise RuntimeError(f"{name}: CUDA tensors required - this build has no CPU path")
+    if not (cu_seqlens_q.is_cuda and cu_seqlens_k.is_cuda and cu_seqlens_q.device == q.device
+            and cu_seqlens_k.device == q.device):
+        raise RuntimeError(f"{name}: cu_seqlens must be on q's CUDA device (the host never reads them)")
+
+
+def flash_cosine_sim_attention_varlen(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale=8,
+                                      groups=1, causal=False, l2norm_qk=True, mask=None, attn_bias=None):
+    """Cosine-sim attention over packed variable-length sequences (training: forward and backward).
+
+    q: (total_q, heads, head_dim); k, v: (total_k, kv_heads, head_dim), kv_heads dividing heads (query head h reads kv
+    head h // (heads // kv_heads)).  Views with a contiguous head dim (e.g. slices of a packed projection output) are
+    read without a copy.  cu_seqlens_q, cu_seqlens_k: contiguous int32 CUDA tensors (batch + 1,), non-decreasing from 0;
+    sequence b is query rows [cu_seqlens_q[b], cu_seqlens_q[b + 1]) and key rows [cu_seqlens_k[b], cu_seqlens_k[b + 1]).
+    Pass the same tensor twice for self-attention.  They are never read on the host, so a call does not synchronise and
+    a training step can be captured in a CUDA graph.  max_seqlen_q, max_seqlen_k: Python ints, at least every length
+    (they size the grids; lengths above them are clamped).
+
+    Each sequence gets what flash_cosine_sim_attention gives on it alone: the same scale, groups, l2norm and exponent
+    shift; causal masking is bottom-right per sequence (key j visible to query i iff j <= i + len_k - len_q).  Empty
+    sequences are allowed, and query rows that see no key give 0.  Rows outside every sequence ([0, cu[0]) and
+    [cu[-1], total), e.g. the unused end of a fixed-size packing buffer) give o = 0 and zero gradients.  Packed tensors
+    with no query or no key rows give zeros (and zero gradients) without a kernel launch.  float16 / bfloat16 and head dims 64 and 128 only; no float32, mask or
+    attn_bias.  Returns o (total_q, heads, head_dim)."""
+    _check_varlen_args(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, groups, mask, attn_bias)
+    if q.shape[0] == 0 or k.shape[0] == 0:
+        return _EmptyVarlenAttention.apply(q, k, v)
+    return _FusedVarlenAttention.apply(q, k, v, cu_seqlens_q, cu_seqlens_k, max(int(max_seqlen_q), 1),
+                                       max(int(max_seqlen_k), 1), float(scale), bool(causal), int(groups),
+                                       bool(l2norm_qk))

@@ -15,8 +15,8 @@ import torch
 import torch.nn.functional as F
 from torch import nn
 
-from .flash_cosine_sim_attention import (flash_cosine_sim_attention, flash_cosine_sim_attention_with_kv_cache,
-                                         plain_cosine_sim_attention)
+from .flash_cosine_sim_attention import (flash_cosine_sim_attention, flash_cosine_sim_attention_varlen,
+                                         flash_cosine_sim_attention_with_kv_cache, plain_cosine_sim_attention)
 
 
 def _softmax_attention(q, k, v, **unused):
@@ -92,7 +92,14 @@ class Attention(nn.Module):
         self.to_v = nn.Linear(dim, dim_head * kv_heads, bias=False)
         self.to_out = nn.Linear(inner, dim, bias=False)
 
-    def forward(self, x, cache=None):
+    def forward(self, x, cache=None, cu_seqlens=None, max_seqlen=None):
+        """cu_seqlens: x is one packed row of documents, (1, total, dim), and cu_seqlens (documents + 1,) int32 their
+        boundaries; every document attends causally to itself only.  max_seqlen: at least every document's length
+        (default: total)."""
+        if cu_seqlens is not None:
+            if cache is not None:
+                raise NotImplementedError("packed documents (cu_seqlens) with a key/value cache are not supported")
+            return self._forward_packed(x, cu_seqlens, max_seqlen)
         b, n, _ = x.shape
         x = self.norm(x)
         # (b, n, h*d) -> (b, h, n, d) views: strided, feature dim contiguous - the fused op reads
@@ -105,6 +112,38 @@ class Attention(nn.Module):
         else:
             o = self._attend_cached(q, k, v, cache)
         return self.to_out(o.transpose(1, 2).reshape(b, n, -1))
+
+    def _forward_packed(self, x, cu_seqlens, max_seqlen):
+        if x.ndim != 3 or x.shape[0] != 1:
+            raise ValueError(f"packed documents take x of shape (1, total, dim), got {tuple(x.shape)}")
+        n = x.shape[1]
+        x = self.norm(x)
+        # (1, total, h*d) -> (total, h, d) views of the projections, read by the varlen kernels without a copy
+        q = self.to_q(x).view(n, self.heads, -1)
+        k, v = self.to_k(x).view(n, self.kv_heads, -1), self.to_v(x).view(n, self.kv_heads, -1)
+        if self.use_cuda_kernel:
+            unsupported = sorted(set(self.kernel_kwargs) - {"l2norm_qk"})
+            if unsupported:
+                raise NotImplementedError(f"packed documents do not support the attention keywords {unsupported}")
+            m = n if max_seqlen is None else int(max_seqlen)
+            o = flash_cosine_sim_attention_varlen(q, k, v, cu_seqlens, cu_seqlens, m, m, scale=self.scale,
+                                                  groups=self.l2norm_groups, causal=True,
+                                                  l2norm_qk=self.kernel_kwargs.get("l2norm_qk", True))
+        else:
+            # the reference: one call per document (reads the boundaries on the host)
+            bounds = cu_seqlens.tolist()
+            # rows outside every document give 0, as with the kernel
+            outs = [q.new_zeros(bounds[0], self.heads, q.shape[-1])] if bounds[0] > 0 else []
+            for s, e in zip(bounds[:-1], bounds[1:]):
+                if e > s:
+                    per_doc = lambda t: t[s:e].transpose(0, 1).unsqueeze(0)
+                    o_d = self.attn_fn(per_doc(q), per_doc(k), per_doc(v), causal=True, scale=self.scale,
+                                       groups=self.l2norm_groups)
+                    outs.append(o_d[0].transpose(0, 1))
+            if bounds[-1] < n:
+                outs.append(q.new_zeros(n - bounds[-1], self.heads, q.shape[-1]))
+            o = torch.cat(outs) if outs else q.new_zeros(q.shape)
+        return self.to_out(o.reshape(1, n, -1))
 
     def _attend_cached(self, q, k, v, cache):
         """q, k, v of the next n tokens against the cached prefix; appends k, v to the cache."""
@@ -205,9 +244,17 @@ class CosineSimCausalTransformer(nn.Module):
         self.train(was_training)
         return out[:, n0:]
 
-    def forward(self, x, return_loss=False, cache=None):
+    def forward(self, x, return_loss=False, cache=None, cu_seqlens=None, max_seqlen=None):
         """cache: the list new_cache() returned - x are then the next tokens after the cached ones, and their
-        positions start at the cache's length."""
+        positions start at the cache's length.  cu_seqlens: x is one packed row of documents, (1, total), split at
+        the int32 boundaries cu_seqlens (documents + 1,); positions restart at 0 in every document and no document
+        sees another.  max_seqlen: at least every document's length (default: min(total, max_seq_len)); documents
+        must not be longer than max_seq_len."""
+        if cu_seqlens is not None:
+            if cache is not None or return_loss:
+                raise NotImplementedError("packed documents (cu_seqlens) with a key/value cache or return_loss are not "
+                                          "supported")
+            return self._forward_packed(x, cu_seqlens, max_seqlen)
         if return_loss:
             x, labels = x[:, :-1], x[:, 1:]
         start = 0 if cache is None else cache[0].length
@@ -224,3 +271,22 @@ class CosineSimCausalTransformer(nn.Module):
         if not return_loss:
             return logits
         return F.cross_entropy(logits.transpose(1, 2), labels)
+
+    def _forward_packed(self, x, cu_seqlens, max_seqlen):
+        if x.ndim != 2 or x.shape[0] != 1:
+            raise ValueError(f"packed documents take x of shape (1, total), got {tuple(x.shape)}")
+        n = x.shape[1]
+        if max_seqlen is None:
+            max_seqlen = min(n, self.max_seq_len)
+        elif max_seqlen > self.max_seq_len:
+            raise ValueError(f"max_seqlen {max_seqlen} exceeds max_seq_len {self.max_seq_len}")
+        # positions restart at 0 in every document, computed on the device: row t belongs to the last document that
+        # starts at or before it (clamped into the embedding table for out-of-contract boundaries)
+        t = torch.arange(n, device=x.device, dtype=cu_seqlens.dtype)
+        doc = (torch.searchsorted(cu_seqlens, t, right=True) - 1).clamp(0, cu_seqlens.shape[0] - 1)
+        pos = (t - cu_seqlens[doc]).clamp(0, self.max_seq_len - 1)
+        x = self.token_emb(x) + self.pos_emb(pos)[None]
+        for attn, attn_norm, ff, ff_norm in self.layers:
+            x = attn_norm(attn(x, cu_seqlens=cu_seqlens, max_seqlen=max_seqlen) + x * self.residual_scale)
+            x = ff_norm(ff(x) + x * self.residual_scale)
+        return self.to_logits(x)

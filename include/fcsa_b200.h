@@ -271,6 +271,46 @@ int fcsa_decode(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* 
                 const int32_t* cache_seqlens, const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t n_new,
                 int32_t groups, const fcsa_tensor* o, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- packed variable-length sequences (no reference counterpart) ------------------------------------------------------
+ * Training attention over B sequences of different lengths packed along the row dimension, without padding:
+ *   p              : batch = B (sequences), seq_q / seq_k = maximum lengths (they size the grids and clamp the device
+ *                    lengths), heads / kv_heads / head_dim / causal / scale / shift as in fcsa_problem; no key_mask,
+ *                    out_f32 = 0
+ *   vl             : the cumulative lengths, DEVICE int32 arrays of B + 1 entries, non-decreasing from 0, never read by
+ *                    the host (a step can be captured in a CUDA graph).  Sequence b owns query rows
+ *                    [cu_seqlens_q[b], cu_seqlens_q[b + 1]) and key rows [cu_seqlens_k[b], cu_seqlens_k[b + 1]).
+ *                    total_q / total_k: the rows of the packed tensors
+ *   q, o, d_o, dq  : (total_q, heads, head_dim) as fcsa_tensor with sh, sn set (sb unused)
+ *   k, v, dk, dv   : (total_k, kv_heads, head_dim), likewise
+ *   inv_l          : (heads, total_q) fp32
+ *   n              : groups > 0: q, k are l2-normalised as in fcsa_forward_fused; q_hat / k_hat are (total, heads,
+ *                    head_dim) and q_rnorm / k_rnorm [heads][total][groups].  groups == 0: q, k are used as given (the
+ *                    forward ignores q_hat, k_hat and the rnorms; the backward reads q, k from q_hat, k_hat).
+ * Each sequence gets what fcsa_forward_fused / fcsa_backward_fused give on it alone, with the causal rule applied to
+ * its own lengths (key j visible to query i iff j <= i + len_k - len_q); rows with no visible key give o = 0.
+ * Rows that belong to no sequence ([0, cu[0]) and [cu[B], total), e.g. the unused end of a fixed-size packing buffer)
+ * get o = 0 and zero dq, dk, dv.  Out-of-contract lengths (above the maxima, or rows past the totals) are clamped:
+ * nothing is accessed outside the tensors, and the rows past the clamp are unspecified.
+ * Workspaces: the backward's scratch and zeroed buffers (same contract as fcsa_backward's: the zeroed one is zero on
+ * entry and on exit) are pure functions of B, heads, kv_heads, the totals and head_dim.
+ */
+typedef struct fcsa_varlen {
+  const int32_t* cu_seqlens_q;
+  const int32_t* cu_seqlens_k;
+  int32_t total_q;
+  int32_t total_k;
+} fcsa_varlen;
+
+int fcsa_forward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_tensor* q, const fcsa_tensor* k,
+                              const fcsa_tensor* v, const fcsa_l2norm* n, const fcsa_tensor* o, float* inv_l,
+                              void* stream);
+size_t fcsa_backward_fused_varlen_workspace_bytes(const fcsa_problem* p, const fcsa_varlen* vl);
+size_t fcsa_backward_fused_varlen_zeroed_bytes(const fcsa_problem* p, const fcsa_varlen* vl);
+int fcsa_backward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_l2norm* n,
+                               const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
+                               const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv, void* workspace,
+                               size_t workspace_bytes, void* zeroed, size_t zeroed_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
