@@ -318,8 +318,10 @@ __device__ __forceinline__ uint32_t pack2<__nv_bfloat16>(float lo, float hi) {
 template <>
 __device__ __forceinline__ uint32_t pack2<__half>(float lo, float hi) {
   uint32_t r;
-  // satfinite: an out-of-range value becomes +-65504 instead of inf (fp16 has no headroom for
-  // exp(scale * q.k) when grouped l2norm lets q.k exceed 1)
+  // satfinite: an out-of-range value becomes +-65504 instead of inf.  This does not make an
+  // overflowing p right: the forward adds the unsaturated fp32 p to the row sum, so a row with
+  // p > 65504 (fp16, grouped l2norm, scale*(groups - 1) > ln 65504, see _choose_shift) comes out
+  // finite and scaled down by 65504 / p; the host warns when a call can reach that
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }

@@ -257,9 +257,12 @@ def _choose_shift(dtype, scale, groups, l2norm_qk):
             is 2^-14 .. 2^15 (e^20); shift = scale*groups - 15 ln 2 puts the largest possible p at 2^15 and, as
             long as scale*groups <= 10, the smallest at 2^15 e^-20 > 2^-14: nothing under- or overflows.
       fp16, scale*groups > 10: more range than fp16 has without a row max.  Same choice as the reference
-            (shift = scale); the kernels saturate p at 65504 instead of producing inf and tiny p flush to
-            zero - rows whose best match is poor lose precision.  Use bf16 (or float32 inputs, which switch
-            to the bf16 kernels by themselves) for grouped l2norm with a large scale*groups."""
+            (shift = scale): tiny p flush to zero, and once scale*(groups - 1) > ln 65504 the rows whose best
+            match is GOOD (q.k near `groups`) have p = exp(scale*(q.k - 1)) above fp16's maximum.  The kernels
+            saturate that p at 65504 for P V but add the unsaturated fp32 p to the row sum, so such a row comes
+            out finite and wrong (o scaled down by 65504 / p; dq, dk follow).  `_fp16_overflows` tells when that
+            can happen and the entry points warn.  Use bf16 (or float32 inputs, which switch to the bf16
+            kernels by themselves) for grouped l2norm with a large scale*groups."""
     if not l2norm_qk:
         return float(scale)
     if dtype == torch.bfloat16:
@@ -267,6 +270,22 @@ def _choose_shift(dtype, scale, groups, l2norm_qk):
     if scale * groups <= _FP16_GROUPED_RANGE:
         return float(scale * groups) - 15.0 * math.log(2.0)
     return float(scale)
+
+
+def _fp16_overflows(dtype, scale, groups, l2norm_qk):
+    """True when fp16 kernels with l2norm can meet p = exp(scale*q.k - shift) above fp16's maximum 65504: q.k reaches
+    `groups` (a query aligned with a key in every l2norm group), so the largest p is exp(scale*groups - shift)."""
+    if dtype != torch.float16 or not l2norm_qk:
+        return False
+    return scale * groups - _choose_shift(dtype, scale, groups, True) > math.log(65504.0)
+
+
+def _warn_fp16_overflow(dtype, scale, groups, l2norm_qk):
+    if _fp16_overflows(dtype, scale, groups, l2norm_qk):
+        _warn_once("f16-overflow", f"flash_cosine_sim_attention: float16 with l2norm at scale {scale:g} and groups "
+                                   f"{groups}: exp(scale*q.k - shift) exceeds fp16's maximum when q.k is near "
+                                   "`groups`, so rows whose query matches a key well come out wrong (finite, not "
+                                   "inf) and so do their gradients; use bfloat16")
 
 
 class _FusedCosineSimAttention(Function):
@@ -537,6 +556,7 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
         return _float32_on_half_kernels(q, k, v, mask, attn_bias, scale, groups, causal, l2norm_qk, attn_bias_batch_dim)
     if q.dtype not in _KERNEL_DTYPES:
         raise TypeError(f"flash_cosine_sim_attention: dtype {q.dtype} is not supported (float16, bfloat16, float32)")
+    _warn_fp16_overflow(q.dtype, scale, groups, l2norm_qk)
     if D not in _KERNEL_HEAD_DIMS:
         # Head dims the kernels are not instantiated for (the reference's 16, 32 and 96): zero-pad the
         # features to 64 / 128 and run the same wgmma kernels.  Zero features change neither q.k nor
@@ -645,6 +665,7 @@ def flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens,
     capacity.  float16 / bfloat16 and head dims 64 and 128 only; no autograd, attn_bias, mask, float32 or merged
     batch-heads.  Returns o (batch, heads, n_q, head_dim)."""
     _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias)
+    _warn_fp16_overflow(q.dtype, scale, groups, l2norm_qk)
     shift = _choose_shift(q.dtype, scale, groups, l2norm_qk)
     return _ext().decode(q, k_cache, v_cache, cache_seqlens, k, v, float(scale), float(shift), bool(causal),
                          int(groups) if l2norm_qk else 0)
@@ -755,6 +776,7 @@ def flash_cosine_sim_attention_varlen(q, k, v, cu_seqlens_q, cu_seqlens_k, max_s
     with no query or no key rows give zeros (and zero gradients) without a kernel launch.  float16 / bfloat16 and head dims 64 and 128 only; no float32, mask or
     attn_bias.  Returns o (total_q, heads, head_dim)."""
     _check_varlen_args(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, groups, mask, attn_bias)
+    _warn_fp16_overflow(q.dtype, scale, groups, l2norm_qk)
     if q.shape[0] == 0 or k.shape[0] == 0:
         return _EmptyVarlenAttention.apply(q, k, v)
     return _FusedVarlenAttention.apply(q, k, v, cu_seqlens_q, cu_seqlens_k, max(int(max_seqlen_q), 1),

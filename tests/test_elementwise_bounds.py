@@ -5,7 +5,8 @@ import numpy as np
 import pytest
 import torch
 
-from elementwise_bounds import C, U, attention_bounds, check_bound, kernel_shift
+import logit_range
+from elementwise_bounds import C, U, attention_bounds, check_bound, kernel_shift, ratio
 from gqa_reference import gqa_attention
 from oracle import cosine_sim_attention_oracle as oracle
 
@@ -71,9 +72,11 @@ def emulate(q, k, v, do, fmt, mask=None, attn_bias=None, scale=8, groups=1, caus
     """What the kernels compute, in float32 with every 16-bit rounding in its place: q^, k^ stored in T; S = q^ k^T
     and p = exp(scale S + bias - shift) in fp32; p -> T before P V, l summed in fp32, o -> T; in the backward
     delta from the stored o, P -> T before dV, dS -> T before dK / dQ, the l2norm backward on the stored q^, k^ with
-    fp32 1/||x||, outputs -> T (d_bias summed in fp32)."""
+    fp32 1/||x||, outputs -> T (d_bias summed in fp32).  p is packed with saturation in fp16 (65504, not inf) while l
+    sums the unsaturated fp32 p, and 1/||x|| uses the l2norm's 1e-12 clamp, as in the kernels."""
     f32 = np.float32
     T = lambda x: oracle.round_to(x, fmt).astype(f32)
+    Tp = (lambda x: T(np.minimum(x, f32(65504)))) if fmt == "f16" else T
     shift = f32(kernel_shift(fmt, scale, groups, l2norm_qk, attn_bias))
     merged, single = q.ndim == 3, k.ndim == 3
     if merged:
@@ -104,7 +107,7 @@ def emulate(q, k, v, do, fmt, mask=None, attn_bias=None, scale=8, groups=1, caus
             p = np.where(vis, np.exp(logit - shift), f32(0))
             l = p.sum(-1, dtype=f32)
             inv_l = f32(1) / np.maximum(l, f32(1e-37))
-            o[b, h] = T((T(p) @ v[b, hk]) * inv_l[:, None])
+            o[b, h] = T((Tp(p) @ v[b, hk]) * inv_l[:, None])
             delta = (do[b, h] * o[b, h]).sum(-1, dtype=f32, keepdims=True)
             with np.errstate(over="ignore"):         # rows without a visible key: 0 * (1 / 1e-37), then masked
                 P = np.where(vis, np.exp(logit - shift) * inv_l[:, None], f32(0))
@@ -119,7 +122,8 @@ def emulate(q, k, v, do, fmt, mask=None, attn_bias=None, scale=8, groups=1, caus
     def l2bwd(dy, y, n):
         g = y.reshape(*y.shape[:-1], groups, -1)
         d = dy.reshape(g.shape)
-        return ((d - g * (g * d).sum(-1, keepdims=True)) * (f32(1) / n.astype(f32))[..., None]).reshape(y.shape)
+        rn = f32(1) / np.maximum(n, 1e-12).astype(f32)
+        return ((d - g * (g * d).sum(-1, keepdims=True)) * rn[..., None]).reshape(y.shape)
     dq, dk = (l2bwd(dqn, qn, nq), l2bwd(dkn, kn, nk)) if l2norm_qk else (dqn, dkn)
     out = [T(o), T(dq), T(dk), T(dv)] + ([] if db is None else [T(db)])
     if merged:
@@ -150,6 +154,71 @@ def test_emulated_rounding_within_bound(name, fmt):
     for n, g in zip(("o", "dq", "dk", "dv", "d_bias"), got):
         w = check_bound(n, torch.from_numpy(g), ref, bound, fmt, c=C / 2) * C / 2
         EMULATION_WORST[f"{fmt}:{n}"] = max(EMULATION_WORST.get(f"{fmt}:{n}", 0.0), w)
+
+
+# ---- the ends of the logit range (tests/logit_range.py): q^.k^ near +-groups, duplicate keys, zero rows -----------
+# (groups, scale): fp16 only where p = exp(scale q.k - shift) fits its range; bf16 also at large scale * groups
+LOGIT_RANGE_GS = {"bf16": [(1, 8), (1, 10), (2, 5), (8, 1), (4, 8), (1, 32), (2, 16)],
+                  "f16": [(1, 8), (1, 10), (2, 5), (8, 1)]}
+DTYPES = {"bf16": torch.bfloat16, "f16": torch.float16}
+
+
+def _emulate_family(family, fmt, groups, scale, causal, seed, shape=(1, 4, 2, 300, 64)):
+    B, H, Hk, N, D = shape
+    q, k, v, do, _ = logit_range.dense(family, B, H, Hk, N, N, D, DTYPES[fmt], causal=causal, seed=seed)
+    q, k, v, do = (t.double().numpy() for t in (q, k, v, do))
+    kw = dict(groups=groups, scale=scale, causal=causal)
+    with np.errstate(over="ignore"):                 # fp16 gradients of a zero row: x 1e12, out of range
+        got = emulate(q, k, v, do, fmt, **kw)
+    ref, bound = attention_bounds(q, k, v, do, round_qk=fmt, fmt=fmt, shift=kernel_shift(fmt, scale, groups), **kw)
+    return got, ref, bound
+
+
+@pytest.mark.parametrize("fmt,groups,scale", [(f, g, s) for f in LOGIT_RANGE_GS for g, s in LOGIT_RANGE_GS[f]])
+@pytest.mark.parametrize("family", logit_range.FAMILIES)
+def test_emulated_logit_range_within_bound(family, fmt, groups, scale):
+    """Every input family at every (groups, scale) of its dtype, causal and not: the emulation stays within C / 2,
+    the pin of the Gaussian cases.  fp16 gradients of the zero rows are out of range by construction (x 1e12)."""
+    for causal in (False, True):
+        got, ref, bound = _emulate_family(family, fmt, groups, scale, causal, seed=groups + scale + causal)
+        names = ("o",) if (family == "zero_rows" and fmt == "f16") else ("o", "dq", "dk", "dv")
+        for n, g in zip(names, got):
+            w = check_bound(n, torch.from_numpy(g), ref, bound, fmt, c=C / 2) * C / 2
+            EMULATION_WORST[f"{fmt}:{n}"] = max(EMULATION_WORST.get(f"{fmt}:{n}", 0.0), w)
+
+
+def test_fp16_overflow_helper_matches_the_largest_p():
+    """`_fp16_overflows` is exactly `exp(scale * groups - shift) > 65504` (the largest p, at q.k = groups) for fp16 with
+    l2norm, and never true for bf16, float32 or without l2norm."""
+    m = pytest.importorskip("flash_cosine_sim_attention_b200.flash_cosine_sim_attention")
+    for groups in (1, 2, 3, 4, 8, 16, 32):
+        for scale in (0.5, 1, 1.25, 2, 3, 4, 5, 6, 7, 8, 10, 11, 12, 16, 24, 32):
+            shift = m._choose_shift(torch.float16, scale, groups, True)
+            with np.errstate(over="ignore"):
+                want = np.exp(np.float64(scale * groups - shift)) > 65504
+            assert m._fp16_overflows(torch.float16, scale, groups, True) == want, (groups, scale)
+            for dt, l2 in ((torch.bfloat16, True), (torch.float32, True), (torch.float16, False)):
+                assert not m._fp16_overflows(dt, scale, groups, l2)
+    for groups, scale, want in ((4, 8, True), (3, 8, True), (2, 16, True), (2, 8, False), (8, 1, False),
+                                (1, 10, False), (1, 32, False)):
+        assert m._fp16_overflows(torch.float16, scale, groups, True) == want, (groups, scale)
+
+
+def test_emulated_fp16_overflow_breaks_the_bound(capsys):
+    """Where `_fp16_overflows` warns, the kernels' arithmetic is wrong, not imprecise: at (1, 1, 256, 64), groups 4,
+    scale 8, queries that are noisy copies of keys (sigma 0.3), every row's best p exceeds 65504 and the emulated o
+    misses the bound by orders of magnitude; bf16 on the same input stays within C / 2."""
+    out = {}
+    for fmt in ("f16", "bf16"):
+        got, ref, bound = _emulate_family("aligned0.3", fmt, 4, 8, False, seed=0, shape=(1, 1, 1, 256, 64))
+        o = torch.from_numpy(got[0]).double()
+        rel = float(((o - ref["o"]).norm(dim=-1) / ref["o"].norm(dim=-1)).max())
+        worst = float(torch.nan_to_num(ratio(o, ref["o"], bound["o"], fmt), posinf=1e300).max()) / C
+        out[fmt] = (rel, worst)
+    assert out["f16"][1] > 10 and out["bf16"][1] <= 0.5, out
+    with capsys.disabled():
+        print(f"\n  emulated fp16 overflow (groups 4, scale 8, aligned0.3): o relative error {out['f16'][0]:.3g}, "
+              f"worst err / (C u M) {out['f16'][1]:.3g}; bf16 {out['bf16'][1]:.3g}", end="")
 
 
 # ---- planted errors: kernel-shaped mistakes, built from float64 results, that the bound must reject --------------
