@@ -37,7 +37,9 @@ class FusedPrimitives:
     def forward(self, q, k, v, causal):
         from .flash_cosine_sim_attention import _ext
         o, inv_l = _ext().forward_ex(q, k, v, None, None, False, None, self.scale, self.shift, causal, 0, True, True)[:2]
-        return o, inv_l
+        # the extension returns inv_l as (B, H, N), H = 1 for merged (B*H, N, D) inputs; the merge broadcasts it
+        # against o, so it takes q's row shape (the backward reads only its pointer)
+        return o, inv_l.view(q.shape[:-1])
 
     def backward(self, do, o, inv_l, q, k, v, causal):
         # o: the merged output in fp32; dq, dk, dv come back in fp32 (out_f32) so that the sums over blocks and
@@ -146,15 +148,31 @@ class _ContextParallel(Function):
 
 def context_parallel_cosine_sim_attention(q, k, v, *, scale=8, groups=1, causal=False, l2norm_qk=True, group=None,
                                           primitives=None):
-    """q, k, v: THIS RANK'S contiguous block of the sequence, (batch, heads, n_local, dim), equal n_local on every
-    rank (block r = positions [r n_local, (r+1) n_local)).  Returns this rank's block of the output; gradients flow
-    to the local q, k, v.  Key-padding masks / attn_bias are not supported on this path."""
-    from .flash_cosine_sim_attention import _choose_shift, l2norm_tensors
+    """q, k, v: THIS RANK'S contiguous block of the sequence, (batch, heads, n_local, dim) or merged
+    (batch*heads, n_local, dim), equal n_local on every rank (block r = positions [r n_local, (r+1) n_local)).
+    Returns this rank's block of the output; gradients flow to the local q, k, v.  Key-padding masks / attn_bias are
+    not supported on this path.
+
+    With the fused kernels (primitives=None) the inputs must be float16 or bfloat16 CUDA tensors with head dim 64 or
+    128; anything else is rejected here, before any collective.  float16 warns where exp(scale*q.k - shift) can exceed
+    its range (as `flash_cosine_sim_attention` does)."""
+    from .flash_cosine_sim_attention import (_KERNEL_DTYPES, _KERNEL_HEAD_DIMS, _choose_shift, _warn_fp16_overflow,
+                                             l2norm_tensors)
     assert dist.is_initialized(), "context parallelism needs an initialised process group"
     assert q.shape[-2] == k.shape[-2] == v.shape[-2], "every rank holds the same number of queries and keys"
     assert k.shape[:-2] == q.shape[:-2] and v.shape[:-2] == q.shape[:-2], (
         "context parallelism needs keys/values with as many heads as the queries (grouped-query or single-head "
         "keys/values are not supported on this path: expand them with repeat_interleave first)")
+    if primitives is None:
+        if q.dtype not in _KERNEL_DTYPES or k.dtype != q.dtype or v.dtype != q.dtype:
+            raise TypeError(f"context_parallel_cosine_sim_attention: dtype {q.dtype} (k {k.dtype}, v {v.dtype}) is not "
+                            "supported: q, k, v must all be float16 or all bfloat16 (no float32 on this path)")
+        if q.shape[-1] not in _KERNEL_HEAD_DIMS:
+            raise NotImplementedError(f"context_parallel_cosine_sim_attention: head dim {q.shape[-1]} is not "
+                                      "supported: 64 or 128 only")
+        if not (q.is_cuda and k.is_cuda and v.is_cuda):
+            raise RuntimeError("context_parallel_cosine_sim_attention: CUDA tensors required (the fused kernels)")
+        _warn_fp16_overflow(q.dtype, scale, groups, l2norm_qk)
     if l2norm_qk:
         q, k = l2norm_tensors(q, k, groups=groups)        # per row: local, differentiable (fused kernels on CUDA)
     if primitives is None:

@@ -49,7 +49,12 @@ def main():
     # rows of the other ranks get no gradient on this rank
     assert float(qs.grad[:lo].abs().sum() + qs.grad[hi:].abs().sum()) == 0.0
     worst = max(worst, *e)
-    assert max(e) < 1e-6, f"batch split: {e}"          # same kernels on the same data: bit-identical
+    # same kernels on the same data: o, dk and dv are bitwise equal; dq is summed by fp32 atomics in no fixed
+    # order (DESIGN 4.2), so it is held to the gradient tolerance
+    assert torch.equal(o, of), f"batch split: o differs ({e[0]:.3g})"
+    assert torch.equal(ks.grad[lo:hi], kf.grad[lo:hi]) and torch.equal(vs.grad[lo:hi], vf.grad[lo:hi]), (
+        f"batch split: dk / dv differ ({e[2]:.3g}, {e[3]:.3g})")
+    assert e[1] <= 2e-2, f"batch split: dq {e[1]:.3g}"    # TOL_GRAD of bf16 (tests/test_gpu_parity.py)
 
     # ---- 2. heads split, single-head keys/values: dk, dv all-reduced ---------------------------------
     B, H, N, D = 1, 2 * world, 256, 64

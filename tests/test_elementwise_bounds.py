@@ -119,18 +119,22 @@ def emulate(q, k, v, do, fmt, mask=None, attn_bias=None, scale=8, groups=1, caus
             if db is not None:
                 db[b if attn_bias_batch_dim else h] += ds
 
-    def l2bwd(dy, y, n):
-        g = y.reshape(*y.shape[:-1], groups, -1)
-        d = dy.reshape(g.shape)
-        rn = f32(1) / np.maximum(n, 1e-12).astype(f32)
-        return ((d - g * (g * d).sum(-1, keepdims=True)) * rn[..., None]).reshape(y.shape)
-    dq, dk = (l2bwd(dqn, qn, nq), l2bwd(dkn, kn, nk)) if l2norm_qk else (dqn, dkn)
+    dq, dk = (_l2bwd(dqn, qn, nq, groups), _l2bwd(dkn, kn, nk, groups)) if l2norm_qk else (dqn, dkn)
     out = [T(o), T(dq), T(dk), T(dv)] + ([] if db is None else [T(db)])
     if merged:
         out[0], out[1], out[2], out[3] = out[0][:, 0], out[1][:, 0], out[2][:, 0], out[3][:, 0]
     elif single:
         out[2], out[3] = out[2][:, 0], out[3][:, 0]
     return out
+
+
+def _l2bwd(dy, y, n, groups):
+    """The l2norm backward in float32 on the stored y = x^ with 1/||x|| from the 1e-12 clamp."""
+    f32 = np.float32
+    g = y.reshape(*y.shape[:-1], groups, -1)
+    d = dy.reshape(g.shape)
+    rn = f32(1) / np.maximum(n, 1e-12).astype(f32)
+    return ((d - g * (g * d).sum(-1, keepdims=True)) * rn[..., None]).reshape(y.shape)
 
 
 EMULATION_WORST = {}
@@ -219,6 +223,84 @@ def test_emulated_fp16_overflow_breaks_the_bound(capsys):
     with capsys.disabled():
         print(f"\n  emulated fp16 overflow (groups 4, scale 8, aligned0.3): o relative error {out['f16'][0]:.3g}, "
               f"worst err / (C u M) {out['f16'][1]:.3g}; bf16 {out['bf16'][1]:.3g}", end="")
+
+
+# ---- context parallelism (context_parallel.py): key blocks, an additive merge, the backward per block --------------
+def emulate_context_parallel(q, k, v, do, fmt, world, scale=8, groups=1, causal=False):
+    """What the fused context-parallel path computes, in float32 with every 16-bit rounding in its place.  The sequence
+    is cut into `world` blocks of queries and keys.  Query block r sees key blocks s <= r when causal (block r itself
+    with the causal diagonal), all of them otherwise.  q^, k^ are stored in T (l2norm_tensors).  Per (r, s) the forward
+    forms p = exp(scale S - shift) in fp32, the fp32 row sum l_s and o_s = (p~ V_s) / l_s, with p~ = p rounded to T (as
+    in `emulate`) and o_s left in fp32 (out_f32).  The merge is o = sum_s o_s l_s / sum_s l_s in fp32, stored to T.  The
+    backward per (r, s) uses the GLOBAL 1/l and the fp32 o (delta from it): P -> T before dV, dS -> T before dq^ and
+    dk^.  dq^ is summed over the blocks in fp32, dk^ and dv over the query blocks in fp32 (the reduce-scatter), each
+    rounded to T once; dq^ and dk^ then go through the separate l2norm backward, output -> T.
+    q, k, v, do: (B, H, N, D) arrays of 16-bit values, N a multiple of `world`.  Returns [o, dq, dk, dv]."""
+    f32 = np.float32
+    T = lambda x: oracle.round_to(x, fmt).astype(f32)
+    Tp = (lambda x: T(np.minimum(x, f32(65504)))) if fmt == "f16" else T
+    shift = f32(kernel_shift(fmt, scale, groups))
+    B, H, N, D = q.shape
+    n = N // world
+    (qn, nq), (kn, nk) = oracle.l2norm(q, groups), oracle.l2norm(k, groups)
+    qn, kn = T(qn), T(kn)
+    v, do = v.astype(f32), do.astype(f32)
+    o, dqn, dkn, dv = (np.zeros(q.shape, f32) for _ in range(4))
+    blk = [slice(r * n, (r + 1) * n) for r in range(world)]
+    diag = np.tril(np.ones((n, n), bool))
+    for b in range(B):
+        for h in range(H):
+            for r in range(world):
+                qr, dor = qn[b, h, blk[r]], do[b, h, blk[r]]
+                seen = [s for s in range(world) if not (causal and s > r)]
+                p, num, den = {}, f32(0), f32(0)
+                for s in seen:
+                    vis = diag if (causal and s == r) else np.ones((n, n), bool)
+                    p[s] = np.where(vis, np.exp(f32(scale) * (qr @ kn[b, h, blk[s]].T) - shift), f32(0))
+                    inv_l_s = f32(1) / np.maximum(p[s].sum(-1, dtype=f32), f32(1e-37))
+                    o_s = (Tp(p[s]) @ v[b, h, blk[s]]) * inv_l_s[:, None]
+                    den_s = f32(1) / inv_l_s
+                    num, den = num + o_s * den_s[:, None], den + den_s
+                inv_l = f32(1) / den
+                o_wide = num * inv_l[:, None]
+                o[b, h, blk[r]] = o_wide
+                delta = (dor * o_wide).sum(-1, dtype=f32, keepdims=True)
+                for s in seen:
+                    P = p[s] * inv_l[:, None]
+                    dv[b, h, blk[s]] += T(P).T @ dor
+                    ds = T(P * (dor @ v[b, h, blk[s]].T - delta))
+                    dqn[b, h, blk[r]] += f32(scale) * (ds @ kn[b, h, blk[s]])
+                    dkn[b, h, blk[s]] += f32(scale) * (ds.T @ qr)
+    dq, dk = _l2bwd(T(dqn), qn, nq, groups), _l2bwd(T(dkn), kn, nk, groups)
+    return [T(o), T(dq), T(dk), T(dv)]
+
+
+# the (groups, scale) of the GPU grid (tests/test_gpu_context_parallel.py) at both ends: fp16 at (2, 8) is the
+# shift = scale regime below the overflow threshold
+CP_GS = {"bf16": [(1, 8), (4, 8), (2, 16)], "f16": [(1, 8), (2, 5), (2, 8)]}
+
+
+@pytest.mark.parametrize("fmt,groups,scale", [(f, g, s) for f in CP_GS for g, s in CP_GS[f]])
+@pytest.mark.parametrize("family", ["gaussian", "aligned0", "one_peak"])
+def test_emulated_context_parallel_within_bound(family, fmt, groups, scale):
+    """W = 3 blocks of 100 rows of (1, 2, 300, 64), causal and not: the context-parallel arrangement makes every 16-bit
+    rounding of the dense kernels and otherwise fewer, plus one rounding of dq^ and dk^ before the l2norm backward (as
+    on the BIAS path).  Its worst err / (u M) against the whole-sequence reference stays within C / 2, the pin of the
+    dense emulation, so the GPU tests hold context parallelism to the same C."""
+    for causal in (False, True):
+        seed = groups + scale + causal
+        if family == "gaussian":
+            g = torch.Generator().manual_seed(seed)
+            q, k, v, do = (torch.randn(1, 2, 300, 64, generator=g).to(DTYPES[fmt]) for _ in range(4))
+        else:
+            q, k, v, do, _ = logit_range.dense(family, 1, 2, 2, 300, 300, 64, DTYPES[fmt], causal=causal, seed=seed)
+        q, k, v, do = (t.double().numpy() for t in (q, k, v, do))
+        got = emulate_context_parallel(q, k, v, do, fmt, 3, scale=scale, groups=groups, causal=causal)
+        ref, bound = attention_bounds(q, k, v, do, round_qk=fmt, fmt=fmt, shift=kernel_shift(fmt, scale, groups),
+                                      groups=groups, scale=scale, causal=causal)
+        for n, t in zip(("o", "dq", "dk", "dv"), got):
+            w = check_bound(n, torch.from_numpy(t), ref, bound, fmt, c=C / 2) * C / 2
+            EMULATION_WORST[f"{fmt}:cp {n}"] = max(EMULATION_WORST.get(f"{fmt}:cp {n}", 0.0), w)
 
 
 # ---- planted errors: kernel-shaped mistakes, built from float64 results, that the bound must reject --------------

@@ -27,6 +27,7 @@ def test_plan_prefers_batch():
     assert plan(4, 8, 8) == ("heads", 8)
     assert plan(4, 8, 2) == ("batch", 4)
     assert plan(3, 5, 2) == ("batch", 3)         # nothing divides: ragged batch split
+    assert plan(3, 2, 2) == ("heads", 2)         # the batch does not divide, the heads do
 
 
 def _free_port():
@@ -75,12 +76,12 @@ CASES = [
     ((4, 2, 9, 64), (4, 2, 11, 64), dict(causal=True), False),          # batch split
     ((1, 4, 9, 64), (1, 4, 9, 64), dict(groups=2), False),              # heads split, per-head kv
     ((1, 4, 9, 64), (1, 12, 64), dict(), True),                         # heads split, shared kv (all-reduce of dk, dv)
-    ((3, 2, 5, 64), (3, 2, 5, 64), dict(scale=2.0), False),             # ragged batch split
+    ((3, 2, 5, 64), (3, 2, 5, 64), dict(scale=2.0), False),             # heads split at B = 3 (plan(3, 2, 2))
     ((6, 7, 64), (6, 7, 64), dict(causal=True), False),                 # merged batch-heads
 ]
 
 
-@pytest.mark.parametrize("case", CASES, ids=["batch", "heads", "heads_shared_kv", "ragged_batch", "merged"])
+@pytest.mark.parametrize("case", CASES, ids=["batch", "heads", "heads_shared_kv", "heads_batch3", "merged"])
 def test_sharded_equals_unsharded_world2(case):
     world = 2
     port = _free_port()
