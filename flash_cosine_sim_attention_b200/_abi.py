@@ -68,7 +68,7 @@ class FcsaProblem(Structure):
         ("key_mask", c_void_p),
         ("key_mask_stride", c_int64),
         ("out_f32", c_int32),
-        ("reserved_", c_int32),
+        ("window", c_int32),
     ]
 
 

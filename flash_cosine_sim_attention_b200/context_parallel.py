@@ -147,7 +147,7 @@ class _ContextParallel(Function):
 
 
 def context_parallel_cosine_sim_attention(q, k, v, *, scale=8, groups=1, causal=False, l2norm_qk=True, group=None,
-                                          primitives=None):
+                                          primitives=None, window=None):
     """q, k, v: THIS RANK'S contiguous block of the sequence, (batch, heads, n_local, dim) or merged
     (batch*heads, n_local, dim), equal n_local on every rank (block r = positions [r n_local, (r+1) n_local)).
     Returns this rank's block of the output; gradients flow to the local q, k, v.  Key-padding masks / attn_bias are
@@ -155,9 +155,13 @@ def context_parallel_cosine_sim_attention(q, k, v, *, scale=8, groups=1, causal=
 
     With the fused kernels (primitives=None) the inputs must be float16 or bfloat16 CUDA tensors with head dim 64 or
     128; anything else is rejected here, before any collective.  float16 warns where exp(scale*q.k - shift) can exceed
-    its range (as `flash_cosine_sim_attention` does)."""
+    its range (as `flash_cosine_sim_attention` does).  Sliding-window attention (`window`) is not supported on this
+    path and is rejected before any collective."""
     from .flash_cosine_sim_attention import (_KERNEL_DTYPES, _KERNEL_HEAD_DIMS, _choose_shift, _warn_fp16_overflow,
                                              l2norm_tensors)
+    if window is not None:
+        raise NotImplementedError("context_parallel_cosine_sim_attention: window (sliding-window attention) is not "
+                                  "supported with context parallelism")
     assert dist.is_initialized(), "context parallelism needs an initialised process group"
     assert q.shape[-2] == k.shape[-2] == v.shape[-2], "every rank holds the same number of queries and keys"
     assert k.shape[:-2] == q.shape[:-2] and v.shape[:-2] == q.shape[:-2], (

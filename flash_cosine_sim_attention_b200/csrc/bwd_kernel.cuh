@@ -371,18 +371,24 @@ __device__ __forceinline__ void l2norm_bwd_key_row(float (&g)[D / 4], const BwdA
   }
 }
 
+template <bool VARLEN, bool WINDOW>
+using BwdArgsOf = std::conditional_t<WINDOW, Windowed<std::conditional_t<VARLEN, BwdVarlenArgs, BwdArgs>>,
+                                     std::conditional_t<VARLEN, BwdVarlenArgs, BwdArgs>>;
+
 // HEAD_LOOP: the CTA works through several query heads (hpc > 1, grouped-query launches); otherwise hpc = 1 is a
 // compile-time constant and the loops below are those of one query head (MHA, MQA, BIAS and split groups of one head).
 // VARLEN: packed sequences (BwdVarlenArgs); `b` is then the sequence, and its lengths replace Nq / Nk.
-template <typename T, int D, bool BIAS = false, bool HEAD_LOOP = false, bool VARLEN = false>
+// WINDOW: sliding-window attention (Windowed<>::window = W): a key tile visits query tiles [i_lo, i_end) instead of
+// [i_lo, nqt), i_end being the tile after the last query row whose lower limit reaches key0 + 127.
+template <typename T, int D, bool BIAS = false, bool HEAD_LOOP = false, bool VARLEN = false, bool WINDOW = false>
 __global__ void __launch_bounds__(384, 1)
 fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                 const __grid_constant__ CUtensorMap tm_v, const __grid_constant__ CUtensorMap tm_do,
-                const __grid_constant__ CUtensorMap tm_dq,
-                const std::conditional_t<VARLEN, BwdVarlenArgs, BwdArgs> a) {
+                const __grid_constant__ CUtensorMap tm_dq, const BwdArgsOf<VARLEN, WINDOW> a) {
   static_assert(D == 64 || D == 128, "head dim 64 or 128");
   static_assert(!(BIAS && HEAD_LOOP), "BIAS launches have one query head per CTA");
   static_assert(!(BIAS && VARLEN), "packed sequences take no bias");
+  static_assert(!(BIAS && WINDOW), "a window takes no bias");
   using Cfg = BwdCfg<D>;
   constexpr bool STAGED = Cfg::kStaged;
   constexpr int QT = Cfg::QT;              // query rows per tile
@@ -462,7 +468,17 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     const int x = key0 - off - (QT - 1);
     i_lo = x <= 0 ? 0 : (x + QT - 1) / QT;
   }
-  const int NI = max(0, nqt - i_lo);          // number of query tiles to visit per query head
+  int W = 0, i_end = nqt;                     // the window; the query tile after the last one visited
+  if constexpr (WINDOW) {
+    W = a.window;
+    if (!a.causal) {                          // first query tile with a row whose band reaches key0
+      const int x = key0 - off - (QT - 1) - (W - 1);
+      i_lo = x <= 0 ? 0 : (x + QT - 1) / QT;
+    }
+    const int last_row = key0 + 127 - off + W - 1;   // the last query row whose lower limit is at most key0 + 127
+    i_end = last_row < 0 ? 0 : min(nqt, last_row / QT + 1);
+  }
+  const int NI = max(0, i_end - i_lo);        // number of query tiles to visit per query head
   const int NT = hpc * NI;                    // flat tile index i: head h0 + i / NI, query tile i_lo + i % NI
 
   if (wg == 0) {
@@ -483,7 +499,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         long long tile0 = ((long long)b * a.H + h) * a.nqt;     // the stats tile of query tile 0
         if constexpr (VARLEN) tile0 = (long long)h * a.ntile + qbase;
         const float* stats_h = a.stats + tile0 * 2 * QT;
-        for (int qt = i_lo; qt < nqt; ++qt, ++i) {
+        for (int qt = i_lo; qt < i_end; ++qt, ++i) {
           const int st = i % NST;
           mbar_wait(BAR(EMPTY + st), ((i / NST) & 1) ^ 1);
           mbar_expect_tx(BAR(FULL + st), 2 * Cfg::kQ + 8 * QT);
@@ -527,14 +543,24 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int kr = 16 * wl + r8;                // this thread's key rows inside the warpgroup's 64: kr, kr + 8
   const int cq = 2 * (lane & 3);              // first of the thread's two columns inside every 8-column block
   // key_lo[hf]: the first query row that sees key row kr + 8 hf (causal: key - (Nk - Nq), else 0), or Nq + QT when
-  // the key does not exist or is masked - one register per row for the masked elementwise stage
+  // the key does not exist or is masked - one register per row for the masked elementwise stage.  WINDOW: a key's
+  // visible query rows are [key + lo_off, key + hi_off], lo_off = -off (causal) or -off - W + 1, hi_off = W - 1 - off;
+  // one register each for both rows (the D = 64 consumers have none to spare)
   int key_g[2], key_lo[2];
+  int lo_off = 0, hi_off = 0;
+  if constexpr (WINDOW) {
+    lo_off = a.causal ? -off : -off - W + 1;
+    hi_off = W - 1 - off;
+  }
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     key_g[hf] = key0 + 64 * w + kr + 8 * hf;
     bool ok = key_g[hf] < Nk;
     if (a.has_mask && ok) ok = a.mask[(long long)b * a.mask_sb + key_g[hf]] != 0;
     key_lo[hf] = !ok ? Nq + QT : (a.causal ? key_g[hf] - off : 0);
+    if constexpr (WINDOW) {
+      if (ok) key_lo[hf] = key_g[hf] + lo_off;
+    }
   }
   // the warpgroup's keys are all real and unmasked: only query tiles crossing the causal diagonal or the end
   // of the sequence need per-element selects
@@ -566,12 +592,13 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   // Element pair e = 2 j + hf: key row kr + 8 hf, query columns 8 j + cq + {0, 1}.
   auto elementwise = [&](const bool MASKED, const float (&s)[QT / 2], const float (&dp)[QT / 2],
                          uint32_t (&pf)[QT / 4], uint32_t (&dsf)[QT / 4], int row0, uint32_t stc3, uint32_t dsbuf) {
-    int hi = QT - 1, lo[2] = {0, 0};
+    int hi = QT - 1, lo[2] = {0, 0}, hi_k[2];
     if (MASKED) {
       hi = min(QT - 1, Nq - 1 - row0);                        // last valid query column of the tile
 #pragma unroll
       for (int hf = 0; hf < 2; ++hf) {                        // first visible query column of each key row
         lo[hf] = max(0, key_lo[hf] - row0);
+        if constexpr (WINDOW) hi_k[hf] = min(hi, key_g[hf] + hi_off - row0);   // ... and the last, with the window
       }
     }
 #pragma unroll
@@ -603,7 +630,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           x0 = fmaf(bv.x, 1.4426950408889634f, x0);
           x1 = fmaf(bv.y, 1.4426950408889634f, x1);
         }
-        const bool v0 = !MASKED || (cc >= lo[hf] && cc <= hi), v1 = !MASKED || (cc + 1 >= lo[hf] && cc + 1 <= hi);
+        const int hk_ = WINDOW ? hi_k[hf] : hi;
+        const bool v0 = !MASKED || (cc >= lo[hf] && cc <= hk_), v1 = !MASKED || (cc + 1 >= lo[hf] && cc + 1 <= hk_);
         const float p0 = v0 ? ex2_approx(x0) : 0.f;
         const float p1 = v1 ? ex2_approx(x1) : 0.f;
         const float ds0 = p0 * (dp[2 * e] + ndl.x), ds1 = p1 * (dp[2 * e + 1] + ndl.y);
@@ -624,7 +652,11 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   auto elementwise_tile = [&](const float (&s)[QT / 2], const float (&dp)[QT / 2], uint32_t (&pf)[QT / 4],
                               uint32_t (&dsf)[QT / 4], int row0, uint32_t stc3, uint32_t dsbuf) {
     // interior tile: every key of the warpgroup sees every query row (no causal diagonal, no ragged end)
-    const bool interior = keys_full && row0 + QT <= Nq && (!a.causal || key0 + 64 * w + 63 - off <= row0);
+    bool interior = keys_full && row0 + QT <= Nq && (!a.causal || key0 + 64 * w + 63 - off <= row0);
+    // (window: the tile's rows lie between the last key's first visible row and the first key's last one)
+    if constexpr (WINDOW)
+      interior = keys_full && row0 + QT <= Nq && key0 + 64 * w + 63 + lo_off <= row0 &&
+                 row0 + QT - 1 <= key0 + 64 * w + hi_off;
     if (!BIAS && interior) elementwise(false, s, dp, pf, dsf, row0, stc3, dsbuf);
     else elementwise(true, s, dp, pf, dsf, row0, stc3, dsbuf);
     fence_proxy_async_smem();
@@ -727,8 +759,12 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     if (NT > 0) {
       mbar_wait(BAR(FULL), 0);
       issue_s_dp(s, dp, sQ, sDO);
-      // i runs over the flat (head, query tile) sequence; row0 restarts at i_lo * QT with every head
-      for (int i = 0, row0 = i_lo * QT; i < NT; ++i, row0 = (!HEAD_LOOP || row0 + QT < (VARLEN ? Nq : a.nqt * QT)) ? row0 + QT : i_lo * QT) {
+      // i runs over the flat (head, query tile) sequence; row0 restarts at i_lo * QT with every head, after the last
+      // tile (window: after tile i_end - 1, i.e. once row0 + QT passes key0 + 127 + hi_off, the last row seeing a key)
+      auto next_in_head = [&](int row0) {
+        return row0 + QT < (VARLEN ? Nq : a.nqt * QT) && (!WINDOW || row0 + QT <= key0 + 127 + hi_off);
+      };
+      for (int i = 0, row0 = i_lo * QT; i < NT; ++i, row0 = (!HEAD_LOOP || next_in_head(row0)) ? row0 + QT : i_lo * QT) {
         const int st = i % NST;
         const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
         wgmma_wait<0>();                        // S^T, dP^T of tile i; dV, dK of tile i - 1; dQ of tile i - 2
@@ -1026,6 +1062,7 @@ __global__ void __launch_bounds__(256) bwd_kv_finish_kernel(const KvFinishArgs a
 struct BwdHostArgs {
   bool dtype_bf16;
   int B, H, kv_heads, Nq, Nk, D, causal;
+  int window = 0;                   // sliding window W (0 = none; never with a bias)
   float scale, shift;
   const uint8_t* mask; long long mask_sb;
   fcsa_tensor q, k, v, o, d_o, dq, dk, dv;
@@ -1142,7 +1179,9 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
       *err = "cuTensorMapEncodeTiled failed (backward dq accumulator)";
       return FCSA_ERR_CUDA;
     }
-    std::conditional_t<VARLEN, BwdVarlenArgs, BwdArgs> a;
+    // (the window's arguments extend the kernel's; the unwindowed launches pass the base)
+    BwdArgsOf<VARLEN, true> a;
+    a.window = h.window;
     a.B = h.B; a.H = h.H; a.Nq = h.Nq; a.Nk = h.Nk; a.kv_heads = h.kv_heads; a.causal = h.causal;
     a.has_mask = h.mask ? 1 : 0; a.nqt = w.nqt;
     if constexpr (VARLEN) {
@@ -1160,15 +1199,24 @@ int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, con
     a.out_f32 = h.out_f32 ? 1 : 0;
     a.k_rnorm = h.k_rnorm; a.groups = h.groups;
     constexpr bool kLoop = !BIAS;
+    const std::conditional_t<VARLEN, BwdVarlenArgs, BwdArgs>& base = a;
+    const bool win = !BIAS && h.window > 0;
     auto kern = a.hpc > 1 ? fcsa_bwd_kernel<T, D, BIAS, kLoop, VARLEN> : fcsa_bwd_kernel<T, D, BIAS, false, VARLEN>;
     e = a.hpc > 1 ? ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS, kLoop, VARLEN>>(Cfg::kSmem)
                   : ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS, false, VARLEN>>(Cfg::kSmem);
+    auto wkern = fcsa_bwd_kernel<T, D, false, false, VARLEN, !BIAS>;    // (BIAS: never launched)
+    if (win) {
+      wkern = a.hpc > 1 ? fcsa_bwd_kernel<T, D, false, kLoop, VARLEN, !BIAS> : wkern;
+      e = a.hpc > 1 ? ensure_dynamic_smem<fcsa_bwd_kernel<T, D, false, kLoop, VARLEN, !BIAS>>(Cfg::kSmem)
+                    : ensure_dynamic_smem<fcsa_bwd_kernel<T, D, false, false, VARLEN, !BIAS>>(Cfg::kSmem);
+    }
     if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(bwd)"; *ce = e; return FCSA_ERR_CUDA; }
     // one CTA per (key tile, batch, kv head, slice of its group); packed sequences: key tiles of the longest one
     const long long items = (long long)((h.Nk + 127) / 128) * h.B * h.kv_heads * split;
     if (items > 0x7FFFFFFFLL) { *err = "problem too large for one launch"; return FCSA_ERR_INVALID; }
     if (h.ev_start) cudaEventRecord(h.ev_start, stream);
-    e = launch_pdl(kern, dim3((unsigned)items), dim3(Cfg::kThreads), Cfg::kSmem, stream, tq, tk, tv, tdo, tdq, a);
+    e = win ? launch_pdl(wkern, dim3((unsigned)items), dim3(Cfg::kThreads), Cfg::kSmem, stream, tq, tk, tv, tdo, tdq, a)
+            : launch_pdl(kern, dim3((unsigned)items), dim3(Cfg::kThreads), Cfg::kSmem, stream, tq, tk, tv, tdo, tdq, base);
     if (h.ev_stop) cudaEventRecord(h.ev_stop, stream);
     if (e != cudaSuccess) { *err = "backward kernel launch"; *ce = e; return FCSA_ERR_CUDA; }
     ++*launches;

@@ -53,7 +53,7 @@ struct DecodeCfg {
 };
 
 // Splits per work item: 1 when the items alone fill the SMs, otherwise the fewest that do, at most one per key tile
-// of the capacity.  (tests/test_decode_host.py mirrors this rule.)
+// of the capacity.  (tests/test_decode_host.py mirrors this rule.)  With a window, `cap` is decode_window_keys.
 inline int decode_split(long long items, int cap, int sm_count) {
   if (items >= sm_count) return 1;
   const long long want = (sm_count + items - 1) / items;
@@ -61,10 +61,21 @@ inline int decode_split(long long items, int cap, int sm_count) {
   return (int)(want < tiles ? want : tiles);
 }
 
-template <typename T, int D>
+// A bound on the keys whose tiles one row block can see under a window W: its rows span at most 64 queries, so its
+// keys lie in a range of 64 + W - 2 (causal) or 64 + 2 W - 3 keys, which touches at most ceil(range / 128) + 1 tiles.
+// The split rule then bounds a block's tiles by the window instead of the capacity.
+inline int decode_window_keys(int cap, int window, bool causal) {
+  const long long range = 64LL + (causal ? 1 : 2) * (long long)window;
+  const long long keys = range + 128;
+  return (int)(keys < cap ? keys : cap);
+}
+
+// WINDOW: sliding-window attention (Windowed<DecodeArgs>::window = W).  A row block's visible tiles start at the tile of
+// its smallest lower limit; the split cuts [t_lo, t_hi) into n_split chunks.
+template <typename T, int D, bool WINDOW = false>
 __global__ void __launch_bounds__(256, DecodeCfg<D>::kCtasPerSm)
 fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_constant__ CUtensorMap tm_v,
-                   const DecodeArgs a) {
+                   const std::conditional_t<WINDOW, Windowed<DecodeArgs>, DecodeArgs> a) {
   using Cfg = DecodeCfg<D>;
   constexpr int S = Cfg::kStages, TILE = Cfg::kTile, DCH = D / 64;
 
@@ -113,8 +124,16 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
     const int last_col = r_last / a.G + off;
     nt = last_col < 0 ? 0 : min(nt, (last_col >> 7) + 1);
   }
-  const int j0 = (int)((long long)nt * split / a.n_split);
-  const int j1 = (int)((long long)nt * (split + 1) / a.n_split);
+  int W = 0, t_lo = 0;                        // the window and the block's first visible tile
+  if constexpr (WINDOW) {
+    W = a.window;
+    const int last_col = r_last / a.G + off + (a.causal ? 0 : W - 1);
+    nt = last_col < 0 ? 0 : min((Tb + 127) >> 7, (last_col >> 7) + 1);
+    const int first_col = r0 / a.G + off - W + 1;
+    t_lo = first_col <= 0 ? 0 : min(first_col >> 7, nt);
+  }
+  const int j0 = t_lo + (int)((long long)(nt - t_lo) * split / a.n_split);
+  const int j1 = t_lo + (int)((long long)(nt - t_lo) * (split + 1) / a.n_split);
 
   if (wg == 0) {
     // =============================== TMA producer ===============================
@@ -174,6 +193,15 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
     const int r = r0 + row_a + 8 * hf;
     lim[hf] = r >= a.R ? -1 : (a.causal ? min(Tb - 1, r / a.G + off) : Tb - 1);
   }
+  int lo[2] = {0, 0};                         // WINDOW: first visible column of each row, and the band's upper side
+  if constexpr (WINDOW) {
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) {
+      const int r = r0 + row_a + 8 * hf;
+      lo[hf] = r / a.G + off - W + 1;
+      if (!a.causal && r < a.R) lim[hf] = min(Tb - 1, r / a.G + off + W - 1);
+    }
+  }
   const int first_lim = r0 / a.G + off;       // the block's smallest causal limit
   const float c1 = a.c1, nc2 = -a.c2;
 
@@ -203,7 +231,9 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
 
     // ---- P = exp2(S*c1 - c2), masked (a select: cache rows past T_b may hold anything); 16-bit P as A fragments --
     const int col0 = j * 128;
-    const bool need_mask = (col0 + 127 >= Tb) || (a.causal && col0 + 127 > first_lim);
+    bool need_mask = (col0 + 127 >= Tb) || (a.causal && col0 + 127 > first_lim);
+    if constexpr (WINDOW)      // a column below the block's largest lower limit, or past its smallest upper one
+      need_mask = need_mask || col0 < r_last / a.G + off - W + 1 || col0 + 127 > first_lim + W - 1;
     uint32_t pf[32];
     auto exp_tile = [&](auto masked_tag) {
       constexpr bool MASKED = decltype(masked_tag)::value;
@@ -214,8 +244,13 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
         float p0 = ex2_approx(fmaf(sacc[2 * i], c1, nc2));
         float p1 = ex2_approx(fmaf(sacc[2 * i + 1], c1, nc2));
         if constexpr (MASKED) {
-          p0 = col <= lim[hf] ? p0 : 0.f;
-          p1 = col + 1 <= lim[hf] ? p1 : 0.f;
+          if constexpr (WINDOW) {
+            p0 = col <= lim[hf] && col >= lo[hf] ? p0 : 0.f;
+            p1 = col + 1 <= lim[hf] && col + 1 >= lo[hf] ? p1 : 0.f;
+          } else {
+            p0 = col <= lim[hf] ? p0 : 0.f;
+            p1 = col + 1 <= lim[hf] ? p1 : 0.f;
+          }
         }
         l[hf] += p0 + p1;
         pf[i] = pack2<T>(p0, p1);

@@ -67,11 +67,19 @@ int check_problem(const fcsa_problem* p) {
                 p->heads);
   if (p->causal && p->key_mask)
     return fail(FCSA_ERR_INVALID, "mask should not be supplied if causality is needed");
+  if (p->window < 0) return fail(FCSA_ERR_INVALID, "window %d < 0 (0 = no window)", p->window);
   return FCSA_OK;
+}
+
+// The window the kernels apply: 0 (the unwindowed kernels) when there is none, or when it is at least seq_q + seq_k and
+// so hides no key (seq_q / seq_k bound every length the problem covers: varlen maxima, the decode capacity).
+int kernel_window(const fcsa_problem* p) {
+  return (long long)p->window >= (long long)p->seq_q + p->seq_k ? 0 : p->window;
 }
 
 int check_bias(const fcsa_problem* p, const fcsa_bias* bias) {
   if (!bias || !bias->ptr) return fail(FCSA_ERR_INVALID, "attn_bias: null");
+  if (p->window != 0) return fail(FCSA_ERR_INVALID, "attn_bias: no sliding window with a bias (window %d)", p->window);
   if (!aligned16(bias->ptr) || (bias->sn % 8) != 0 || (bias->sh % 8) != 0 || (bias->sb % 8) != 0)
     return fail(FCSA_ERR_INVALID, "attn_bias: rows must be 16-byte aligned (strides multiples of 8 elements)");
   if (bias->sn < ((p->seq_k + 7) / 8) * 8)
@@ -99,7 +107,9 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
                                       v->sh, v->sn, 128)))
     return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "v: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - make the tensor contiguous" : "cuTensorMapEncodeTiled failed", r);
 
-  std::conditional_t<VARLEN, fcsa::FwdVarlenArgs, fcsa::FwdArgs> a;
+  // (the window's arguments extend the kernel's; the unwindowed launch passes the base)
+  fcsa::FwdArgsOf<VARLEN, true> a;
+  a.window = kernel_window(p);
   if constexpr (VARLEN) {
     a.cu_q = vl->cu_seqlens_q; a.cu_k = vl->cu_seqlens_k; a.total_q = vl->total_q; a.total_k = vl->total_k;
   }
@@ -128,16 +138,30 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
   a.bias_sn = BIAS ? bias->sn : 0;
   a.bias_amax = BIAS ? bias->amax : nullptr;
 
-  auto kern = fcsa::fcsa_fwd_kernel<T, D, BIAS, VARLEN>;
+  const bool win = !BIAS && a.window > 0;
   {
-    cudaError_t e = fcsa::ensure_dynamic_smem<fcsa::fcsa_fwd_kernel<T, D, BIAS, VARLEN>>(Cfg::kSmem);
+    cudaError_t e;
+    if constexpr (BIAS) e = fcsa::ensure_dynamic_smem<fcsa::fcsa_fwd_kernel<T, D, BIAS, VARLEN>>(Cfg::kSmem);
+    else e = win ? fcsa::ensure_dynamic_smem<fcsa::fcsa_fwd_kernel<T, D, false, VARLEN, true>>(Cfg::kSmem)
+                 : fcsa::ensure_dynamic_smem<fcsa::fcsa_fwd_kernel<T, D, false, VARLEN>>(Cfg::kSmem);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(fwd)");
   }
   // one CTA per (query block of 128 rows, batch, head); packed sequences: blocks of the longest sequence
   const long long grid = (long long)a.n_qblk * p->batch * p->heads;
   if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
   if (g_ev[0][0]) cudaEventRecord(g_ev[0][0], stream);
-  cudaError_t e = fcsa::launch_pdl(kern, dim3((unsigned)grid), dim3(Cfg::kThreads), Cfg::kSmem, stream, tq, tk, tv, a);
+  const std::conditional_t<VARLEN, fcsa::FwdVarlenArgs, fcsa::FwdArgs>& base = a;
+  cudaError_t e;
+  if constexpr (BIAS) {
+    e = fcsa::launch_pdl(fcsa::fcsa_fwd_kernel<T, D, BIAS, VARLEN>, dim3((unsigned)grid), dim3(Cfg::kThreads),
+                         Cfg::kSmem, stream, tq, tk, tv, base);
+  } else if (win) {
+    e = fcsa::launch_pdl(fcsa::fcsa_fwd_kernel<T, D, false, VARLEN, true>, dim3((unsigned)grid), dim3(Cfg::kThreads),
+                         Cfg::kSmem, stream, tq, tk, tv, a);
+  } else {
+    e = fcsa::launch_pdl(fcsa::fcsa_fwd_kernel<T, D, false, VARLEN>, dim3((unsigned)grid), dim3(Cfg::kThreads),
+                         Cfg::kSmem, stream, tq, tk, tv, base);
+  }
   if (g_ev[0][1]) cudaEventRecord(g_ev[0][1], stream);
   if (e != cudaSuccess) return cuda_fail(e, "forward kernel launch");
   g_launches.fetch_add(1);
@@ -203,7 +227,8 @@ int decode_shape(const fcsa_problem* p, DecodeShape* s) {
   s->R = (p->heads / p->kv_heads) * p->seq_q;
   s->n_rb = (s->R + 63) / 64;
   s->items = (long long)p->batch * p->kv_heads * s->n_rb;
-  s->n_split = fcsa::decode_split(s->items, p->seq_k, sms);
+  const int w = kernel_window(p);
+  s->n_split = fcsa::decode_split(s->items, w > 0 ? fcsa::decode_window_keys(p->seq_k, w, p->causal != 0) : p->seq_k, sms);
   return FCSA_OK;
 }
 
@@ -227,7 +252,8 @@ int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tenso
   if ((r = fcsa::make_tensor_map_bhnd(&tv, vc->ptr, fcsa::tma_dtype16(bf), p->batch, p->kv_heads, p->seq_k, D, vc->sb,
                                       vc->sh, vc->sn, 128)))
     return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "v_cache: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map" : "cuTensorMapEncodeTiled failed", r);
-  fcsa::DecodeArgs a;
+  fcsa::Windowed<fcsa::DecodeArgs> a;
+  a.window = kernel_window(p);
   a.B = p->batch; a.H = p->heads; a.KVH = p->kv_heads; a.G = p->heads / p->kv_heads;
   a.Nq = p->seq_q; a.cap = p->seq_k; a.n_new = n_new;
   a.causal = p->causal ? 1 : 0;
@@ -239,20 +265,25 @@ int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tenso
   a.q = q->ptr; a.q_sb = q->sb; a.q_sh = q->sh; a.q_sn = q->sn;
   a.o = o->ptr; a.o_sb = o->sb; a.o_sh = o->sh; a.o_sn = o->sn;
   a.part = part;
+  const bool win = a.window > 0;
+  const fcsa::DecodeArgs& base = a;
   {
-    cudaError_t e = fcsa::ensure_dynamic_smem<fcsa::fcsa_decode_kernel<T, D>>(Cfg::kSmem);
+    cudaError_t e = win ? fcsa::ensure_dynamic_smem<fcsa::fcsa_decode_kernel<T, D, true>>(Cfg::kSmem)
+                        : fcsa::ensure_dynamic_smem<fcsa::fcsa_decode_kernel<T, D>>(Cfg::kSmem);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(decode)");
   }
   const long long grid = sh.items * sh.n_split;
   if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "decode: problem too large for one launch");
-  cudaError_t e = fcsa::launch_pdl(fcsa::fcsa_decode_kernel<T, D>, dim3((unsigned)grid), dim3(Cfg::kThreads),
-                                   Cfg::kSmem, stream, tk, tv, a);
+  cudaError_t e = win ? fcsa::launch_pdl(fcsa::fcsa_decode_kernel<T, D, true>, dim3((unsigned)grid),
+                                         dim3(Cfg::kThreads), Cfg::kSmem, stream, tk, tv, a)
+                      : fcsa::launch_pdl(fcsa::fcsa_decode_kernel<T, D>, dim3((unsigned)grid), dim3(Cfg::kThreads),
+                                         Cfg::kSmem, stream, tk, tv, base);
   if (e != cudaSuccess) return cuda_fail(e, "decode kernel launch");
   g_launches.fetch_add(1);
   if (sh.n_split == 1) return FCSA_OK;
   const long long threads = sh.items * 64 * (D / 4);
   e = fcsa::launch_pdl(fcsa::decode_combine_kernel<T, D>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0,
-                       stream, a);
+                       stream, base);
   if (e != cudaSuccess) return cuda_fail(e, "decode combine launch");
   g_launches.fetch_add(1);
   return FCSA_OK;
@@ -394,6 +425,7 @@ static int backward_impl(const fcsa_problem* p, const fcsa_tensor* q, const fcsa
   h.dtype_bf16 = p->dtype == FCSA_BF16;
   h.B = p->batch; h.H = p->heads; h.kv_heads = p->kv_heads; h.Nq = p->seq_q; h.Nk = p->seq_k;
   h.D = p->head_dim; h.causal = p->causal ? 1 : 0;
+  h.window = kernel_window(p);
   h.scale = p->scale; h.shift = p->shift;
   h.mask = p->key_mask; h.mask_sb = p->key_mask_stride;
   h.q = *q; h.k = *k; h.v = *v; h.o = *o; h.d_o = *d_o; h.dq = *dq; h.dk = *dk; h.dv = *dv;
@@ -665,6 +697,7 @@ int fcsa_backward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, con
   h.dtype_bf16 = p->dtype == FCSA_BF16;
   h.B = p->batch; h.H = p->heads; h.kv_heads = p->kv_heads; h.Nq = p->seq_q; h.Nk = p->seq_k;
   h.D = p->head_dim; h.causal = p->causal ? 1 : 0;
+  h.window = kernel_window(p);
   h.scale = p->scale; h.shift = p->shift;
   h.mask = nullptr; h.mask_sb = 0;
   h.q = n->q_hat; h.k = n->k_hat; h.v = *v; h.o = *o; h.d_o = *d_o; h.dq = *dq; h.dk = *dk; h.dv = *dv;

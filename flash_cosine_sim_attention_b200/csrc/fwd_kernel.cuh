@@ -65,12 +65,18 @@ struct FwdCfg {
   static_assert(kSmem <= 232448, "forward kernel shared memory");
 };
 
-template <typename T, int D, bool BIAS = false, bool VARLEN = false>
+template <bool VARLEN, bool WINDOW>
+using FwdArgsOf = std::conditional_t<WINDOW, Windowed<std::conditional_t<VARLEN, FwdVarlenArgs, FwdArgs>>,
+                                     std::conditional_t<VARLEN, FwdVarlenArgs, FwdArgs>>;
+
+// WINDOW: sliding-window attention (Windowed<>::window = W).  A block visits key tiles [j_lo, NT) instead of
+// [0, NT): j_lo is the tile of the smallest lower limit of its rows, and NT moves up by W - 1 when not causal.
+template <typename T, int D, bool BIAS = false, bool VARLEN = false, bool WINDOW = false>
 __global__ void __launch_bounds__(384, 1)
 fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
-                const __grid_constant__ CUtensorMap tm_v,
-                const std::conditional_t<VARLEN, FwdVarlenArgs, FwdArgs> a) {
+                const __grid_constant__ CUtensorMap tm_v, const FwdArgsOf<VARLEN, WINDOW> a) {
   static_assert(!(BIAS && VARLEN), "packed sequences take no bias");
+  static_assert(!(BIAS && WINDOW), "a window takes no bias");
   using Cfg = FwdCfg<D>;
   constexpr int S = Cfg::kStages, TILE = Cfg::kTile, DCH = D / 64;
 
@@ -128,20 +134,28 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     const int last_col = min(m0 + 127, Nq - 1) + off;
     NT = last_col < 0 ? 0 : min(NT, (last_col >> 7) + 1);
   }
+  int W = 0, j_lo = 0;                                        // the window and the first key tile visited
+  if constexpr (WINDOW) {
+    W = a.window;
+    const int last_col = min(m0 + 127, Nq - 1) + off + (a.causal ? 0 : W - 1);
+    NT = last_col < 0 ? 0 : min((Nk + 127) >> 7, (last_col >> 7) + 1);
+    const int first_col = m0 + off - W + 1;                   // the lower limit of the block's first row
+    j_lo = first_col <= 0 ? 0 : min(first_col >> 7, NT);
+  }
 
   if (wg == 0) {
     // =============================== TMA producer ===============================
     reg_dealloc<kProducerRegs>();
-    if (warp == 0 && elect_one() && NT > 0) {
+    if (warp == 0 && elect_one() && NT > j_lo) {
       tma_prefetch_desc(&tm_q);
       tma_prefetch_desc(&tm_k);
       tma_prefetch_desc(&tm_v);
       mbar_expect_tx(BAR(Q_FULL), TILE);
 #pragma unroll
       for (int ch = 0; ch < DCH; ++ch) tma_load_4d(sQ + ch * 16384, &tm_q, BAR(Q_FULL), ch * 64, q_row0 + m0, h, tb);
-      for (int j = 0; j < NT; ++j) {
-        const int s = j % S;
-        const uint32_t par = ((j / S) & 1) ^ 1;
+      for (int j = j_lo; j < NT; ++j) {
+        const int s = (j - j_lo) % S;
+        const uint32_t par = (((j - j_lo) / S) & 1) ^ 1;
         mbar_wait(BAR(K_EMPTY + s), par);
         mbar_expect_tx(BAR(K_FULL + s), TILE);
 #pragma unroll
@@ -180,17 +194,26 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   int lim[2];
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) lim[hf] = a.causal ? min(Nk - 1, row_a + 8 * hf + off) : Nk - 1;
+  // WINDOW: first visible column of each row, and the non-causal band's upper side
+  int lo[2] = {0, 0};
+  if constexpr (WINDOW) {
+#pragma unroll
+    for (int hf = 0; hf < 2; ++hf) {
+      lo[hf] = row_a + 8 * hf + off - W + 1;
+      if (!a.causal) lim[hf] = min(Nk - 1, row_a + 8 * hf + off + W - 1);
+    }
+  }
 
   float o[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
   float l[2] = {0.f, 0.f};
-  if (NT > 0) mbar_wait(BAR(Q_FULL), 0);
+  if (NT > j_lo) mbar_wait(BAR(Q_FULL), 0);
   const uint32_t sQw = sQ + w * 64 * 128;     // this warpgroup's 64 rows inside every 64-feature chunk of Q
 
-  for (int j = 0; j < NT; ++j) {
-    const int s = j % S;
-    const uint32_t par = (j / S) & 1;
+  for (int j = j_lo; j < NT; ++j) {
+    const int s = (j - j_lo) % S;
+    const uint32_t par = ((j - j_lo) / S) & 1;
     // ---- S = Q K^T (64 x 128, fp32) ----
     float sacc[64];
     mbar_wait(BAR(K_FULL + s), par);
@@ -208,7 +231,10 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
     // ---- P = exp2(S*c1 - c2 [+ bias*log2e]), masked; row sums in fp32; 16-bit P as A fragments ----
     const int col0 = j * 128;
-    const bool need_mask = a.has_mask || (col0 + 127 >= Nk) || (a.causal && col0 + 127 > m0 + 64 * w + off);
+    bool need_mask = a.has_mask || (col0 + 127 >= Nk) || (a.causal && col0 + 127 > m0 + 64 * w + off);
+    // (window: a column below the warpgroup's largest lower limit, or past its smallest upper one)
+    if constexpr (WINDOW)
+      need_mask = need_mask || col0 < m0 + 64 * w + 63 + off - W + 1 || col0 + 127 > m0 + 64 * w + off + W - 1;
     uint32_t pf[32];
     auto exp_tile = [&](auto masked_tag) {
       constexpr bool MASKED = decltype(masked_tag)::value;
@@ -228,6 +254,10 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         float p1 = ex2_approx(fmaf(sacc[2 * i + 1], c1, add1));
         if constexpr (MASKED) {
           bool v0 = col <= lim[hf], v1 = col + 1 <= lim[hf];
+          if constexpr (WINDOW) {
+            v0 = v0 && col >= lo[hf];
+            v1 = v1 && col + 1 >= lo[hf];
+          }
           if (a.has_mask) {
             v0 = v0 && a.mask[(long long)b * a.mask_sb + col] != 0;
             v1 = v1 && a.mask[(long long)b * a.mask_sb + col + 1] != 0;

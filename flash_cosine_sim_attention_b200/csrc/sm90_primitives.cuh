@@ -389,4 +389,12 @@ __device__ __forceinline__ SeqSpan seq_span(const int* cu, int b, int max_len, i
   return {s, min(e - s, max_len)};
 }
 
+// Sliding-window (local) attention: the WINDOW instantiations take their kernel's arguments plus the window W >= 1.
+// With off = Nk - Nq and d = i + off - j, key j is visible to query i iff 0 <= d < W (causal) or |d| < W (not causal),
+// on top of the kernel's other limits.  The host runs a window of at least Nq + Nk on the unwindowed kernels.
+template <class Base>
+struct Windowed : Base {
+  int window;
+};
+
 }  // namespace fcsa

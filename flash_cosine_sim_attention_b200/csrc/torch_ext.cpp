@@ -101,11 +101,13 @@ struct Shapes {
   }
 };
 
+// window: sliding-window attention (0 = none); the library rejects a negative one
 fcsa_problem make_problem(const Shapes& sh, const Tensor& q, double scale, double shift, bool causal,
-                          const optional<Tensor>& mask_u8, bool out_f32 = false) {
+                          const optional<Tensor>& mask_u8, bool out_f32 = false, int64_t window = 0) {
+  TORCH_CHECK(window >= 0 && window <= 0x7FFFFFFF, "window must be a non-negative int32 (0 = none), got ", window);
   fcsa_problem p;
   p.out_f32 = out_f32 ? 1 : 0;
-  p.reserved_ = 0;
+  p.window = (int32_t)window;
   p.dtype = dtype_code(q);
   p.batch = (int32_t)sh.B; p.heads = (int32_t)sh.H; p.kv_heads = (int32_t)sh.kv_heads;
   p.seq_q = (int32_t)sh.Nq; p.seq_k = (int32_t)sh.Nk; p.head_dim = (int32_t)sh.D;
@@ -271,13 +273,13 @@ Tensor f32_cast_backward(const Tensor& dy_in, const optional<Tensor>& y, const o
 std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> forward_ex(
     const Tensor& q_in, const Tensor& k_in, const Tensor& v_in, const optional<Tensor>& mask,
     const optional<Tensor>& bias_prepared, bool bias_batch_dim, const optional<Tensor>& bias_amax, double scale,
-    double shift, bool causal, int64_t l2norm_groups, bool need_inv_l, bool out_f32) {
+    double shift, bool causal, int64_t l2norm_groups, bool need_inv_l, bool out_f32, int64_t window) {
   const Shapes sh(q_in, k_in, v_in);
   TORCH_CHECK(!(causal && mask.has_value() && mask->defined()), "mask should not be supplied if causality is needed");
   const c10::cuda::CUDAGuard guard(q_in.device());
   const Tensor q = tma_ready(q_in), k = tma_ready(k_in), v = tma_ready(v_in);
   const optional<Tensor> mask_u8 = prep_mask(mask, sh);
-  const fcsa_problem p = make_problem(sh, q, scale, shift, causal, mask_u8, out_f32);
+  const fcsa_problem p = make_problem(sh, q, scale, shift, causal, mask_u8, out_f32, window);
   Tensor o = at::empty(q.sizes(), out_f32 ? q.options().dtype(at::kFloat) : q.options());   // out_f32: no final rounding
   Tensor inv_l;
   if (need_inv_l) inv_l = at::empty({sh.B, sh.H, sh.Nq}, q.options().dtype(at::kFloat));
@@ -318,7 +320,7 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> backward_ex(
     const Tensor& v_in, const optional<Tensor>& q_rnorm, const optional<Tensor>& k_rnorm,
     const optional<Tensor>& mask, const optional<Tensor>& bias_prepared, bool bias_batch_dim,
     const optional<Tensor>& bias_amax, bool bias_grad, const optional<Tensor>& bias_like, double scale, double shift,
-    bool causal, int64_t groups, bool out_f32) {
+    bool causal, int64_t groups, bool out_f32, int64_t window) {
   const Shapes sh(q_in, k_in, v_in);
   const c10::cuda::CUDAGuard guard(q_in.device());
   const Tensor q = tma_ready(q_in), k = tma_ready(k_in), v = tma_ready(v_in), o = tma_ready(o_in),
@@ -326,7 +328,7 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> backward_ex(
   TORCH_CHECK(d_o.sizes() == q.sizes() && d_o.scalar_type() == q.scalar_type(),
               "d_out must have the shape and dtype of the queries");
   const optional<Tensor> mask_u8 = prep_mask(mask, sh);
-  const fcsa_problem p = make_problem(sh, q, scale, shift, causal, mask_u8, out_f32);
+  const fcsa_problem p = make_problem(sh, q, scale, shift, causal, mask_u8, out_f32, window);
   TORCH_CHECK(o.scalar_type() == (out_f32 ? at::kFloat : q.scalar_type()), "backward_ex: `o` must be ",
               out_f32 ? "float32 (out_f32)" : "in the operand dtype");
   const auto gopt = out_f32 ? q.options().dtype(at::kFloat) : q.options();     // out_f32: float32 gradients
@@ -386,7 +388,7 @@ std::tuple<Tensor, Tensor, bool> forward(const Tensor& q, const Tensor& k, const
   optional<Tensor> bias_prepared;
   if (has_bias) bias_prepared = prep_bias(*attn_bias, sh, q.scalar_type(), attn_bias_batch_dim);
   auto r = forward_ex(q, k, v, mask, bias_prepared, attn_bias_batch_dim, c10::nullopt, scale, scale, causal, 0, true,
-                      false);
+                      false, 0);
   return {std::get<0>(r), std::get<1>(r), should_backwards};
 }
 
@@ -400,7 +402,7 @@ std::tuple<Tensor, Tensor, Tensor, optional<Tensor>> backward(
   optional<Tensor> bias_prepared;
   if (has_bias) bias_prepared = prep_bias(*attn_bias, sh, q.scalar_type(), attn_bias_batch_dim);
   auto r = backward_ex(d_out, o, l, q, k, v, c10::nullopt, c10::nullopt, mask, bias_prepared, attn_bias_batch_dim,
-                       c10::nullopt, has_bias && attn_bias->requires_grad(), attn_bias, scale, scale, causal, 0, false);
+                       c10::nullopt, has_bias && attn_bias->requires_grad(), attn_bias, scale, scale, causal, 0, false, 0);
   optional<Tensor> db;
   if (std::get<3>(r).defined()) db = std::get<3>(r);
   return {std::get<0>(r), std::get<1>(r), std::get<2>(r), db};
@@ -415,7 +417,8 @@ std::tuple<Tensor, Tensor, Tensor, optional<Tensor>> backward(
 // ------------------------------------------------------------------------------------------------
 Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
               const optional<Tensor>& k_in, const optional<Tensor>& v_in, double scale, double shift, bool causal,
-              int64_t groups) {
+              int64_t groups, int64_t window) {
+  TORCH_CHECK(window >= 0 && window <= 0x7FFFFFFF, "decode: window must be a non-negative int32 (0 = none), got ", window);
   TORCH_CHECK(q_in.dim() == 4 && k_cache.dim() == 4 && v_cache.dim() == 4,
               "decode: q, k_cache, v_cache must be (batch, heads, seq, head_dim)");
   TORCH_CHECK(q_in.is_cuda() && k_cache.is_cuda() && v_cache.is_cuda(), "decode: CUDA tensors required");
@@ -460,7 +463,7 @@ Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, 
   p.causal = causal ? 1 : 0;
   p.scale = (float)scale; p.shift = (float)shift;
   p.key_mask = nullptr; p.key_mask_stride = 0;
-  p.out_f32 = 0; p.reserved_ = 0;
+  p.out_f32 = 0; p.window = (int32_t)window;
   Tensor o = at::empty({B, H, Nq, D}, q.options());
   cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
   const size_t need = fcsa_decode_workspace_bytes(&p, (int32_t)n_new);
@@ -500,7 +503,8 @@ struct Varlen {
 };
 
 Varlen varlen_problem(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& cu_q, const Tensor& cu_k,
-                      int64_t max_q, int64_t max_k, double scale, double shift, bool causal) {
+                      int64_t max_q, int64_t max_k, double scale, double shift, bool causal, int64_t window) {
+  TORCH_CHECK(window >= 0 && window <= 0x7FFFFFFF, "varlen: window must be a non-negative int32 (0 = none), got ", window);
   TORCH_CHECK(q.dim() == 3 && k.dim() == 3 && v.dim() == 3,
               "varlen: q must be (total_q, heads, head_dim) and k, v (total_k, kv_heads, head_dim)");
   TORCH_CHECK(q.is_cuda() && k.is_cuda() && v.is_cuda(), "varlen: CUDA tensors required - this build has no CPU path");
@@ -527,7 +531,7 @@ Varlen varlen_problem(const Tensor& q, const Tensor& k, const Tensor& v, const T
   p.causal = causal ? 1 : 0;
   p.scale = (float)scale; p.shift = (float)shift;
   p.key_mask = nullptr; p.key_mask_stride = 0;
-  p.out_f32 = 0; p.reserved_ = 0;
+  p.out_f32 = 0; p.window = (int32_t)window;
   r.vl.cu_seqlens_q = cu_q.data_ptr<int32_t>();
   r.vl.cu_seqlens_k = cu_k.data_ptr<int32_t>();
   r.vl.total_q = (int32_t)q.size(0);
@@ -539,10 +543,10 @@ Varlen varlen_problem(const Tensor& q, const Tensor& k, const Tensor& v, const T
 // undefined when groups == 0, inv_l undefined unless need_inv_l
 std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> forward_varlen(
     const Tensor& q_in, const Tensor& k_in, const Tensor& v_in, const Tensor& cu_q, const Tensor& cu_k, int64_t max_q,
-    int64_t max_k, double scale, double shift, bool causal, int64_t groups, bool need_inv_l) {
+    int64_t max_k, double scale, double shift, bool causal, int64_t groups, bool need_inv_l, int64_t window) {
   const c10::cuda::CUDAGuard guard(q_in.device());
   const Tensor q = tma_ready(q_in), k = tma_ready(k_in), v = tma_ready(v_in);
-  const Varlen vr = varlen_problem(q, k, v, cu_q, cu_k, max_q, max_k, scale, shift, causal);
+  const Varlen vr = varlen_problem(q, k, v, cu_q, cu_k, max_q, max_k, scale, shift, causal, window);
   const int64_t H = q.size(1), Hk = k.size(1), Tq = q.size(0), Tk = k.size(0);
   Tensor o = at::empty(q.sizes(), q.options());
   Tensor inv_l;
@@ -570,11 +574,12 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> forward_varlen(
 std::tuple<Tensor, Tensor, Tensor> backward_varlen(
     const Tensor& d_out, const Tensor& o_in, const Tensor& inv_l, const Tensor& q_in, const Tensor& k_in,
     const Tensor& v_in, const optional<Tensor>& q_rnorm, const optional<Tensor>& k_rnorm, const Tensor& cu_q,
-    const Tensor& cu_k, int64_t max_q, int64_t max_k, double scale, double shift, bool causal, int64_t groups) {
+    const Tensor& cu_k, int64_t max_q, int64_t max_k, double scale, double shift, bool causal, int64_t groups,
+    int64_t window) {
   const c10::cuda::CUDAGuard guard(q_in.device());
   const Tensor q = tma_ready(q_in), k = tma_ready(k_in), v = tma_ready(v_in), o = tma_ready(o_in),
                d_o = tma_ready(d_out);
-  const Varlen vr = varlen_problem(q, k, v, cu_q, cu_k, max_q, max_k, scale, shift, causal);
+  const Varlen vr = varlen_problem(q, k, v, cu_q, cu_k, max_q, max_k, scale, shift, causal, window);
   TORCH_CHECK(d_o.sizes() == q.sizes() && d_o.scalar_type() == q.scalar_type() && o.sizes() == q.sizes() &&
                   o.scalar_type() == q.scalar_type(),
               "backward_varlen: o and d_out must have the shape and dtype of the queries");
@@ -632,16 +637,33 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("forward", &forward, "Flash Cosine-Sim Attention Forward");
   m.def("backward", &backward, "Flash Cosine-Sim Attention Backward");
   m.def("debug", &debug, "Debug");
-  m.def("forward_ex", &forward_ex, "forward with explicit shift / fused l2norm / prepared bias");
-  m.def("backward_ex", &backward_ex, "backward of forward_ex");
+  namespace py = pybind11;
+  // (window: a trailing argument, default 0 = no window, after the positional ones every caller passes)
+  m.def("forward_ex", &forward_ex, "forward with explicit shift / fused l2norm / prepared bias", py::arg("q"),
+        py::arg("k"), py::arg("v"), py::arg("mask"), py::arg("bias_prepared"), py::arg("bias_batch_dim"),
+        py::arg("bias_amax"), py::arg("scale"), py::arg("shift"), py::arg("causal"), py::arg("l2norm_groups"),
+        py::arg("need_inv_l"), py::arg("out_f32"), py::arg("window") = 0);
+  m.def("backward_ex", &backward_ex, "backward of forward_ex", py::arg("d_out"), py::arg("o"), py::arg("inv_l"),
+        py::arg("q"), py::arg("k"), py::arg("v"), py::arg("q_rnorm"), py::arg("k_rnorm"), py::arg("mask"),
+        py::arg("bias_prepared"), py::arg("bias_batch_dim"), py::arg("bias_amax"), py::arg("bias_grad"),
+        py::arg("bias_like"), py::arg("scale"), py::arg("shift"), py::arg("causal"), py::arg("groups"),
+        py::arg("out_f32"), py::arg("window") = 0);
   m.def("prepare_bias", &prepare_bias, "attn_bias -> padded, aligned tensor in the problem dtype");
   m.def("f32_cast", &f32_cast, "float32 -> (l2norm +) scaled cast to the 16-bit operand dtype");
   m.def("f32_cast_backward", &f32_cast_backward, "backward of f32_cast: float32 gradient w.r.t. the float32 input");
   m.def("l2norm_forward", &l2norm_forward, "grouped l2norm: x -> (y, 1/norm)");
   m.def("l2norm_backward", &l2norm_backward, "grouped l2norm backward from the normalised y");
-  m.def("forward_varlen", &forward_varlen, "packed variable-length sequences: forward (fused l2norm when groups > 0)");
-  m.def("backward_varlen", &backward_varlen, "backward of forward_varlen");
-  m.def("decode", &decode, "new queries against a key/value cache, appending k / v at cache_seqlens");
+  m.def("forward_varlen", &forward_varlen, "packed variable-length sequences: forward (fused l2norm when groups > 0)",
+        py::arg("q"), py::arg("k"), py::arg("v"), py::arg("cu_q"), py::arg("cu_k"), py::arg("max_q"), py::arg("max_k"),
+        py::arg("scale"), py::arg("shift"), py::arg("causal"), py::arg("groups"), py::arg("need_inv_l"),
+        py::arg("window") = 0);
+  m.def("backward_varlen", &backward_varlen, "backward of forward_varlen", py::arg("d_out"), py::arg("o"),
+        py::arg("inv_l"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("q_rnorm"), py::arg("k_rnorm"),
+        py::arg("cu_q"), py::arg("cu_k"), py::arg("max_q"), py::arg("max_k"), py::arg("scale"), py::arg("shift"),
+        py::arg("causal"), py::arg("groups"), py::arg("window") = 0);
+  m.def("decode", &decode, "new queries against a key/value cache, appending k / v at cache_seqlens", py::arg("q"),
+        py::arg("k_cache"), py::arg("v_cache"), py::arg("cache_seqlens"), py::arg("k"), py::arg("v"), py::arg("scale"),
+        py::arg("shift"), py::arg("causal"), py::arg("groups"), py::arg("window") = 0);
   m.def("release_workspaces", &release_workspaces, "free the cached backward workspaces; returns the bytes released");
   m.def("abi_version", []() { return fcsa_version(); });
   m.def("_error_path_selftest", []() { FCSA_CHECK(fcsa_forward(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr)); },

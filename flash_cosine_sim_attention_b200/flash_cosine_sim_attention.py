@@ -292,28 +292,28 @@ class _FusedCosineSimAttention(Function):
     """One autograd node for l2norm(q), l2norm(k) -> attention, all in CUDA kernels."""
 
     @staticmethod
-    def forward(ctx, q, k, v, mask, scale, causal, groups, l2norm_qk, shift_groups=0):
+    def forward(ctx, q, k, v, mask, scale, causal, groups, l2norm_qk, shift_groups=0, window=0):
         ext = _ext()
         # shift_groups > 0: q, k arrive already normalised over that many groups (padded head dims)
         shift = (_choose_shift(q.dtype, scale, shift_groups, True) if shift_groups > 0
                  else _choose_shift(q.dtype, scale, groups, l2norm_qk))
         needs_grad = any(ctx.needs_input_grad[:3])
         o, inv_l, qn, kn, rq, rk = ext.forward_ex(q, k, v, mask, None, False, None, scale, shift, causal,
-                                                  groups if l2norm_qk else 0, needs_grad, False)
+                                                  groups if l2norm_qk else 0, needs_grad, False, window)
         if needs_grad:
             if not l2norm_qk:
                 qn, kn = q, k
             ctx.save_for_backward(o, inv_l, qn, kn, v, mask, rq, rk)
-            ctx.params = (scale, shift, causal, groups, l2norm_qk)
+            ctx.params = (scale, shift, causal, groups, l2norm_qk, window)
         return o
 
     @staticmethod
     def backward(ctx, do):
         o, inv_l, qn, kn, v, mask, rq, rk = ctx.saved_tensors
-        scale, shift, causal, groups, l2norm_qk = ctx.params
+        scale, shift, causal, groups, l2norm_qk, window = ctx.params
         dq, dk, dv, _ = _ext().backward_ex(do, o, inv_l, qn, kn, v, rq, rk, mask, None, False, None, False, None,
-                                           scale, shift, causal, groups if l2norm_qk else 0, False)
-        return dq, dk, dv, None, None, None, None, None, None
+                                           scale, shift, causal, groups if l2norm_qk else 0, False, window)
+        return dq, dk, dv, None, None, None, None, None, None, None
 
 
 class _L2Norm(Function):
@@ -335,6 +335,27 @@ class _L2Norm(Function):
 # --------------------------------------------------------------------------------------------
 # public API
 # --------------------------------------------------------------------------------------------
+
+def _check_window(window, attn_bias, name):
+    """The `window` keyword of the attention entry points: None (no window) or a positive int W; returns W or 0.
+    With off = n_k - n_q and d = i + off - j, key j is visible to query i iff 0 <= d < W (causal) or |d| < W (not
+    causal).  Rejected before any launch: a bool or non-int, W < 1, and a window together with attn_bias."""
+    if window is None:
+        return 0
+    if isinstance(window, bool) or not isinstance(window, int):
+        raise TypeError(f"{name}: window must be a positive int or None, got {window!r}")
+    if window < 1:
+        raise ValueError(f"{name}: window must be at least 1 (None for no window), got {window}")
+    if exists(attn_bias):
+        raise NotImplementedError(f"{name}: window with attn_bias is not supported (the bias kernels take no window)")
+    return min(window, 2 ** 31 - 1)
+
+
+def _band(nq, nk, window, causal, device):
+    """(nq, nk) bool: the keys a sliding window of `window` lets each query see (see `_check_window`)."""
+    d = torch.arange(nq, device=device)[:, None] + (nk - nq) - torch.arange(nk, device=device)[None, :]
+    return ((d >= 0) & (d < window)) if causal else (d.abs() < window)
+
 
 def _l2norm_torch(t, groups):
     shape = t.shape
@@ -361,11 +382,13 @@ def l2norm_tensors(*tensors, groups=1):
 
 
 def plain_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, groups=1, causal=False,
-                               l2norm_qk=True, attn_bias_batch_dim=False):
+                               l2norm_qk=True, attn_bias_batch_dim=False, window=None):
     """The naive, un-fused formulation (reference py:75-126): explicit similarity matrix,
     masked softmax, weighted sum.  Public API of the reference package (used by
-    transformer.py when the fused kernel is switched off); any device, any float dtype."""
+    transformer.py when the fused kernel is switched off); any device, any float dtype.
+    window: sliding-window attention as in flash_cosine_sim_attention, applied as a band mask."""
     assert not (causal and exists(mask)), "mask should not be supplied if causality is needed"
+    window = _check_window(window, None, "plain_cosine_sim_attention")
     merged = q.ndim == 3
     single_head_kv = k.ndim == 3
     if merged:
@@ -401,6 +424,8 @@ def plain_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
         sim = sim.masked_fill(future, neg)
     if exists(mask):
         sim = sim.masked_fill(~mask[(slice(None),) + lead + (None, slice(None))], neg)
+    if window:
+        sim = sim.masked_fill(~_band(sim.shape[-2], sim.shape[-1], window, causal, q.device), neg)
     out = torch.matmul(sim.softmax(dim=-1), vv)
     if grouped:
         out = out.flatten(1, 2)
@@ -457,7 +482,8 @@ class _Float32OnHalfKernels(Function):
     (its backward is the cast pass of the gradients); 0: they are used as given."""
 
     @staticmethod
-    def forward(ctx, q, k, v, mask, attn_bias, scale, causal, attn_bias_batch_dim, shift, half, use_amax, norm_groups):
+    def forward(ctx, q, k, v, mask, attn_bias, scale, causal, attn_bias_batch_dim, shift, half, use_amax, norm_groups,
+                window=0):
         ext = _ext()
         D = q.shape[-1]
         Dp = D if D in _KERNEL_HEAD_DIMS else (64 if D < 64 else 128)        # 16 / 32 / 96: zero-padded features
@@ -472,30 +498,32 @@ class _Float32OnHalfKernels(Function):
             if use_amax:
                 amax = attn_bias.detach().amax().float().reshape(1)
         needs_grad = any(ctx.needs_input_grad[:3]) or (exists(attn_bias) and ctx.needs_input_grad[4])
-        o, inv_l = ext.forward_ex(qh, kh, vh, mask, bias, batch_dim, amax, scale, shift, causal, 0, needs_grad, True)[:2]
+        o, inv_l = ext.forward_ex(qh, kh, vh, mask, bias, batch_dim, amax, scale, shift, causal, 0, needs_grad, True,
+                                  window)[:2]
         if needs_grad:
             ctx.save_for_backward(o, inv_l, qh, kh, vh, mask, bias, amax, sv, rq, rk)
-            ctx.params = (scale, shift, causal, batch_dim, D, exists(attn_bias) and ctx.needs_input_grad[4], norm_groups)
+            ctx.params = (scale, shift, causal, batch_dim, D, exists(attn_bias) and ctx.needs_input_grad[4], norm_groups,
+                          window)
         return o[..., :D] * sv
 
     @staticmethod
     def backward(ctx, g):
         o, inv_l, qh, kh, vh, mask, bias, amax, sv, rq, rk = ctx.saved_tensors
-        scale, shift, causal, batch_dim, D, bias_grad, norm_groups = ctx.params
+        scale, shift, causal, batch_dim, D, bias_grad, norm_groups, window = ctx.params
         # o = o_kernel * sv, so d(o_kernel) = g * sv; it enters the kernels as fp16 scaled into [1, 2):
         # g * sv / sg with sg = pg * sv, pg = pow2 scale of g  ->  the cast pass computes g / pg
         pg = _pow2_scale(g, 1)
         gh, _ = _cast16(g, qh.dtype, 0, pg, True, qh.shape[-1])
         dq, dk, dv, db = _ext().backward_ex(gh, o, inv_l, qh, kh, vh, None, None, mask, bias, batch_dim, amax,
-                                            bias_grad, None, scale, shift, causal, 0, True)
+                                            bias_grad, None, scale, shift, causal, 0, True, window)
         sg = pg * sv                                          # undo the gradient scale; dv also undoes v / sv
         dq = _uncast16(dq, qh, rq, norm_groups, sg, False, D)
         dk = _uncast16(dk, kh, rk, norm_groups, sg, False, D)
         dv = _uncast16(dv, None, None, 0, pg, False, D)
-        return dq, dk, dv, None, (db * sg if bias_grad else None), None, None, None, None, None, None, None
+        return dq, dk, dv, None, (db * sg if bias_grad else None), None, None, None, None, None, None, None, None
 
 
-def _float32_on_half_kernels(q, k, v, mask, attn_bias, scale, groups, causal, l2norm_qk, attn_bias_batch_dim):
+def _float32_on_half_kernels(q, k, v, mask, attn_bias, scale, groups, causal, l2norm_qk, attn_bias_batch_dim, window=0):
     D = q.shape[-1]
     assert D % groups == 0, "groups must divide the head dim"
     # fp16 (11-bit significand, like tf32) whenever its exponent range holds exp(scale * q.k); bf16 (8 bits, fp32's
@@ -514,7 +542,8 @@ def _float32_on_half_kernels(q, k, v, mask, attn_bias, scale, groups, causal, l2
             q, k = _l2norm_torch(q, groups), _l2norm_torch(k, groups)       # fp32, differentiable
     shift = _choose_shift(h, scale, groups if l2norm_qk else 1, l2norm_qk)
     return _Float32OnHalfKernels.apply(q, k, v, mask, attn_bias, float(scale), bool(causal), bool(attn_bias_batch_dim),
-                                       float(shift), h, bool(l2norm_qk and h == torch.float16), int(norm_groups))
+                                       float(shift), h, bool(l2norm_qk and h == torch.float16), int(norm_groups),
+                                       int(window))
 
 
 _warned = set()
@@ -527,9 +556,14 @@ def _warn_once(key, msg):
 
 
 def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, groups=1, causal=False,
-                               l2norm_qk=True, attn_bias_batch_dim=False, l2norm_groups=None):
+                               l2norm_qk=True, attn_bias_batch_dim=False, l2norm_groups=None, window=None):
     """Fused cosine-similarity attention (reference py:308-334, same arguments and meaning;
     `l2norm_groups` is accepted as an alias of `groups`).
+
+    window: sliding-window (local) attention, None or a positive int W.  With off = n_k - n_q (the bottom-right
+    alignment of causal masking) and d = i + off - j, key j is visible to query i iff 0 <= d < W with causal=True (the
+    query itself and the W - 1 keys before it) and iff |d| < W otherwise, on top of `mask`.  The kernels skip the key
+    tiles outside the band, so a causal pass costs O(n * W).  Rows that see no key give 0.  Not with attn_bias.
 
     Every supported input runs the hand-written sm_90a kernels: float16 / bfloat16 natively, float32 at
     tf32-class operand precision on the fp16 kernels (see _float32_on_half_kernels), head dims 64 and 128
@@ -538,6 +572,7 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
     if exists(l2norm_groups):
         groups = l2norm_groups
     assert not (causal and exists(mask)), "mask should not be supplied if causality is needed"
+    window = _check_window(window, attn_bias, "flash_cosine_sim_attention")
     if not q.is_cuda:
         raise RuntimeError(
             "flash_cosine_sim_attention: CUDA tensors required - this build has no CPU path "
@@ -553,7 +588,8 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
     if exists(attn_bias) and not attn_bias.is_cuda:
         raise RuntimeError("flash_cosine_sim_attention: attn_bias must be a CUDA tensor")
     if q.dtype == torch.float32:
-        return _float32_on_half_kernels(q, k, v, mask, attn_bias, scale, groups, causal, l2norm_qk, attn_bias_batch_dim)
+        return _float32_on_half_kernels(q, k, v, mask, attn_bias, scale, groups, causal, l2norm_qk, attn_bias_batch_dim,
+                                        window)
     if q.dtype not in _KERNEL_DTYPES:
         raise TypeError(f"flash_cosine_sim_attention: dtype {q.dtype} is not supported (float16, bfloat16, float32)")
     _warn_fp16_overflow(q.dtype, scale, groups, l2norm_qk)
@@ -574,7 +610,7 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
                                               bool(attn_bias_batch_dim), float(shift), amax)
         else:
             o = _FusedCosineSimAttention.apply(pad(q), pad(k), pad(v), mask, float(scale), bool(causal), 1, False,
-                                               int(groups) if l2norm_qk else 0)
+                                               int(groups) if l2norm_qk else 0, window)
         return o[..., :D]
     if exists(attn_bias):
         # additive bias: l2norm kernels (with their own backward), then the BIAS instantiations of the
@@ -591,7 +627,8 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
                                              bool(attn_bias_batch_dim), float(shift), amax)
     gs = q.shape[-1] // groups
     assert (gs & (gs - 1)) == 0, "groups must divide the head dim into power-of-two chunks"
-    return _FusedCosineSimAttention.apply(q, k, v, mask, float(scale), bool(causal), int(groups), bool(l2norm_qk))
+    return _FusedCosineSimAttention.apply(q, k, v, mask, float(scale), bool(causal), int(groups), bool(l2norm_qk), 0,
+                                          window)
 
 
 def _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias):
@@ -646,7 +683,7 @@ def _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask,
 
 
 def flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens, k=None, v=None, scale=8, groups=1,
-                                             causal=True, l2norm_qk=True, mask=None, attn_bias=None):
+                                             causal=True, l2norm_qk=True, mask=None, attn_bias=None, window=None):
     """Cosine-sim attention of new queries against a key/value cache, for inference (generation).
 
     q: (batch, heads, n_q, head_dim) new queries.  k_cache, v_cache: (batch, kv_heads, capacity, head_dim), kv_heads
@@ -663,38 +700,41 @@ def flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens,
 
     L_b + n_new must not exceed the capacity: rows that do not fit are not written, and T_b is clamped to the
     capacity.  float16 / bfloat16 and head dims 64 and 128 only; no autograd, attn_bias, mask, float32 or merged
-    batch-heads.  Returns o (batch, heads, n_q, head_dim)."""
+    batch-heads.  window: sliding-window attention as in flash_cosine_sim_attention with n_k = T_b; a step then reads
+    the tiles of its window, not the whole valid cache (the cache itself stays full-length).
+    Returns o (batch, heads, n_q, head_dim)."""
+    window = _check_window(window, attn_bias, "flash_cosine_sim_attention_with_kv_cache")
     _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias)
     _warn_fp16_overflow(q.dtype, scale, groups, l2norm_qk)
     shift = _choose_shift(q.dtype, scale, groups, l2norm_qk)
     return _ext().decode(q, k_cache, v_cache, cache_seqlens, k, v, float(scale), float(shift), bool(causal),
-                         int(groups) if l2norm_qk else 0)
+                         int(groups) if l2norm_qk else 0, window)
 
 
 class _FusedVarlenAttention(Function):
     """One autograd node for packed sequences: l2norm(q), l2norm(k) -> attention, all in CUDA kernels."""
 
     @staticmethod
-    def forward(ctx, q, k, v, cu_q, cu_k, max_q, max_k, scale, causal, groups, l2norm_qk):
+    def forward(ctx, q, k, v, cu_q, cu_k, max_q, max_k, scale, causal, groups, l2norm_qk, window=0):
         shift = _choose_shift(q.dtype, scale, groups, l2norm_qk)
         g = groups if l2norm_qk else 0
         needs_grad = any(ctx.needs_input_grad[:3])
         o, inv_l, qn, kn, rq, rk = _ext().forward_varlen(q, k, v, cu_q, cu_k, max_q, max_k, scale, shift, causal, g,
-                                                         needs_grad)
+                                                         needs_grad, window)
         if needs_grad:
             if not l2norm_qk:
                 qn, kn = q, k
             ctx.save_for_backward(o, inv_l, qn, kn, v, rq, rk, cu_q, cu_k)
-            ctx.params = (max_q, max_k, scale, shift, causal, g)
+            ctx.params = (max_q, max_k, scale, shift, causal, g, window)
         return o
 
     @staticmethod
     def backward(ctx, do):
         o, inv_l, qn, kn, v, rq, rk, cu_q, cu_k = ctx.saved_tensors
-        max_q, max_k, scale, shift, causal, g = ctx.params
+        max_q, max_k, scale, shift, causal, g, window = ctx.params
         dq, dk, dv = _ext().backward_varlen(do, o, inv_l, qn, kn, v, rq, rk, cu_q, cu_k, max_q, max_k, scale, shift,
-                                            causal, g)
-        return (dq, dk, dv) + (None,) * 8
+                                            causal, g, window)
+        return (dq, dk, dv) + (None,) * 9
 
 
 class _EmptyVarlenAttention(Function):
@@ -758,7 +798,7 @@ def _check_varlen_args(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_se
 
 
 def flash_cosine_sim_attention_varlen(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale=8,
-                                      groups=1, causal=False, l2norm_qk=True, mask=None, attn_bias=None):
+                                      groups=1, causal=False, l2norm_qk=True, mask=None, attn_bias=None, window=None):
     """Cosine-sim attention over packed variable-length sequences (training: forward and backward).
 
     q: (total_q, heads, head_dim); k, v: (total_k, kv_heads, head_dim), kv_heads dividing heads (query head h reads kv
@@ -774,11 +814,13 @@ def flash_cosine_sim_attention_varlen(q, k, v, cu_seqlens_q, cu_seqlens_k, max_s
     sequences are allowed, and query rows that see no key give 0.  Rows outside every sequence ([0, cu[0]) and
     [cu[-1], total), e.g. the unused end of a fixed-size packing buffer) give o = 0 and zero gradients.  Packed tensors
     with no query or no key rows give zeros (and zero gradients) without a kernel launch.  float16 / bfloat16 and head dims 64 and 128 only; no float32, mask or
-    attn_bias.  Returns o (total_q, heads, head_dim)."""
+    attn_bias.  window: sliding-window attention as in flash_cosine_sim_attention, with each sequence's own lengths.
+    Returns o (total_q, heads, head_dim)."""
+    window = _check_window(window, attn_bias, "flash_cosine_sim_attention_varlen")
     _check_varlen_args(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, groups, mask, attn_bias)
     _warn_fp16_overflow(q.dtype, scale, groups, l2norm_qk)
     if q.shape[0] == 0 or k.shape[0] == 0:
         return _EmptyVarlenAttention.apply(q, k, v)
     return _FusedVarlenAttention.apply(q, k, v, cu_seqlens_q, cu_seqlens_k, max(int(max_seqlen_q), 1),
                                        max(int(max_seqlen_k), 1), float(scale), bool(causal), int(groups),
-                                       bool(l2norm_qk))
+                                       bool(l2norm_qk), window)

@@ -63,8 +63,13 @@ class KVCache:
 
 class Attention(nn.Module):
     def __init__(self, dim, dim_head=64, heads=8, scale=8, l2norm_groups=1, pre_norm=False,
-                 use_cuda_kernel=False, non_cosine_sim_attn=False, groups=None, kv_heads=None, **kwargs):
+                 use_cuda_kernel=False, non_cosine_sim_attn=False, groups=None, kv_heads=None, window=None, **kwargs):
         super().__init__()
+        # window: sliding-window attention - each token attends to itself and the window - 1 tokens before it, on
+        # every path (dense, packed documents, the key/value cache; the cache itself stays full-length)
+        if window is not None and non_cosine_sim_attn:
+            raise NotImplementedError("window is implemented for cosine-sim attention only (not non_cosine_sim_attn)")
+        self.window = window
         # kv_heads: grouped-query attention - `kv_heads` key/value heads (dividing `heads`), each read by
         # heads // kv_heads consecutive query heads.  None = one per query head (the reference's layout).
         kv_heads = heads if kv_heads is None else kv_heads
@@ -108,7 +113,7 @@ class Attention(nn.Module):
         q = split(self.to_q(x), self.heads)
         k, v = split(self.to_k(x), self.kv_heads), split(self.to_v(x), self.kv_heads)
         if cache is None:
-            o = self.attn_fn(q, k, v, causal=True, scale=self.scale, groups=self.l2norm_groups)
+            o = self.attn_fn(q, k, v, causal=True, scale=self.scale, groups=self.l2norm_groups, window=self.window)
         else:
             o = self._attend_cached(q, k, v, cache)
         return self.to_out(o.transpose(1, 2).reshape(b, n, -1))
@@ -128,7 +133,7 @@ class Attention(nn.Module):
             m = n if max_seqlen is None else int(max_seqlen)
             o = flash_cosine_sim_attention_varlen(q, k, v, cu_seqlens, cu_seqlens, m, m, scale=self.scale,
                                                   groups=self.l2norm_groups, causal=True,
-                                                  l2norm_qk=self.kernel_kwargs.get("l2norm_qk", True))
+                                                  l2norm_qk=self.kernel_kwargs.get("l2norm_qk", True), window=self.window)
         else:
             # the reference: one call per document (reads the boundaries on the host)
             bounds = cu_seqlens.tolist()
@@ -138,7 +143,7 @@ class Attention(nn.Module):
                 if e > s:
                     per_doc = lambda t: t[s:e].transpose(0, 1).unsqueeze(0)
                     o_d = self.attn_fn(per_doc(q), per_doc(k), per_doc(v), causal=True, scale=self.scale,
-                                       groups=self.l2norm_groups)
+                                       groups=self.l2norm_groups, window=self.window)
                     outs.append(o_d[0].transpose(0, 1))
             if bounds[-1] < n:
                 outs.append(q.new_zeros(n - bounds[-1], self.heads, q.shape[-1]))
@@ -168,12 +173,13 @@ class Attention(nn.Module):
         if self.use_cuda_kernel:
             o = flash_cosine_sim_attention_with_kv_cache(q, cache.k, cache.v, cache.seqlens, k, v, scale=self.scale,
                                                          groups=self.l2norm_groups, causal=True,
-                                                         l2norm_qk=self.kernel_kwargs.get("l2norm_qk", True))
+                                                         l2norm_qk=self.kernel_kwargs.get("l2norm_qk", True),
+                                                         window=self.window)
         else:
             cache.k[:, :, L:L + n] = k
             cache.v[:, :, L:L + n] = v
             o = plain_cosine_sim_attention(q, cache.k[:, :, :L + n], cache.v[:, :, :L + n], causal=True,
-                                           scale=self.scale, groups=self.l2norm_groups)
+                                           scale=self.scale, groups=self.l2norm_groups, window=self.window)
         cache.seqlens += n
         cache.length += n
         return o
@@ -182,7 +188,7 @@ class Attention(nn.Module):
 class CosineSimCausalTransformer(nn.Module):
     def __init__(self, *, num_tokens, dim, max_seq_len, depth, attn_scale=8, attn_l2norm_groups=1,
                  heads=8, dim_head=64, use_cuda_kernel=False, pre_norm=False, non_cosine_sim_attn=False,
-                 kv_heads=None, **kwargs):
+                 kv_heads=None, window=None, **kwargs):
         super().__init__()
         self.max_seq_len = max_seq_len
         self.token_emb = nn.Embedding(num_tokens, dim)
@@ -194,7 +200,7 @@ class CosineSimCausalTransformer(nn.Module):
             nn.ModuleList([
                 Attention(dim, dim_head=dim_head, heads=heads, use_cuda_kernel=use_cuda_kernel,
                           scale=attn_scale, groups=attn_l2norm_groups, pre_norm=pre_norm,
-                          non_cosine_sim_attn=non_cosine_sim_attn, kv_heads=kv_heads, **kwargs),
+                          non_cosine_sim_attn=non_cosine_sim_attn, kv_heads=kv_heads, window=window, **kwargs),
                 norm(),
                 FeedForward(dim, pre_norm=pre_norm),
                 norm(),

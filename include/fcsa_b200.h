@@ -78,7 +78,14 @@ typedef struct fcsa_problem {
                         1: they are float32 tensors (strides then count float32 elements) - the accumulators are
                         fp32 anyway, this only skips the final rounding to 16 bit.  q, k, v, d_o stay 16-bit
                         operands.  Used for float32 callers (reference: Float dispatch, cu:1702-1703)        */
-  int32_t reserved_;
+  int32_t window;    /* sliding-window (local) attention; 0 = none.  With off = seq_k - seq_q and d = i + off - j, key j
+                        is visible to query i iff 0 <= d < window (causal) or |d| < window (not causal), on top of the
+                        key mask.  Rows that see no key give o = 0 and zero gradients.  Negative: FCSA_ERR_INVALID;
+                        nonzero on the _bias entry points: FCSA_ERR_INVALID.  Taken by fcsa_forward, fcsa_backward,
+                        the _fused and _fused_varlen pairs (lengths per sequence) and fcsa_decode (seq_k = T_b there).
+                        The backward's workspace sizes do not depend on it; the decode workspace can only shrink
+                        (fewer key splits).  This field was `reserved_` before; a library built
+                        before it existed ignores it (fcsa_version() is 300 either way)                      */
 } fcsa_problem;
 
 /* Library / ABI version: major*10000 + minor*100 + patch. */
