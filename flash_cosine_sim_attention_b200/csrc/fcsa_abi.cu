@@ -98,7 +98,7 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
   CUtensorMap tq, tk, tv;
   int r;
   if ((r = fcsa::make_tensor_map_bhnd(&tq, q->ptr, fcsa::tma_dtype16(bf), tB, p->heads, tNq, D, q->sb, q->sh,
-                                      q->sn, 128)))
+                                      q->sn, Cfg::kBlockM)))       // Q: one box of the CTA's query rows
     return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "q: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - make the tensor contiguous" : "cuTensorMapEncodeTiled failed", r);
   if ((r = fcsa::make_tensor_map_bhnd(&tk, k->ptr, fcsa::tma_dtype16(bf), tB, p->kv_heads, tNk, D, k->sb,
                                       k->sh, k->sn, 128)))
@@ -120,7 +120,7 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
   a.causal = p->causal ? 1 : 0;
   a.has_mask = p->key_mask ? 1 : 0;
   a.group = p->heads / p->kv_heads;
-  a.n_qblk = (p->seq_q + 127) / 128;
+  a.n_qblk = (p->seq_q + Cfg::kBlockM - 1) / Cfg::kBlockM;
   const float log2e = 1.4426950408889634f;
   a.c1 = p->scale * log2e;
   a.c2 = p->shift * log2e;
@@ -146,7 +146,7 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
                  : fcsa::ensure_dynamic_smem<fcsa::fcsa_fwd_kernel<T, D, false, VARLEN>>(Cfg::kSmem);
     if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(fwd)");
   }
-  // one CTA per (query block of 128 rows, batch, head); packed sequences: blocks of the longest sequence
+  // one CTA per (query block of kBlockM rows, batch, head); packed sequences: blocks of the longest sequence
   const long long grid = (long long)a.n_qblk * p->batch * p->heads;
   if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
   if (g_ev[0][0]) cudaEventRecord(g_ev[0][0], stream);

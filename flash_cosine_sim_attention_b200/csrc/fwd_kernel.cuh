@@ -5,15 +5,17 @@
 // final 1/max(l, eps) scaling, cu:1239-1246; bottom-right aligned causal mask, cu:1097/1210;
 // key-padding mask, cu:1198-1212) - a different machine mapping:
 //
-//   * one CTA = 128 query rows of one (batch, head); CTAs are numbered heaviest first (causal: the last
-//     query blocks see the most keys), so the block scheduler starts the long ones first
+//   * one CTA = BM query rows of one (batch, head) (FwdCfg: 192 for D = 64, 128 for D = 128); CTAs are
+//     numbered heaviest first (causal: the last query blocks see the most keys), so the block scheduler
+//     starts the long ones first
 //   * warpgroup 0 : TMA producer (one thread): Q once, then K and V tiles of 128 keys through
-//                   mbarrier rings; the warpgroup gives most of its registers to the other two
-//   * warpgroups 1, 2: 64 query rows each.  Per key tile: S = Q K^T (wgmma, both operands in shared
-//                   memory) -> P = exp2(S*c1 - c2) in registers -> O += P V (wgmma with P as the register
-//                   A operand).  Because there is no row max there is no rescaling of O: the accumulator
-//                   stays in registers until the epilogue.  The two warpgroups share every K / V tile and
-//                   interleave on the tensor cores: one runs its exps while the other's MMAs run.
+//                   mbarrier rings; the warpgroup gives most of its registers to the consumers
+//   * warpgroups 1 .. BM / 64: 64 query rows each.  Per key tile: S = Q K^T (wgmma, both operands in
+//                   shared memory) -> P = exp2(S*c1 - c2) in registers -> O += P V (wgmma with P as the
+//                   register A operand).  Because there is no row max there is no rescaling of O: the
+//                   accumulator stays in registers until the epilogue.  The consumers share every K / V tile
+//                   and run independently of each other, each waiting on its own products; three of them
+//                   (D = 64) drift out of phase, so one's exps overlap another's products more often than two do.
 #pragma once
 
 #include "sm90_primitives.cuh"
@@ -25,7 +27,7 @@ struct FwdArgs {
   int causal;        // bottom-right aligned: key j visible to query i iff j <= i + (Nk - Nq)
   int has_mask;      // key padding mask (B, Nk), nonzero = keep
   int group;         // query heads per key/value head (H / kv_heads): head h reads kv head h / group
-  int n_qblk;        // ceil(Nq / 128)
+  int n_qblk;        // ceil(Nq / FwdCfg<D>::kBlockM)
   float c1;          // scale * log2(e)
   float c2;          // shift * log2(e)
   const uint8_t* mask;
@@ -52,16 +54,25 @@ struct FwdVarlenArgs : FwdArgs {
   int total_q, total_k;
 };
 
+// D = 64 runs three consumer warpgroups over 192 query rows: their S, O and P fit 160 registers, and three
+// independent consumers of the same K / V tiles cannot all stay in the same phase, so one's exponentials overlap
+// another's products more often than with two (DESIGN.md 4.1).  D = 128 (O alone is 64 registers) keeps two.
 template <int D>
 struct FwdCfg {
-  static constexpr int kTile = 128 * D * 2;          // bytes of one 128-row operand tile
+  static constexpr int kConsumers = (D == 64) ? 3 : 2;                 // consumer warpgroups, 64 query rows each
+  static constexpr int kBlockM = 64 * kConsumers;                      // query rows of one CTA
+  static constexpr int kThreads = 128 * (1 + kConsumers);              // + the producer warpgroup
+  static constexpr int kProducerRegs = kConsumers == 3 ? kProducerRegs3 : fcsa::kProducerRegs;
+  static constexpr int kConsumerRegs = kConsumers == 3 ? kConsumerRegs3 : fcsa::kConsumerRegs;
+  static constexpr int kTile = 128 * D * 2;          // bytes of one 128-row K / V tile
+  static constexpr int kQ = kBlockM * D * 2;         // bytes of the Q tile (kBlockM rows per 64-feature chunk)
   static constexpr int kStages = (D == 64) ? 4 : 2;   // K / V ring depth
   static constexpr int kOffQ = 0;
-  static constexpr int kOffK = kTile;
+  static constexpr int kOffK = kQ;
   static constexpr int kOffV = kOffK + kStages * kTile;
   static constexpr int kOffBar = kOffV + kStages * kTile;
   static constexpr int kSmem = kOffBar + 256 + 1024;  // + alignment slack
-  static constexpr int kThreads = 384;                // producer warpgroup + 2 consumer warpgroups
+  static_assert(kQ % 1024 == 0, "operand tiles start on 1024-byte swizzle atoms");
   static_assert(kSmem <= 232448, "forward kernel shared memory");
 };
 
@@ -72,13 +83,13 @@ using FwdArgsOf = std::conditional_t<WINDOW, Windowed<std::conditional_t<VARLEN,
 // WINDOW: sliding-window attention (Windowed<>::window = W).  A block visits key tiles [j_lo, NT) instead of
 // [0, NT): j_lo is the tile of the smallest lower limit of its rows, and NT moves up by W - 1 when not causal.
 template <typename T, int D, bool BIAS = false, bool VARLEN = false, bool WINDOW = false>
-__global__ void __launch_bounds__(384, 1)
+__global__ void __launch_bounds__(FwdCfg<D>::kThreads, 1)
 fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                 const __grid_constant__ CUtensorMap tm_v, const FwdArgsOf<VARLEN, WINDOW> a) {
   static_assert(!(BIAS && VARLEN), "packed sequences take no bias");
   static_assert(!(BIAS && WINDOW), "a window takes no bias");
   using Cfg = FwdCfg<D>;
-  constexpr int S = Cfg::kStages, TILE = Cfg::kTile, DCH = D / 64;
+  constexpr int S = Cfg::kStages, TILE = Cfg::kTile, DCH = D / 64, BM = Cfg::kBlockM;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
@@ -96,7 +107,7 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int wg = warp >> 2;
   pdl_launch_dependents();
 
-  // ---- work item: 128 query rows of one (batch, head) ------------------------------------
+  // ---- work item: BM query rows of one (batch, head) ------------------------------------
   // (the heads of one (batch, query block) are consecutive CTAs: the `group` heads sharing a key/value head
   // stream the same K / V tiles close together in time and meet in L2)
   const int bh_count = a.B * a.H;
@@ -105,7 +116,7 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int qblk = a.causal ? (a.n_qblk - 1 - rank) : rank;   // heaviest causal blocks first
   const int b = bh / a.H, h = bh - b * a.H;
   const int hk = h / a.group;
-  const int m0 = qblk * 128;
+  const int m0 = qblk * BM;
   // the (batch) coordinate of the tensor maps and the first query / key row of the sequence: packed sequences are
   // row offsets into maps of batch extent 1; their lengths are read after pdl_wait (a previous kernel may write them)
   const int tb = VARLEN ? 0 : b;
@@ -115,9 +126,9 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     mbar_init(BAR(Q_FULL), 1);
     for (int s = 0; s < S; ++s) {
       mbar_init(BAR(K_FULL + s), 1);
-      mbar_init(BAR(K_EMPTY + s), 256);
+      mbar_init(BAR(K_EMPTY + s), 128 * Cfg::kConsumers);
       mbar_init(BAR(V_FULL + s), 1);
-      mbar_init(BAR(V_EMPTY + s), 256);
+      mbar_init(BAR(V_EMPTY + s), 128 * Cfg::kConsumers);
     }
     fence_mbar_init();
   }
@@ -131,13 +142,13 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int off = Nk - Nq;
   int NT = (Nk + 127) >> 7;                                   // key tiles this block visits
   if (a.causal) {
-    const int last_col = min(m0 + 127, Nq - 1) + off;
+    const int last_col = min(m0 + BM - 1, Nq - 1) + off;
     NT = last_col < 0 ? 0 : min(NT, (last_col >> 7) + 1);
   }
   int W = 0, j_lo = 0;                                        // the window and the first key tile visited
   if constexpr (WINDOW) {
     W = a.window;
-    const int last_col = min(m0 + 127, Nq - 1) + off + (a.causal ? 0 : W - 1);
+    const int last_col = min(m0 + BM - 1, Nq - 1) + off + (a.causal ? 0 : W - 1);
     NT = last_col < 0 ? 0 : min((Nk + 127) >> 7, (last_col >> 7) + 1);
     const int first_col = m0 + off - W + 1;                   // the lower limit of the block's first row
     j_lo = first_col <= 0 ? 0 : min(first_col >> 7, NT);
@@ -145,14 +156,14 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
   if (wg == 0) {
     // =============================== TMA producer ===============================
-    reg_dealloc<kProducerRegs>();
+    reg_dealloc<Cfg::kProducerRegs>();
     if (warp == 0 && elect_one() && NT > j_lo) {
       tma_prefetch_desc(&tm_q);
       tma_prefetch_desc(&tm_k);
       tma_prefetch_desc(&tm_v);
-      mbar_expect_tx(BAR(Q_FULL), TILE);
+      mbar_expect_tx(BAR(Q_FULL), Cfg::kQ);
 #pragma unroll
-      for (int ch = 0; ch < DCH; ++ch) tma_load_4d(sQ + ch * 16384, &tm_q, BAR(Q_FULL), ch * 64, q_row0 + m0, h, tb);
+      for (int ch = 0; ch < DCH; ++ch) tma_load_4d(sQ + ch * BM * 128, &tm_q, BAR(Q_FULL), ch * 64, q_row0 + m0, h, tb);
       for (int j = j_lo; j < NT; ++j) {
         const int s = (j - j_lo) % S;
         const uint32_t par = (((j - j_lo) / S) & 1) ^ 1;
@@ -172,8 +183,8 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   }
 
   // =============================== consumer warpgroups =========================
-  reg_alloc<kConsumerRegs>();
-  const int w = wg - 1;                       // which 64 of the block's 128 query rows
+  reg_alloc<Cfg::kConsumerRegs>();
+  const int w = wg - 1;                       // which 64 of the block's BM query rows
   const int wl = warp & 3;
   // this thread's two rows (accumulator layout, sm90_primitives.cuh): row_a and row_a + 8
   const int row_a = m0 + 64 * w + 16 * wl + (lane >> 2);
@@ -203,6 +214,21 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       if (!a.causal) lim[hf] = min(Nk - 1, row_a + 8 * hf + off + W - 1);
     }
   }
+  // The key tiles [jw_lo, jw_hi) this warpgroup's own 64 rows see: the block's rules applied to its first and last
+  // row.  On the block's other tiles every p of these rows is 0 (with 192-row blocks, the trailing causal tiles of
+  // the first warpgroups and all tiles of rows past the end), so the warpgroup only passes their ring slots on.
+  const int r0 = m0 + 64 * w;
+  int jw_lo = j_lo, jw_hi = NT;
+  if (r0 >= Nq) {
+    jw_hi = 0;
+  } else if (a.causal || WINDOW) {
+    const int last_col = min(r0 + 63, Nq - 1) + off + (a.causal ? 0 : W - 1);
+    jw_hi = last_col < 0 ? 0 : (last_col >> 7) + 1;
+  }
+  if constexpr (WINDOW) {
+    const int first_col = r0 + off - W + 1;
+    if (first_col > 0) jw_lo = max(j_lo, first_col >> 7);
+  }
 
   float o[D / 2];
 #pragma unroll
@@ -214,15 +240,22 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   for (int j = j_lo; j < NT; ++j) {
     const int s = (j - j_lo) % S;
     const uint32_t par = ((j - j_lo) / S) & 1;
+    if (j < jw_lo || j >= jw_hi) {            // (after the FULL wait: an arrival must count for this use of the slot)
+      mbar_wait(BAR(K_FULL + s), par);
+      mbar_arrive(BAR(K_EMPTY + s));
+      mbar_wait(BAR(V_FULL + s), par);
+      mbar_arrive(BAR(V_EMPTY + s));
+      continue;
+    }
     // ---- S = Q K^T (64 x 128, fp32) ----
     float sacc[64];
     mbar_wait(BAR(K_FULL + s), par);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk) {
-      const uint32_t ko = (kk >> 2) * 16384 + (kk & 3) * 32;
-      wgmma_ss_n128<T, 0, 0>(sacc, gmma_desc_sw128(sQw + ko, 16, 1024),
-                             gmma_desc_sw128(sK + s * TILE + ko, 16, 1024), kk > 0 ? 1u : 0u);
+      const uint32_t ko = (kk & 3) * 32;       // + the 64-feature chunk (kk >> 2) below
+      wgmma_ss_n128<T, 0, 0>(sacc, gmma_desc_sw128(sQw + (kk >> 2) * BM * 128 + ko, 16, 1024),
+                             gmma_desc_sw128(sK + s * TILE + (kk >> 2) * 16384 + ko, 16, 1024), kk > 0 ? 1u : 0u);
     }
     wgmma_commit();
     wgmma_wait<0>();

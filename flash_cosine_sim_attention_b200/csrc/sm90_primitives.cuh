@@ -167,6 +167,10 @@ __device__ __forceinline__ void bulk_wait() {
 // warpgroups): 128 x 40 + 256 x 232 = 384 x 168, the pool a CTA of __launch_bounds__(384, 1) is launched with.
 constexpr int kProducerRegs = 40;
 constexpr int kConsumerRegs = 232;
+// The same for 512 threads (one producer, three consumer warpgroups: the D = 64 forward):
+// 128 x 24 + 384 x 160 = 64512 <= 65536, the pool of __launch_bounds__(512, 1) (128 per thread).
+constexpr int kProducerRegs3 = 24;
+constexpr int kConsumerRegs3 = 160;
 
 // register re-budgeting between warpgroups (all warps of a warpgroup must execute it)
 template <int N>
