@@ -91,18 +91,21 @@ def _f64(t, device):
 
 def attention_bounds(q, k, v, d_out=None, mask=None, attn_bias=None, scale=8, groups=1, causal=False,
                      l2norm_qk=True, attn_bias_batch_dim=False, round_qk=None, fmt="bf16", shift=None,
-                     device=None, chunk=1024):
+                     device=None, chunk=1024, eta=None, ds_scale=1.0):
     """float64 reference and per-element bound M of cosine-sim attention (module docstring).
 
     fmt: the kernels' operand type ("bf16" | "f16"), which sets u and eta.  round_qk: the type q^, k^ are stored in
     before the attention (as `oracle.attention`).  shift: the kernels' logit shift (`kernel_shift`); it only enters
-    the eta term of o, and None takes each row's maximum.  Returns (ref, bound): dicts over QUANTITIES (o only
-    without d_out, d_bias only with a bias) of float64 tensors on `device` shaped like the inputs."""
+    the eta term of o, and None takes each row's maximum.  eta: overrides the format's eta (0 gives the bound without
+    the subnormal terms, to measure their share).  ds_scale: how many times smaller the kernels' dS is than the
+    caller's (the float32 path runs them on v / sv and dO / pg, so on dS / (sv pg)); the eta of dS's rounding counts
+    that many times over in the caller's units.  Returns (ref, bound): dicts over QUANTITIES (o only without d_out,
+    d_bias only with a bias) of float64 tensors on `device` shaped like the inputs."""
     device = device or (q.device if torch.is_tensor(q) else "cpu")
     q, k, v, do, bias = (_f64(t, device) for t in (q, k, v, d_out, attn_bias))
     mask = None if mask is None else torch.as_tensor(mask).to(device=device, dtype=torch.bool)
     assert not (causal and mask is not None)
-    u, eta = U[fmt], ETA[fmt]
+    u, eta = U[fmt], (ETA[fmt] if eta is None else eta)
     merged, single = q.ndim == 3, k.ndim == 3
     if merged:
         q, k, v = q[:, None], k[:, None], v[:, None]
@@ -131,18 +134,20 @@ def attention_bounds(q, k, v, d_out=None, mask=None, attn_bias=None, scale=8, gr
     for b in range(B):
         for h in range(H):
             hk = h // G
-            kb, vb = kn[b, hk], v[b, hk]
             for r0 in range(0, Nq, chunk):
                 r1 = min(Nq, r0 + chunk)
+                # causal: the keys past the chunk's last visible one contribute exactly 0, so they are left out
+                ke = min(Nk, max(1, r1 + off)) if causal else Nk
+                kb, vb = kn[b, hk, :ke], v[b, hk, :ke]
                 rows = torch.arange(r0, r1, device=device)
-                vis = torch.ones(r1 - r0, Nk, dtype=torch.bool, device=device)
+                vis = torch.ones(r1 - r0, ke, dtype=torch.bool, device=device)
                 if causal:
-                    vis &= cols[None, :] <= rows[:, None] + off
+                    vis &= cols[None, :ke] <= rows[:, None] + off
                 if mask is not None:
-                    vis &= mask[b][None, :]
+                    vis &= mask[b][None, :ke]
                 s = scale * (qn[b, h, r0:r1] @ kb.T)
                 if bias is not None:
-                    s = s + bias[b if attn_bias_batch_dim else h, r0:r1]
+                    s = s + bias[b if attn_bias_batch_dim else h, r0:r1, :ke]
                 s = s.masked_fill(~vis, -math.inf)
                 anyv = vis.any(-1)
                 m = torch.where(anyv, s.amax(-1), torch.zeros_like(s[:, 0]))
@@ -161,21 +166,21 @@ def attention_bounds(q, k, v, d_out=None, mask=None, attn_bias=None, scale=8, gr
                 if not grads:
                     continue
                 dob = do[b, h, r0:r1]
-                dv[b, hk] += P.T @ dob
-                Mdv[b, hk] += P.T @ dob.abs() + (eta / u) * (visf.T @ dob.abs())
+                dv[b, hk, :ke] += P.T @ dob
+                Mdv[b, hk, :ke] += P.T @ dob.abs() + (eta / u) * (visf.T @ dob.abs())
                 dp = dob @ vb.T
                 delta = (dob * ob).sum(-1, keepdim=True)
                 ds = P * (dp - delta)
-                A = ds.abs() + P * (dob.abs() * ob.abs()).sum(-1, keepdim=True) + (eta / u) * visf
+                A = ds.abs() + P * (dob.abs() * ob.abs()).sum(-1, keepdim=True) + (eta / u) * ds_scale * visf
                 dqn[b, h, r0:r1] = scale * (ds @ kb)
                 Mdq[b, h, r0:r1] = scale * (A @ kb.abs())
                 qb = qn[b, h, r0:r1]
-                dkn[b, hk] += scale * (ds.T @ qb)
-                Mdk[b, hk] += scale * (A.T @ qb.abs())
+                dkn[b, hk, :ke] += scale * (ds.T @ qb)
+                Mdk[b, hk, :ke] += scale * (A.T @ qb.abs())
                 if bias is not None:
                     i = b if attn_bias_batch_dim else h
-                    dbias[i, r0:r1] += ds
-                    Mdb[i, r0:r1] += A
+                    dbias[i, r0:r1, :ke] += ds
+                    Mdb[i, r0:r1, :ke] += A
     ref, bound = {"o": o}, {"o": Mo}
     if grads:
         Mdq += dqn.abs()

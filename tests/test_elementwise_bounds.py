@@ -137,6 +137,78 @@ def _l2bwd(dy, y, n, groups):
     return ((d - g * (g * d).sum(-1, keepdims=True)) * rn[..., None]).reshape(y.shape)
 
 
+def emulate_long_causal(q, k, v, do, fmt, rows=512, scale=8):
+    """`emulate` for one causal (1, 1, N, D) problem at long N, in torch float32 on the CPU, chunked over query rows.
+    The fp32 sums run as in the kernels: the row sum l, O = P~ V and dQ = dS~ K are summed tile by tile over 128 keys
+    (each tile's partial in fp32, the tiles added one after another), dK and dV over the query rows.  Returns
+    [o, dq, dk, dv] as (1, 1, N, D) float64 tensors."""
+    dt = torch.bfloat16 if fmt == "bf16" else torch.float16
+    T = lambda x: x.to(dt).float()
+    Tp = (lambda x: T(x.clamp(max=65504.0))) if fmt == "f16" else T
+    shift = float(kernel_shift(fmt, scale))
+    f = lambda x: torch.from_numpy(np.ascontiguousarray(x[0, 0])).float()
+    q, k, v, do = f(q), f(k), f(v), f(do)
+    qn, kn = T(q / q.norm(dim=-1, keepdim=True)), T(k / k.norm(dim=-1, keepdim=True))
+    N, D = q.shape
+    o, dqn = torch.zeros(N, D), torch.zeros(N, D)
+    dkn, dv = torch.zeros(N, D), torch.zeros(N, D)
+
+    def tile_sum(x, y):
+        """sum over the key tiles of x[:, tile] @ y[tile], one tile after another, in fp32"""
+        nt = x.shape[1] // 128
+        part = torch.bmm(x.reshape(-1, nt, 128).transpose(0, 1), y.reshape(nt, 128, -1))
+        acc = torch.zeros_like(part[0])
+        for t in range(nt):
+            acc += part[t]
+        return acc
+
+    for r0 in range(0, N, rows):
+        r1 = min(N, r0 + rows)
+        ke = (r1 + 127) // 128 * 128                   # whole key tiles up to the chunk's last visible key
+        kp = torch.zeros(ke, D)
+        vp = torch.zeros(ke, D)
+        kp[:min(ke, N)], vp[:min(ke, N)] = kn[:ke], v[:ke]
+        cols = torch.arange(ke)
+        vis = cols[None, :] <= torch.arange(r0, r1)[:, None]
+        p = torch.where(vis, torch.exp(scale * (qn[r0:r1] @ kp.T) - shift), torch.zeros(()))
+        lt = p.reshape(r1 - r0, -1, 128).sum(-1)
+        l = torch.zeros(r1 - r0)
+        for t in range(lt.shape[1]):
+            l += lt[:, t]
+        inv_l = 1.0 / l.clamp_min(1e-37)
+        ob = T(tile_sum(Tp(p), vp) * inv_l[:, None])
+        o[r0:r1] = ob
+        dob = do[r0:r1]
+        delta = (dob * ob).sum(-1, keepdim=True)
+        P = p * inv_l[:, None]
+        dv[:ke] += (T(P).T @ dob)[:min(ke, N)]
+        dsr = T(P * (dob @ vp.T - delta))
+        dqn[r0:r1] = scale * tile_sum(dsr, kp)
+        dkn[:ke] += (scale * (dsr.T @ qn[r0:r1]))[:min(ke, N)]
+    l2 = lambda dy, x, y: (dy - y * (y * dy).sum(-1, keepdim=True)) / x.norm(dim=-1, keepdim=True)
+    out = [T(o), T(l2(dqn, q, qn)), T(l2(dkn, k, kn)), T(dv)]
+    return [t.double()[None, None] for t in out]
+
+
+@pytest.mark.parametrize("fmt", ["bf16", "f16"])
+def test_emulated_rounding_within_bound_at_32k(fmt, capsys):
+    """Causal (1, 1, 32768, 64): the emulation's worst err / (u M) stays within C / 2 where fp16 P ~ 1/N and dS are
+    subnormal and the fp32 sums run over 256 key tiles, so C = 2 holds at long context too."""
+    N = 32768
+    rng = np.random.default_rng(5)
+    q, k, v, do = (oracle.round_to(rng.standard_normal((1, 1, N, 64)), fmt) for _ in range(4))
+    got = emulate_long_causal(q, k, v, do, fmt)
+    ref, bound = attention_bounds(q, k, v, do, causal=True, round_qk=fmt, fmt=fmt, shift=kernel_shift(fmt, 8),
+                                  chunk=512)
+    worst = {}
+    for n, g in zip(("o", "dq", "dk", "dv"), got):
+        worst[n] = check_bound(n, g, ref, bound, fmt, c=C / 2) * C / 2
+        EMULATION_WORST[f"{fmt}:{n}@32k"] = worst[n]
+    with capsys.disabled():
+        print(f"\n  emulation at causal 32768 x 64, {fmt}: worst err / (u M) "
+              + "  ".join(f"{n} {w:.3f}" for n, w in worst.items()), end="")
+
+
 EMULATION_WORST = {}
 
 

@@ -78,6 +78,16 @@ def float32_operands(q, k, v, do, attn_bias=None, scale=8, groups=1, l2norm_qk=T
     return fmt, q, k, scaled(v), None if do is None else scaled(do), round_to(attn_bias, fmt)
 
 
+def float32_ds_scale(v, do):
+    """sv * pg: the float32 path runs the kernels on v / sv and dO / pg (`_pow2_scale`), so the dS they round to 16 bit
+    is the caller's dS / (sv pg), and the absolute eta of that rounding counts sv pg times over in the caller's units."""
+    if do is None:
+        return 1.0
+    from flash_cosine_sim_attention_b200.flash_cosine_sim_attention import _pow2_scale
+    f = lambda t: torch.as_tensor(t).detach().float()
+    return float(_pow2_scale(f(v), 1) * _pow2_scale(f(do), 1))
+
+
 def bound_check(dtype, got, q, k, v, do=None, mask=None, **kw):
     """The element-wise bound of every output in `got` ({name: tensor}) against the float64 reference of the same
     inputs, computed on the GPU; records the worst err / (C u M) per dtype and quantity under '<name>/bound'.
@@ -85,6 +95,7 @@ def bound_check(dtype, got, q, k, v, do=None, mask=None, **kw):
     l2 = kw.get("l2norm_qk", True)
     bias = kw.get("attn_bias")
     if dtype == torch.float32:
+        kw["ds_scale"] = float32_ds_scale(v, do)
         fmt, q, k, v, do, kw["attn_bias"] = float32_operands(q, k, v, do, bias, kw.get("scale", 8),
                                                              kw.get("groups", 1), l2)
     else:

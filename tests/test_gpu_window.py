@@ -14,7 +14,7 @@ import torch
 from elementwise_bounds import FMT, check_bound, kernel_shift
 from window_bounds import window_attention_bounds
 from test_gpu_gqa import group_split, loop_batch, sm_count
-from test_gpu_parity import TOL_GRAD, TOL_OUT, fcsa, float32_operands, make_inputs, record  # noqa: F401
+from test_gpu_parity import TOL_GRAD, TOL_OUT, fcsa, float32_ds_scale, float32_operands, make_inputs, record  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -48,13 +48,16 @@ def wcheck(fcsa, qs, kvs, dtype, window, seed=0, mask_p=None, path=None, grads=T
             assert launched >= 5, launched
         got.update(dq=qd.grad, dk=kd.grad, dv=vd.grad)
     l2 = kw.get("l2norm_qk", True)
+    ds_scale = 1.0
     if dtype == torch.float32:
+        ds_scale = float32_ds_scale(v, do if grads else None)
         fmt, q, k, v, do, _ = float32_operands(q, k, v, do, None, kw.get("scale", 8), kw.get("groups", 1), l2)
     else:
         fmt = FMT[dtype]
     shift = kernel_shift(fmt, kw.get("scale", 8), kw.get("groups", 1), l2)
     ref, bound = window_attention_bounds(q, k, v, do if grads else None, mask=mask, round_qk=fmt if l2 else None,
-                                         fmt=fmt, shift=shift, device="cuda", window=window, **kw)
+                                         fmt=fmt, shift=shift, device="cuda", window=window,
+                                         ds_scale=ds_scale, **kw)
     for name, t in got.items():
         assert t.shape == ref[name].shape
         record(dtype, f"window:{name}/bound", check_bound(name, t, ref, bound, fmt), 1.0)

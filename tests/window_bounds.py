@@ -13,9 +13,10 @@ from elementwise_bounds import ETA, U, _f64, _l2norm, _l2norm_backward, _l2norm_
 
 
 def window_attention_bounds(q, k, v, d_out=None, mask=None, window=None, scale=8, groups=1, causal=False,
-                            l2norm_qk=True, round_qk=None, fmt="bf16", shift=None, device=None, chunk=1024):
+                            l2norm_qk=True, round_qk=None, fmt="bf16", shift=None, device=None, chunk=1024,
+                            ds_scale=1.0):
     """(ref, bound) dicts over o (and dq, dk, dv with d_out) of float64 tensors on `device`, shaped like the inputs.
-    window=None is no window."""
+    window=None is no window.  ds_scale: as in attention_bounds."""
     device = device or (q.device if torch.is_tensor(q) else "cpu")
     q, k, v, do = (_f64(t, device) for t in (q, k, v, d_out))
     mask = None if mask is None else torch.as_tensor(mask).to(device=device, dtype=torch.bool)
@@ -47,17 +48,23 @@ def window_attention_bounds(q, k, v, d_out=None, mask=None, window=None, scale=8
     for b in range(B):
         for h in range(H):
             hk = h // G
-            kb, vb = kn[b, hk], v[b, hk]
             for r0 in range(0, Nq, chunk):
                 r1 = min(Nq, r0 + chunk)
-                d = torch.arange(r0, r1, device=device)[:, None] + off - cols[None, :]
+                # keys [k0, ke) hold every key the chunk's rows can see; the others contribute exactly 0 (as in
+                # attention_bounds, and the same range when the band hides nothing)
+                ke = Nk
+                if causal or window is not None:
+                    ke = min(Nk, max(1, r1 + off + (0 if causal else window - 1)))
+                k0 = 0 if window is None else min(ke - 1, max(0, r0 + off - window + 1))
+                kb, vb = kn[b, hk, k0:ke], v[b, hk, k0:ke]
+                d = torch.arange(r0, r1, device=device)[:, None] + off - cols[None, k0:ke]
                 vis = torch.ones_like(d, dtype=torch.bool)
                 if causal:
                     vis &= d >= 0
                 if window is not None:
                     vis &= (d < window) if causal else (d.abs() < window)
                 if mask is not None:
-                    vis &= mask[b][None, :]
+                    vis &= mask[b][None, k0:ke]
                 anyv = vis.any(-1)
                 visf = vis.double()
                 s = (scale * (qn[b, h, r0:r1] @ kb.T)).masked_fill(~vis, -math.inf)
@@ -74,15 +81,15 @@ def window_attention_bounds(q, k, v, d_out=None, mask=None, window=None, scale=8
                 if not grads:
                     continue
                 dob = do[b, h, r0:r1]
-                dv[b, hk] += P.T @ dob
-                Mdv[b, hk] += P.T @ dob.abs() + (eta / u) * (visf.T @ dob.abs())
+                dv[b, hk, k0:ke] += P.T @ dob
+                Mdv[b, hk, k0:ke] += P.T @ dob.abs() + (eta / u) * (visf.T @ dob.abs())
                 ds = P * (dob @ vb.T - (dob * ob).sum(-1, keepdim=True))
-                A = ds.abs() + P * (dob.abs() * ob.abs()).sum(-1, keepdim=True) + (eta / u) * visf
+                A = ds.abs() + P * (dob.abs() * ob.abs()).sum(-1, keepdim=True) + (eta / u) * ds_scale * visf
                 dqn[b, h, r0:r1] = scale * (ds @ kb)
                 Mdq[b, h, r0:r1] = scale * (A @ kb.abs())
                 qb = qn[b, h, r0:r1]
-                dkn[b, hk] += scale * (ds.T @ qb)
-                Mdk[b, hk] += scale * (A.T @ qb.abs())
+                dkn[b, hk, k0:ke] += scale * (ds.T @ qb)
+                Mdk[b, hk, k0:ke] += scale * (A.T @ qb.abs())
     ref, bound = {"o": o}, {"o": Mo}
     if grads:
         Mdq += dqn.abs()
