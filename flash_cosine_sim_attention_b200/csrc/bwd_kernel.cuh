@@ -1056,242 +1056,4 @@ __global__ void __launch_bounds__(256) bwd_kv_finish_kernel(const KvFinishArgs a
   *reinterpret_cast<uint4*>(dst) = o4;
 }
 
-// ------------------------------------------------------------------------------------------
-// host runner
-// ------------------------------------------------------------------------------------------
-struct BwdHostArgs {
-  bool dtype_bf16;
-  int B, H, kv_heads, Nq, Nk, D, causal;
-  int window = 0;                   // sliding window W (0 = none; never with a bias)
-  float scale, shift;
-  const uint8_t* mask; long long mask_sb;
-  fcsa_tensor q, k, v, o, d_o, dq, dk, dv;
-  const float* inv_l;
-  bool out_f32 = false;             // o (read), dq, dk, dv (written) are float32
-  void* workspace;                  // scratch
-  void* zeroed;                     // zero on entry, zero again on exit (dq accumulator)
-  cudaEvent_t ev_start = nullptr, ev_stop = nullptr;   // optional: recorded around the main kernel
-  cudaEvent_t ev_prep[2] = {nullptr, nullptr}, ev_finish[2] = {nullptr, nullptr};   // ... the preprocess / dq finish
-  // fused l2norm backward (q, k above are then the NORMALISED tensors and dq, dk the gradients
-  // w.r.t. the raw ones); both null = plain backward
-  const float* q_rnorm = nullptr;
-  const float* k_rnorm = nullptr;
-  int groups = 1;
-  // additive bias (nullptr = none) and its fp32 gradient accumulator (nullptr = not needed)
-  const void* bias = nullptr; long long bias_sb = 0, bias_sh = 0, bias_sn = 0;
-  const float* bias_amax = nullptr;           // optional device scalar added (if positive) to the shift
-  float* dbias = nullptr; long long dbias_sb = 0, dbias_sh = 0;
-  // packed sequences (run_backward_varlen): B sequences, Nq / Nk the maximum lengths, q, d_o, o, dq (total_q, H, D)
-  // and k, v, dk, dv (total_k, kv_heads, D) with sb unused, inv_l (H, total_q), the rnorms [heads][total][groups]
-  const int* cu_q = nullptr;
-  const int* cu_k = nullptr;
-  int total_q = 0, total_k = 0;
-};
-
-// Slices per key/value-head group (query heads per CTA = G / split).  One CTA per group keeps dk / dv in registers
-// (no accumulator, no finish pass, bitwise reproducible), but the grid then has B * kv_heads * key tiles CTAs; below
-// one CTA per SM the group is split into the fewest slices that fill the device.  Keys/values shared by all heads
-// (kv_heads == 1) and the BIAS kernels (no registers to spare for the head loop) take one query head per CTA.
-inline int bwd_group_split(int B, int H, int kv_heads, int Nk, bool bias, int sm_count) {
-  const int G = H / kv_heads;
-  if (G == 1) return 1;
-  if (bias || kv_heads == 1) return G;
-  const long long unsplit = (long long)((Nk + 127) / 128) * B * kv_heads;
-  if (unsplit >= sm_count) return 1;
-  for (int s = 2; s < G; ++s)
-    if (G % s == 0 && unsplit * s >= sm_count) return s;
-  return G;
-}
-
-template <typename T, int D, bool BIAS = false, bool VARLEN = false>
-int run_backward_t(const BwdHostArgs& h, cudaStream_t stream, int* launches, const char** err,
-                   cudaError_t* ce) {
-  using Cfg = BwdCfg<D>;
-  const BwdWorkspace w = VARLEN ? bwd_varlen_workspace_layout(h.B, h.H, h.kv_heads, h.total_q, h.total_k, D)
-                                : bwd_workspace_layout(h.B, h.H, h.kv_heads, h.Nq, h.Nk, D);
-  // the batch, key rows and query tiles of the tensors as addressed: packed sequences are one batch of total rows
-  const int tB = VARLEN ? 1 : h.B, tNq = VARLEN ? h.total_q : h.Nq, tNk = VARLEN ? h.total_k : h.Nk;
-  const int nqt = (h.Nq + Cfg::QT - 1) / Cfg::QT;     // query tiles of the longest sequence
-  uint8_t* ws = reinterpret_cast<uint8_t*>(h.workspace);
-  uint8_t* zs = reinterpret_cast<uint8_t*>(h.zeroed);
-  float* stats = reinterpret_cast<float*>(ws + w.stats_off);
-  float* dq_acc = reinterpret_cast<float*>(zs + w.dq_off);
-  float* dkv_acc = reinterpret_cast<float*>(ws + w.dkv_off);
-  const float log2e = 1.4426950408889634f;
-  cudaError_t e;
-  int split = 1;
-  if (h.kv_heads < h.H) {
-    int sms = 0;
-    e = device_sm_count(&sms);
-    if (e != cudaSuccess) { *err = "cudaDeviceGetAttribute(multiProcessorCount)"; *ce = e; return FCSA_ERR_CUDA; }
-    split = bwd_group_split(h.B, h.H, h.kv_heads, h.Nk, BIAS, sms);
-  }
-  const bool to_acc = split > 1;
-  const size_t dkv_elems = (size_t)tB * h.kv_heads * tNk * D;
-
-  // dk/dv accumulators of split groups are per call (the dq accumulator is self-cleaning)
-  if (to_acc) {
-    e = cudaMemsetAsync(dkv_acc, 0, 2 * dkv_elems * 4, stream);
-    if (e != cudaSuccess) { *err = "cudaMemsetAsync(workspace)"; *ce = e; return FCSA_ERR_CUDA; }
-  }
-
-  // 1. preprocess
-  {
-    std::conditional_t<VARLEN, PrepVarlenArgs, PrepArgs> pa;
-    pa.B = h.B; pa.H = h.H; pa.Nq = h.Nq; pa.Nk = h.Nk; pa.D = D; pa.nqt = nqt; pa.QT = Cfg::QT; pa.causal = h.causal;
-    if constexpr (VARLEN) { pa.cu_q = h.cu_q; pa.total_q = h.total_q; pa.ntile = w.nqt; }
-    pa.c2 = h.shift * log2e;
-    pa.shift_extra = h.bias_amax;
-    pa.o_f32 = h.out_f32 ? 1 : 0;
-    pa.o = h.o.ptr; pa.o_sb = h.o.sb; pa.o_sh = h.o.sh; pa.o_sn = h.o.sn;
-    pa.d_o = h.d_o.ptr; pa.do_sb = h.d_o.sb; pa.do_sh = h.d_o.sh; pa.do_sn = h.d_o.sn;
-    pa.inv_l = h.inv_l; pa.stats = stats;
-    const int rows_per_block = 2 * (256 / (D / 8));
-    const int padded = nqt * Cfg::QT;
-    pa.bpb = (padded + rows_per_block - 1) / rows_per_block;
-    const long long grid = (long long)pa.bpb * h.B * h.H;
-    if (grid > 0x7FFFFFFFLL) { *err = "problem too large for one launch"; return FCSA_ERR_INVALID; }
-    if (h.ev_prep[0]) cudaEventRecord(h.ev_prep[0], stream);
-    e = launch_pdl(bwd_prep_kernel<T, D / 8, VARLEN>, dim3((unsigned)grid), dim3(256), 0, stream, pa);
-    if (h.ev_prep[1]) cudaEventRecord(h.ev_prep[1], stream);
-    if (e != cudaSuccess) { *err = "backward preprocess launch"; *ce = e; return FCSA_ERR_CUDA; }
-    ++*launches;
-  }
-  // 2. main
-  {
-    CUtensorMap tq, tk, tv, tdo, tdq;
-    const CUtensorMapDataType dt = tma_dtype16(h.dtype_bf16);
-    if (make_tensor_map_bhnd(&tq, h.q.ptr, dt, tB, h.H, tNq, D, h.q.sb, h.q.sh, h.q.sn, Cfg::QT) ||
-        make_tensor_map_bhnd(&tk, h.k.ptr, dt, tB, h.kv_heads, tNk, D, h.k.sb, h.k.sh, h.k.sn, 128) ||
-        make_tensor_map_bhnd(&tv, h.v.ptr, dt, tB, h.kv_heads, tNk, D, h.v.sb, h.v.sh, h.v.sn, 128) ||
-        make_tensor_map_bhnd(&tdo, h.d_o.ptr, dt, tB, h.H, tNq, D, h.d_o.sb, h.d_o.sh, h.d_o.sn, Cfg::QT)) {
-      *err = "cuTensorMapEncodeTiled failed (backward): q, k, v, d_o must be views a TMA tensor map can express "
-             "(positive strides, 16-byte aligned)";
-      return FCSA_ERR_INVALID;
-    }
-    // the dq accumulator as [B][H][Nq][D] fp32 over its padded rows: boxes of 32 features x QT rows (packed
-    // sequences: [1][H][ntile * QT][D], every tile inside the map)
-    memset(&tdq, 0, sizeof(tdq));
-    const long long acc_sh = (long long)w.nqt * Cfg::QT * D;
-    if (Cfg::kStaged &&
-        make_tensor_map_bhnd(&tdq, dq_acc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, tB, h.H, VARLEN ? w.nqt * Cfg::QT : h.Nq, D,
-                             h.H * acc_sh, acc_sh, D, Cfg::QT, 32)) {
-      *err = "cuTensorMapEncodeTiled failed (backward dq accumulator)";
-      return FCSA_ERR_CUDA;
-    }
-    // (the window's arguments extend the kernel's; the unwindowed launches pass the base)
-    BwdArgsOf<VARLEN, true> a;
-    a.window = h.window;
-    a.B = h.B; a.H = h.H; a.Nq = h.Nq; a.Nk = h.Nk; a.kv_heads = h.kv_heads; a.causal = h.causal;
-    a.has_mask = h.mask ? 1 : 0; a.nqt = w.nqt;
-    if constexpr (VARLEN) {
-      a.cu_q = h.cu_q; a.cu_k = h.cu_k; a.total_q = h.total_q; a.total_k = h.total_k; a.ntile = w.nqt;
-    }
-    a.split = split; a.hpc = h.H / h.kv_heads / split;
-    a.c1 = h.scale * log2e; a.scale = h.scale;
-    a.mask = h.mask; a.mask_sb = h.mask_sb;
-    a.stats = stats; a.dq_acc = dq_acc;
-    a.dk_acc = dkv_acc; a.dv_acc = dkv_acc + dkv_elems;
-    a.dk = h.dk.ptr; a.dk_sb = h.dk.sb; a.dk_sh = h.dk.sh; a.dk_sn = h.dk.sn;
-    a.dv = h.dv.ptr; a.dv_sb = h.dv.sb; a.dv_sh = h.dv.sh; a.dv_sn = h.dv.sn;
-    a.bias = h.bias; a.bias_sb = h.bias_sb; a.bias_sh = h.bias_sh; a.bias_sn = h.bias_sn;
-    a.dbias = h.dbias; a.dbias_sb = h.dbias_sb; a.dbias_sh = h.dbias_sh;
-    a.out_f32 = h.out_f32 ? 1 : 0;
-    a.k_rnorm = h.k_rnorm; a.groups = h.groups;
-    constexpr bool kLoop = !BIAS;
-    const std::conditional_t<VARLEN, BwdVarlenArgs, BwdArgs>& base = a;
-    const bool win = !BIAS && h.window > 0;
-    auto kern = a.hpc > 1 ? fcsa_bwd_kernel<T, D, BIAS, kLoop, VARLEN> : fcsa_bwd_kernel<T, D, BIAS, false, VARLEN>;
-    e = a.hpc > 1 ? ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS, kLoop, VARLEN>>(Cfg::kSmem)
-                  : ensure_dynamic_smem<fcsa_bwd_kernel<T, D, BIAS, false, VARLEN>>(Cfg::kSmem);
-    auto wkern = fcsa_bwd_kernel<T, D, false, false, VARLEN, !BIAS>;    // (BIAS: never launched)
-    if (win) {
-      wkern = a.hpc > 1 ? fcsa_bwd_kernel<T, D, false, kLoop, VARLEN, !BIAS> : wkern;
-      e = a.hpc > 1 ? ensure_dynamic_smem<fcsa_bwd_kernel<T, D, false, kLoop, VARLEN, !BIAS>>(Cfg::kSmem)
-                    : ensure_dynamic_smem<fcsa_bwd_kernel<T, D, false, false, VARLEN, !BIAS>>(Cfg::kSmem);
-    }
-    if (e != cudaSuccess) { *err = "cudaFuncSetAttribute(bwd)"; *ce = e; return FCSA_ERR_CUDA; }
-    // one CTA per (key tile, batch, kv head, slice of its group); packed sequences: key tiles of the longest one
-    const long long items = (long long)((h.Nk + 127) / 128) * h.B * h.kv_heads * split;
-    if (items > 0x7FFFFFFFLL) { *err = "problem too large for one launch"; return FCSA_ERR_INVALID; }
-    if (h.ev_start) cudaEventRecord(h.ev_start, stream);
-    e = win ? launch_pdl(wkern, dim3((unsigned)items), dim3(Cfg::kThreads), Cfg::kSmem, stream, tq, tk, tv, tdo, tdq, a)
-            : launch_pdl(kern, dim3((unsigned)items), dim3(Cfg::kThreads), Cfg::kSmem, stream, tq, tk, tv, tdo, tdq, base);
-    if (h.ev_stop) cudaEventRecord(h.ev_stop, stream);
-    if (e != cudaSuccess) { *err = "backward kernel launch"; *ce = e; return FCSA_ERR_CUDA; }
-    ++*launches;
-  }
-  // 3. finish
-  {
-    std::conditional_t<VARLEN, DqFinishVarlenArgs, DqFinishArgs> fa;
-    fa.B = h.B; fa.H = h.H; fa.Nq = h.Nq; fa.D = D; fa.nqt = w.nqt; fa.padded = w.nqt * Cfg::QT; fa.scale = h.scale;
-    if constexpr (VARLEN) { fa.padded = nqt * Cfg::QT; fa.cu_q = h.cu_q; fa.total_q = h.total_q; fa.ntile = w.nqt; }
-    fa.dq_acc = dq_acc; fa.dq = h.dq.ptr; fa.sb = h.dq.sb; fa.sh = h.dq.sh; fa.sn = h.dq.sn;
-    fa.q_hat = h.q.ptr; fa.q_sb = h.q.sb; fa.q_sh = h.q.sh; fa.q_sn = h.q.sn;
-    fa.q_rnorm = h.q_rnorm; fa.G = h.groups; fa.out_f32 = h.out_f32 ? 1 : 0;
-    const long long threads = (long long)h.B * h.H * (VARLEN ? fa.padded : h.Nq) * (D / 8);
-    const long long blocks = (threads + 255) / 256;
-    if (blocks > 0x7FFFFFFFLL) { *err = "problem too large for one launch"; return FCSA_ERR_INVALID; }
-    if (h.ev_finish[0]) cudaEventRecord(h.ev_finish[0], stream);
-    e = launch_pdl(bwd_dq_finish_kernel<T, D, VARLEN>, dim3((unsigned)blocks), dim3(256), 0, stream, fa);
-    if (h.ev_finish[1]) cudaEventRecord(h.ev_finish[1], stream);
-    if (e != cudaSuccess) { *err = "dq finish launch"; *ce = e; return FCSA_ERR_CUDA; }
-    ++*launches;
-    if (to_acc) {
-      for (int which = 0; which < 2; ++which) {
-        KvFinishArgs ka;
-        ka.B = tB; ka.Hk = h.kv_heads; ka.Nk = tNk; ka.D = D; ka.out_f32 = h.out_f32 ? 1 : 0;
-        ka.acc = dkv_acc + (which ? dkv_elems : 0);
-        const fcsa_tensor& t = which ? h.dv : h.dk;
-        ka.out = t.ptr; ka.sb = t.sb; ka.sh = t.sh; ka.sn = t.sn;
-        const long long tot = (long long)dkv_elems / 8;
-        bwd_kv_finish_kernel<T><<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(ka);
-        e = cudaGetLastError();
-        if (e != cudaSuccess) { *err = "dk/dv finish launch"; *ce = e; return FCSA_ERR_CUDA; }
-        ++*launches;
-      }
-    }
-    if (h.k_rnorm != nullptr && to_acc) {
-      // l2norm backward of dk (gradient w.r.t. the raw keys) as its own pass over the head-summed dk; otherwise
-      // the main kernel's epilogue applies it
-      RowArgs la = {};
-      la.B = tB; la.D = D; la.G = h.groups;
-      la.t[0] = {h.kv_heads, tNk, h.dk, h.k, h.dk, const_cast<float*>(h.k_rnorm)};
-      e = launch_row_bwd(la, h.dtype_bf16, false, stream);
-      if (e != cudaSuccess) { *err = "l2norm backward (dk) launch"; *ce = e; return FCSA_ERR_CUDA; }
-      ++*launches;
-    }
-  }
-  return FCSA_OK;
-}
-
-// packed sequences (h.cu_q, h.cu_k set); no bias, no mask, 16-bit outputs
-inline int run_backward_varlen(const BwdHostArgs& h, cudaStream_t stream, int* launches, const char** err,
-                               cudaError_t* ce) {
-  if (h.D == 64) {
-    if (h.dtype_bf16) return run_backward_t<__nv_bfloat16, 64, false, true>(h, stream, launches, err, ce);
-    return run_backward_t<__half, 64, false, true>(h, stream, launches, err, ce);
-  }
-  if (h.dtype_bf16) return run_backward_t<__nv_bfloat16, 128, false, true>(h, stream, launches, err, ce);
-  return run_backward_t<__half, 128, false, true>(h, stream, launches, err, ce);
-}
-
-inline int run_backward(const BwdHostArgs& h, cudaStream_t stream, int* launches, const char** err,
-                        cudaError_t* ce) {
-  if (h.bias != nullptr) {
-    if (h.D == 64) {
-      if (h.dtype_bf16) return run_backward_t<__nv_bfloat16, 64, true>(h, stream, launches, err, ce);
-      return run_backward_t<__half, 64, true>(h, stream, launches, err, ce);
-    }
-    if (h.dtype_bf16) return run_backward_t<__nv_bfloat16, 128, true>(h, stream, launches, err, ce);
-    return run_backward_t<__half, 128, true>(h, stream, launches, err, ce);
-  }
-  if (h.D == 64) {
-    if (h.dtype_bf16) return run_backward_t<__nv_bfloat16, 64>(h, stream, launches, err, ce);
-    return run_backward_t<__half, 64>(h, stream, launches, err, ce);
-  }
-  if (h.dtype_bf16) return run_backward_t<__nv_bfloat16, 128>(h, stream, launches, err, ce);
-  return run_backward_t<__half, 128>(h, stream, launches, err, ce);
-}
-
 }  // namespace fcsa

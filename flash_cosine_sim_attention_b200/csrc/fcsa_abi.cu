@@ -1,6 +1,6 @@
 // Host side of libfcsa_b200.so: argument validation, TMA tensor-map construction, the
-// {f16, bf16} x {64, 128} switch and the kernel launches behind the C ABI of
-// include/fcsa_b200.h.
+// {f16, bf16} x {64, 128} dispatch and the forward, decode, backward and row-pass launches behind
+// the C ABI of include/fcsa_b200.h.
 //
 // Replaces the reference's host op + pybind layer (flash_cosine_sim_attention_cuda.cu:1630-1933)
 // and its dispatch macros (dispatch.h:38-73).  Differences by design: launches go to the
@@ -15,6 +15,7 @@
 
 #include <algorithm>
 #include <atomic>
+#include <type_traits>
 
 #include "../../include/fcsa_b200.h"
 #include "bwd_kernel.cuh"
@@ -87,27 +88,77 @@ int check_bias(const fcsa_problem* p, const fcsa_bias* bias) {
   return FCSA_OK;
 }
 
+template <typename T>
+struct type_tag {
+  using type = T;
+};
+
+// Calls f(type_tag<T>{}, std::integral_constant<int, D>{}) with the element type and head dim of a checked problem:
+// the one place where the host code turns (dtype, head_dim) into template arguments.
+template <typename F>
+int dispatch(const fcsa_problem* p, F&& f) {
+  using D64 = std::integral_constant<int, 64>;
+  using D128 = std::integral_constant<int, 128>;
+  if (p->dtype == FCSA_BF16)
+    return p->head_dim == 64 ? f(type_tag<__nv_bfloat16>{}, D64{}) : f(type_tag<__nv_bfloat16>{}, D128{});
+  return p->head_dim == 64 ? f(type_tag<__half>{}, D64{}) : f(type_tag<__half>{}, D128{});
+}
+
+// The TMA map of a [b][h][n][D] operand of element type T (boxes of box_rows rows x 64 features).  A failure names
+// the operand.
+template <typename T, int D>
+int map_operand(CUtensorMap* tm, const char* name, const fcsa_tensor& t, int64_t B, int64_t H, int64_t N, int box_rows) {
+  const int r = fcsa::make_tensor_map_bhnd(tm, t.ptr, fcsa::tma_dtype16(std::is_same<T, __nv_bfloat16>::value), B, H,
+                                           N, D, t.sb, t.sh, t.sn, box_rows);
+  if (r == -2)
+    return fail(FCSA_ERR_INVALID, "%s: expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - "
+                "make the tensor contiguous (%d)", name, r);
+  if (r) return fail(FCSA_ERR_CUDA, "%s: cuTensorMapEncodeTiled failed (%d)", name, r);
+  return FCSA_OK;
+}
+
+// error and launch count of one launch
+int launched(cudaError_t e, const char* what) {
+  if (e != cudaSuccess) return cuda_fail(e, what);
+  g_launches.fetch_add(1);
+  return FCSA_OK;
+}
+
+// A kernel as a type, so that a site can pick one of several variants and pass it to a single launch
+template <auto Kern>
+using kernel_c = std::integral_constant<decltype(Kern), Kern>;
+
+// Launch of an attention kernel: its dynamic shared memory set once per (kernel, device), then a PDL launch between
+// the events ev[0] / ev[1] when they are set.  A kernel whose parameter is the base of `args`' window arguments
+// (the unwindowed variants) receives that base.
+template <auto Kern, typename... Args>
+int launch_attention(const char* what, const cudaEvent_t* ev, long long grid, int threads, int smem,
+                     cudaStream_t stream, const Args&... args) {
+  cudaError_t e = fcsa::ensure_dynamic_smem<Kern>(smem);
+  if (e != cudaSuccess) return fail(FCSA_ERR_CUDA, "cudaFuncSetAttribute(%s): %s", what, cudaGetErrorString(e));
+  if (ev && ev[0]) cudaEventRecord(ev[0], stream);
+  e = fcsa::launch_pdl(Kern, dim3((unsigned)grid), dim3(threads), smem, stream, args...);
+  if (ev && ev[1]) cudaEventRecord(ev[1], stream);
+  if (e != cudaSuccess) return fail(FCSA_ERR_CUDA, "%s kernel launch: %s", what, cudaGetErrorString(e));
+  g_launches.fetch_add(1);
+  return FCSA_OK;
+}
+
 // VARLEN: packed sequences (vl); q, k, v, o are then one batch of total_q / total_k rows
 template <typename T, int D, bool BIAS = false, bool VARLEN = false>
 int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
                    const fcsa_tensor* v, const fcsa_tensor* o, float* inv_l, cudaStream_t stream,
                    const fcsa_bias* bias = nullptr, const fcsa_varlen* vl = nullptr) {
   using Cfg = fcsa::FwdCfg<D>;
-  const bool bf = p->dtype == FCSA_BF16;
   const int tB = VARLEN ? 1 : p->batch, tNq = VARLEN ? vl->total_q : p->seq_q, tNk = VARLEN ? vl->total_k : p->seq_k;
   CUtensorMap tq, tk, tv;
   int r;
-  if ((r = fcsa::make_tensor_map_bhnd(&tq, q->ptr, fcsa::tma_dtype16(bf), tB, p->heads, tNq, D, q->sb, q->sh,
-                                      q->sn, Cfg::kBlockM)))       // Q: one box of the CTA's query rows
-    return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "q: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - make the tensor contiguous" : "cuTensorMapEncodeTiled failed", r);
-  if ((r = fcsa::make_tensor_map_bhnd(&tk, k->ptr, fcsa::tma_dtype16(bf), tB, p->kv_heads, tNk, D, k->sb,
-                                      k->sh, k->sn, 128)))
-    return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "k: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - make the tensor contiguous" : "cuTensorMapEncodeTiled failed", r);
-  if ((r = fcsa::make_tensor_map_bhnd(&tv, v->ptr, fcsa::tma_dtype16(bf), tB, p->kv_heads, tNk, D, v->sb,
-                                      v->sh, v->sn, 128)))
-    return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "v: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map - make the tensor contiguous" : "cuTensorMapEncodeTiled failed", r);
+  if ((r = map_operand<T, D>(&tq, "q", *q, tB, p->heads, tNq, Cfg::kBlockM)) ||   // Q: one box of the CTA's query rows
+      (r = map_operand<T, D>(&tk, "k", *k, tB, p->kv_heads, tNk, 128)) ||
+      (r = map_operand<T, D>(&tv, "v", *v, tB, p->kv_heads, tNk, 128)))
+    return r;
 
-  // (the window's arguments extend the kernel's; the unwindowed launch passes the base)
+  // (the window's arguments extend the kernel's)
   fcsa::FwdArgsOf<VARLEN, true> a;
   a.window = kernel_window(p);
   if constexpr (VARLEN) {
@@ -138,41 +189,18 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
   a.bias_sn = BIAS ? bias->sn : 0;
   a.bias_amax = BIAS ? bias->amax : nullptr;
 
-  const bool win = !BIAS && a.window > 0;
-  {
-    cudaError_t e;
-    if constexpr (BIAS) e = fcsa::ensure_dynamic_smem<fcsa::fcsa_fwd_kernel<T, D, BIAS, VARLEN>>(Cfg::kSmem);
-    else e = win ? fcsa::ensure_dynamic_smem<fcsa::fcsa_fwd_kernel<T, D, false, VARLEN, true>>(Cfg::kSmem)
-                 : fcsa::ensure_dynamic_smem<fcsa::fcsa_fwd_kernel<T, D, false, VARLEN>>(Cfg::kSmem);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(fwd)");
-  }
   // one CTA per (query block of kBlockM rows, batch, head); packed sequences: blocks of the longest sequence
   const long long grid = (long long)a.n_qblk * p->batch * p->heads;
   if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
-  if (g_ev[0][0]) cudaEventRecord(g_ev[0][0], stream);
-  const std::conditional_t<VARLEN, fcsa::FwdVarlenArgs, fcsa::FwdArgs>& base = a;
-  cudaError_t e;
-  if constexpr (BIAS) {
-    e = fcsa::launch_pdl(fcsa::fcsa_fwd_kernel<T, D, BIAS, VARLEN>, dim3((unsigned)grid), dim3(Cfg::kThreads),
-                         Cfg::kSmem, stream, tq, tk, tv, base);
-  } else if (win) {
-    e = fcsa::launch_pdl(fcsa::fcsa_fwd_kernel<T, D, false, VARLEN, true>, dim3((unsigned)grid), dim3(Cfg::kThreads),
-                         Cfg::kSmem, stream, tq, tk, tv, a);
-  } else {
-    e = fcsa::launch_pdl(fcsa::fcsa_fwd_kernel<T, D, false, VARLEN>, dim3((unsigned)grid), dim3(Cfg::kThreads),
-                         Cfg::kSmem, stream, tq, tk, tv, base);
-  }
-  if (g_ev[0][1]) cudaEventRecord(g_ev[0][1], stream);
-  if (e != cudaSuccess) return cuda_fail(e, "forward kernel launch");
-  g_launches.fetch_add(1);
-  return FCSA_OK;
-}
-
-// error and launch count of one row pass
-int row_pass_launched(cudaError_t e, const char* what) {
-  if (e != cudaSuccess) return cuda_fail(e, what);
-  g_launches.fetch_add(1);
-  return FCSA_OK;
+  const auto launch = [&](auto kern) {
+    return launch_attention<decltype(kern)::value>("forward", g_ev[0], grid, Cfg::kThreads, Cfg::kSmem, stream, tq, tk,
+                                                   tv, a);
+  };
+  if constexpr (BIAS)   // (a bias takes no window)
+    return launch(kernel_c<fcsa::fcsa_fwd_kernel<T, D, true>>{});
+  else
+    return a.window > 0 ? launch(kernel_c<fcsa::fcsa_fwd_kernel<T, D, false, VARLEN, true>>{})
+                        : launch(kernel_c<fcsa::fcsa_fwd_kernel<T, D, false, VARLEN>>{});
 }
 
 // Shapes of the row passes.  The 16-bit l2norm takes head dims 32 to 256 and groups > 0; the float32 cast takes
@@ -243,15 +271,11 @@ int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tenso
                   const fcsa_tensor* vc, const int32_t* seqlens, int32_t n_new, const fcsa_tensor* o, float* part,
                   cudaStream_t stream) {
   using Cfg = fcsa::DecodeCfg<D>;
-  const bool bf = p->dtype == FCSA_BF16;
   CUtensorMap tk, tv;
   int r;
-  if ((r = fcsa::make_tensor_map_bhnd(&tk, kc->ptr, fcsa::tma_dtype16(bf), p->batch, p->kv_heads, p->seq_k, D, kc->sb,
-                                      kc->sh, kc->sn, 128)))
-    return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "k_cache: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map" : "cuTensorMapEncodeTiled failed", r);
-  if ((r = fcsa::make_tensor_map_bhnd(&tv, vc->ptr, fcsa::tma_dtype16(bf), p->batch, p->kv_heads, p->seq_k, D, vc->sb,
-                                      vc->sh, vc->sn, 128)))
-    return fail(r == -2 ? FCSA_ERR_INVALID : FCSA_ERR_CUDA, "v_cache: %s (%d)", r == -2 ? "expanded (stride-0) views of extent > 1 cannot be addressed by a tensor map" : "cuTensorMapEncodeTiled failed", r);
+  if ((r = map_operand<T, D>(&tk, "k_cache", *kc, p->batch, p->kv_heads, p->seq_k, 128)) ||
+      (r = map_operand<T, D>(&tv, "v_cache", *vc, p->batch, p->kv_heads, p->seq_k, 128)))
+    return r;
   fcsa::Windowed<fcsa::DecodeArgs> a;
   a.window = kernel_window(p);
   a.B = p->batch; a.H = p->heads; a.KVH = p->kv_heads; a.G = p->heads / p->kv_heads;
@@ -265,28 +289,18 @@ int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tenso
   a.q = q->ptr; a.q_sb = q->sb; a.q_sh = q->sh; a.q_sn = q->sn;
   a.o = o->ptr; a.o_sb = o->sb; a.o_sh = o->sh; a.o_sn = o->sn;
   a.part = part;
-  const bool win = a.window > 0;
-  const fcsa::DecodeArgs& base = a;
-  {
-    cudaError_t e = win ? fcsa::ensure_dynamic_smem<fcsa::fcsa_decode_kernel<T, D, true>>(Cfg::kSmem)
-                        : fcsa::ensure_dynamic_smem<fcsa::fcsa_decode_kernel<T, D>>(Cfg::kSmem);
-    if (e != cudaSuccess) return cuda_fail(e, "cudaFuncSetAttribute(decode)");
-  }
   const long long grid = sh.items * sh.n_split;
   if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "decode: problem too large for one launch");
-  cudaError_t e = win ? fcsa::launch_pdl(fcsa::fcsa_decode_kernel<T, D, true>, dim3((unsigned)grid),
-                                         dim3(Cfg::kThreads), Cfg::kSmem, stream, tk, tv, a)
-                      : fcsa::launch_pdl(fcsa::fcsa_decode_kernel<T, D>, dim3((unsigned)grid), dim3(Cfg::kThreads),
-                                         Cfg::kSmem, stream, tk, tv, base);
-  if (e != cudaSuccess) return cuda_fail(e, "decode kernel launch");
-  g_launches.fetch_add(1);
-  if (sh.n_split == 1) return FCSA_OK;
+  const auto launch = [&](auto kern) {
+    return launch_attention<decltype(kern)::value>("decode", nullptr, grid, Cfg::kThreads, Cfg::kSmem, stream, tk, tv, a);
+  };
+  r = a.window > 0 ? launch(kernel_c<fcsa::fcsa_decode_kernel<T, D, true>>{})
+                   : launch(kernel_c<fcsa::fcsa_decode_kernel<T, D>>{});
+  if (r || sh.n_split == 1) return r;
   const long long threads = sh.items * 64 * (D / 4);
-  e = fcsa::launch_pdl(fcsa::decode_combine_kernel<T, D>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0,
-                       stream, base);
-  if (e != cudaSuccess) return cuda_fail(e, "decode combine launch");
-  g_launches.fetch_add(1);
-  return FCSA_OK;
+  return launched(fcsa::launch_pdl(fcsa::decode_combine_kernel<T, D>, dim3((unsigned)((threads + 255) / 256)),
+                                   dim3(256), 0, stream, a),
+                  "decode combine launch");
 }
 
 // ---- packed sequences ----------------------------------------------------------------------------
@@ -316,14 +330,205 @@ int launch_varlen_tail(const fcsa_problem* p, fcsa::TailArgs a, int n, cudaStrea
   for (int i = 0; i < n; ++i) vecs = std::max(vecs, (long long)a.t[i].total * a.t[i].H * (p->head_dim / 8));
   // a grid-stride loop: a few waves of blocks at most, whatever the tail's length
   const unsigned blocks = (unsigned)std::max(1LL, std::min((vecs + 255) / 256, 1024LL));
-  const cudaError_t e = fcsa::launch_pdl(fcsa::varlen_tail_kernel, dim3(blocks, n), dim3(256), 0, stream, a);
-  if (e != cudaSuccess) return cuda_fail(e, "varlen tail launch");
-  g_launches.fetch_add(1);
-  return FCSA_OK;
+  return launched(fcsa::launch_pdl(fcsa::varlen_tail_kernel, dim3(blocks, n), dim3(256), 0, stream, a),
+                  "varlen tail launch");
 }
 
-fcsa::BwdWorkspace varlen_layout(const fcsa_problem* p, const fcsa_varlen* vl) {
-  return fcsa::bwd_varlen_workspace_layout(p->batch, p->heads, p->kv_heads, vl->total_q, vl->total_k, p->head_dim);
+// ---- backward ------------------------------------------------------------------------------------
+// The backward's workspaces: dense, or packed sequences (vl)
+fcsa::BwdWorkspace bwd_layout(const fcsa_problem* p, const fcsa_varlen* vl) {
+  if (vl)
+    return fcsa::bwd_varlen_workspace_layout(p->batch, p->heads, p->kv_heads, vl->total_q, vl->total_k, p->head_dim);
+  return fcsa::bwd_workspace_layout(p->batch, p->heads, p->kv_heads, p->seq_q, p->seq_k, p->head_dim);
+}
+
+// The backward's arguments, filled from the problem and the caller's tensors by backward_impl
+struct BwdHostArgs {
+  int B, H, kv_heads, Nq, Nk, causal;
+  int window;                       // sliding window W (0 = none; never with a bias)
+  float scale, shift;
+  const uint8_t* mask; long long mask_sb;
+  fcsa_tensor q, k, v, o, d_o, dq, dk, dv;
+  const float* inv_l;
+  bool out_f32;                     // o (read), dq, dk, dv (written) are float32
+  void* workspace;                  // scratch
+  void* zeroed;                     // zero on entry, zero again on exit (dq accumulator)
+  // fused l2norm backward (q, k above are then the NORMALISED tensors and dq, dk the gradients
+  // w.r.t. the raw ones); both null = plain backward
+  const float* q_rnorm;
+  const float* k_rnorm;
+  int groups;
+  // additive bias (nullptr = none) and its fp32 gradient accumulator (nullptr = not needed)
+  const void* bias = nullptr; long long bias_sb = 0, bias_sh = 0, bias_sn = 0;
+  const float* bias_amax = nullptr;           // optional device scalar added (if positive) to the shift
+  float* dbias = nullptr; long long dbias_sb = 0, dbias_sh = 0;
+  // packed sequences (VARLEN): B sequences, Nq / Nk the maximum lengths, q, d_o, o, dq (total_q, H, D)
+  // and k, v, dk, dv (total_k, kv_heads, D) with sb unused, inv_l (H, total_q), the rnorms [heads][total][groups]
+  const int* cu_q = nullptr;
+  const int* cu_k = nullptr;
+  int total_q = 0, total_k = 0;
+};
+
+// Slices per key/value-head group (query heads per CTA = G / split).  One CTA per group keeps dk / dv in registers
+// (no accumulator, no finish pass, bitwise reproducible), but the grid then has B * kv_heads * key tiles CTAs; below
+// one CTA per SM the group is split into the fewest slices that fill the device.  Keys/values shared by all heads
+// (kv_heads == 1) and the BIAS kernels (no registers to spare for the head loop) take one query head per CTA.
+int bwd_group_split(int B, int H, int kv_heads, int Nk, bool bias, int sm_count) {
+  const int G = H / kv_heads;
+  if (G == 1) return 1;
+  if (bias || kv_heads == 1) return G;
+  const long long unsplit = (long long)((Nk + 127) / 128) * B * kv_heads;
+  if (unsplit >= sm_count) return 1;
+  for (int s = 2; s < G; ++s)
+    if (G % s == 0 && unsplit * s >= sm_count) return s;
+  return G;
+}
+
+// The backward's launches: preprocess, main kernel, dq finish, and for split groups the dk / dv finish (and the l2norm
+// backward of dk).  w: the workspaces' layout (bwd_layout).
+template <typename T, int D, bool BIAS = false, bool VARLEN = false>
+int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream_t stream) {
+  using namespace fcsa;
+  using Cfg = BwdCfg<D>;
+  // the batch, key rows and query tiles of the tensors as addressed: packed sequences are one batch of total rows
+  const int tB = VARLEN ? 1 : h.B, tNq = VARLEN ? h.total_q : h.Nq, tNk = VARLEN ? h.total_k : h.Nk;
+  const int nqt = (h.Nq + Cfg::QT - 1) / Cfg::QT;     // query tiles of the longest sequence
+  uint8_t* ws = reinterpret_cast<uint8_t*>(h.workspace);
+  uint8_t* zs = reinterpret_cast<uint8_t*>(h.zeroed);
+  float* stats = reinterpret_cast<float*>(ws + w.stats_off);
+  float* dq_acc = reinterpret_cast<float*>(zs + w.dq_off);
+  float* dkv_acc = reinterpret_cast<float*>(ws + w.dkv_off);
+  const float log2e = 1.4426950408889634f;
+  cudaError_t e;
+  int r;
+  int split = 1;
+  if (h.kv_heads < h.H) {
+    int sms = 0;
+    e = device_sm_count(&sms);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaDeviceGetAttribute(multiProcessorCount)");
+    split = bwd_group_split(h.B, h.H, h.kv_heads, h.Nk, BIAS, sms);
+  }
+  const bool to_acc = split > 1;
+  const size_t dkv_elems = (size_t)tB * h.kv_heads * tNk * D;
+
+  // dk/dv accumulators of split groups are per call (the dq accumulator is self-cleaning)
+  if (to_acc) {
+    e = cudaMemsetAsync(dkv_acc, 0, 2 * dkv_elems * 4, stream);
+    if (e != cudaSuccess) return cuda_fail(e, "cudaMemsetAsync(workspace)");
+  }
+
+  // 1. preprocess
+  {
+    std::conditional_t<VARLEN, PrepVarlenArgs, PrepArgs> pa;
+    pa.B = h.B; pa.H = h.H; pa.Nq = h.Nq; pa.Nk = h.Nk; pa.D = D; pa.nqt = nqt; pa.QT = Cfg::QT; pa.causal = h.causal;
+    if constexpr (VARLEN) { pa.cu_q = h.cu_q; pa.total_q = h.total_q; pa.ntile = w.nqt; }
+    pa.c2 = h.shift * log2e;
+    pa.shift_extra = h.bias_amax;
+    pa.o_f32 = h.out_f32 ? 1 : 0;
+    pa.o = h.o.ptr; pa.o_sb = h.o.sb; pa.o_sh = h.o.sh; pa.o_sn = h.o.sn;
+    pa.d_o = h.d_o.ptr; pa.do_sb = h.d_o.sb; pa.do_sh = h.d_o.sh; pa.do_sn = h.d_o.sn;
+    pa.inv_l = h.inv_l; pa.stats = stats;
+    const int rows_per_block = 2 * (256 / (D / 8));
+    const int padded = nqt * Cfg::QT;
+    pa.bpb = (padded + rows_per_block - 1) / rows_per_block;
+    const long long grid = (long long)pa.bpb * h.B * h.H;
+    if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
+    if (g_ev[3][0]) cudaEventRecord(g_ev[3][0], stream);
+    e = launch_pdl(bwd_prep_kernel<T, D / 8, VARLEN>, dim3((unsigned)grid), dim3(256), 0, stream, pa);
+    if (g_ev[3][1]) cudaEventRecord(g_ev[3][1], stream);
+    if ((r = launched(e, "backward preprocess launch"))) return r;
+  }
+  // 2. main
+  {
+    CUtensorMap tq, tk, tv, tdo, tdq;
+    if ((r = map_operand<T, D>(&tq, "q", h.q, tB, h.H, tNq, Cfg::QT)) ||
+        (r = map_operand<T, D>(&tk, "k", h.k, tB, h.kv_heads, tNk, 128)) ||
+        (r = map_operand<T, D>(&tv, "v", h.v, tB, h.kv_heads, tNk, 128)) ||
+        (r = map_operand<T, D>(&tdo, "d_o", h.d_o, tB, h.H, tNq, Cfg::QT)))
+      return r;
+    // the dq accumulator as [B][H][Nq][D] fp32 over its padded rows: boxes of 32 features x QT rows (packed
+    // sequences: [1][H][ntile * QT][D], every tile inside the map)
+    memset(&tdq, 0, sizeof(tdq));
+    const long long acc_sh = (long long)w.nqt * Cfg::QT * D;
+    if (Cfg::kStaged &&
+        (r = make_tensor_map_bhnd(&tdq, dq_acc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, tB, h.H, VARLEN ? w.nqt * Cfg::QT : h.Nq,
+                                  D, h.H * acc_sh, acc_sh, D, Cfg::QT, 32)))
+      return fail(FCSA_ERR_CUDA, "dq accumulator: cuTensorMapEncodeTiled failed (%d)", r);
+    // (the window's arguments extend the kernel's)
+    BwdArgsOf<VARLEN, true> a;
+    a.window = h.window;
+    a.B = h.B; a.H = h.H; a.Nq = h.Nq; a.Nk = h.Nk; a.kv_heads = h.kv_heads; a.causal = h.causal;
+    a.has_mask = h.mask ? 1 : 0; a.nqt = w.nqt;
+    if constexpr (VARLEN) {
+      a.cu_q = h.cu_q; a.cu_k = h.cu_k; a.total_q = h.total_q; a.total_k = h.total_k; a.ntile = w.nqt;
+    }
+    a.split = split; a.hpc = h.H / h.kv_heads / split;
+    a.c1 = h.scale * log2e; a.scale = h.scale;
+    a.mask = h.mask; a.mask_sb = h.mask_sb;
+    a.stats = stats; a.dq_acc = dq_acc;
+    a.dk_acc = dkv_acc; a.dv_acc = dkv_acc + dkv_elems;
+    a.dk = h.dk.ptr; a.dk_sb = h.dk.sb; a.dk_sh = h.dk.sh; a.dk_sn = h.dk.sn;
+    a.dv = h.dv.ptr; a.dv_sb = h.dv.sb; a.dv_sh = h.dv.sh; a.dv_sn = h.dv.sn;
+    a.bias = h.bias; a.bias_sb = h.bias_sb; a.bias_sh = h.bias_sh; a.bias_sn = h.bias_sn;
+    a.dbias = h.dbias; a.dbias_sb = h.dbias_sb; a.dbias_sh = h.dbias_sh;
+    a.out_f32 = h.out_f32 ? 1 : 0;
+    a.k_rnorm = h.k_rnorm; a.groups = h.groups;
+    // one CTA per (key tile, batch, kv head, slice of its group); packed sequences: key tiles of the longest one
+    const long long items = (long long)((h.Nk + 127) / 128) * h.B * h.kv_heads * split;
+    if (items > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
+    const auto launch = [&](auto kern) {
+      return launch_attention<decltype(kern)::value>("backward", g_ev[1], items, Cfg::kThreads, Cfg::kSmem, stream,
+                                                     tq, tk, tv, tdo, tdq, a);
+    };
+    if constexpr (BIAS)   // (one query head per CTA, no window)
+      r = launch(kernel_c<fcsa_bwd_kernel<T, D, true>>{});
+    else if (a.hpc > 1)   // HEAD_LOOP
+      r = a.window > 0 ? launch(kernel_c<fcsa_bwd_kernel<T, D, false, true, VARLEN, true>>{})
+                       : launch(kernel_c<fcsa_bwd_kernel<T, D, false, true, VARLEN>>{});
+    else
+      r = a.window > 0 ? launch(kernel_c<fcsa_bwd_kernel<T, D, false, false, VARLEN, true>>{})
+                       : launch(kernel_c<fcsa_bwd_kernel<T, D, false, false, VARLEN>>{});
+    if (r) return r;
+  }
+  // 3. finish
+  {
+    std::conditional_t<VARLEN, DqFinishVarlenArgs, DqFinishArgs> fa;
+    fa.B = h.B; fa.H = h.H; fa.Nq = h.Nq; fa.D = D; fa.nqt = w.nqt; fa.padded = w.nqt * Cfg::QT; fa.scale = h.scale;
+    if constexpr (VARLEN) { fa.padded = nqt * Cfg::QT; fa.cu_q = h.cu_q; fa.total_q = h.total_q; fa.ntile = w.nqt; }
+    fa.dq_acc = dq_acc; fa.dq = h.dq.ptr; fa.sb = h.dq.sb; fa.sh = h.dq.sh; fa.sn = h.dq.sn;
+    fa.q_hat = h.q.ptr; fa.q_sb = h.q.sb; fa.q_sh = h.q.sh; fa.q_sn = h.q.sn;
+    fa.q_rnorm = h.q_rnorm; fa.G = h.groups; fa.out_f32 = h.out_f32 ? 1 : 0;
+    const long long threads = (long long)h.B * h.H * (VARLEN ? fa.padded : h.Nq) * (D / 8);
+    const long long blocks = (threads + 255) / 256;
+    if (blocks > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
+    if (g_ev[4][0]) cudaEventRecord(g_ev[4][0], stream);
+    e = launch_pdl(bwd_dq_finish_kernel<T, D, VARLEN>, dim3((unsigned)blocks), dim3(256), 0, stream, fa);
+    if (g_ev[4][1]) cudaEventRecord(g_ev[4][1], stream);
+    if ((r = launched(e, "dq finish launch"))) return r;
+    if (to_acc) {
+      for (int which = 0; which < 2; ++which) {
+        KvFinishArgs ka;
+        ka.B = tB; ka.Hk = h.kv_heads; ka.Nk = tNk; ka.D = D; ka.out_f32 = h.out_f32 ? 1 : 0;
+        ka.acc = dkv_acc + (which ? dkv_elems : 0);
+        const fcsa_tensor& t = which ? h.dv : h.dk;
+        ka.out = t.ptr; ka.sb = t.sb; ka.sh = t.sh; ka.sn = t.sn;
+        const long long tot = (long long)dkv_elems / 8;
+        bwd_kv_finish_kernel<T><<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(ka);
+        if ((r = launched(cudaGetLastError(), "dk/dv finish launch"))) return r;
+      }
+    }
+    if (h.k_rnorm != nullptr && to_acc) {
+      // l2norm backward of dk (gradient w.r.t. the raw keys) as its own pass over the head-summed dk; otherwise
+      // the main kernel's epilogue applies it
+      RowArgs la = {};
+      la.B = tB; la.D = D; la.G = h.groups;
+      la.t[0] = {h.kv_heads, tNk, h.dk, h.k, h.dk, const_cast<float*>(h.k_rnorm)};
+      if ((r = launched(launch_row_bwd(la, std::is_same<T, __nv_bfloat16>::value, false, stream),
+                        "l2norm backward (dk) launch")))
+        return r;
+    }
+  }
+  return FCSA_OK;
 }
 
 }  // namespace
@@ -351,14 +556,10 @@ int fcsa_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor*
   if ((r = check_tensor(q, "q")) || (r = check_tensor(k, "k")) || (r = check_tensor(v, "v")) ||
       (r = check_tensor(o, "o")))
     return r;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  if (p->dtype == FCSA_BF16) {
-    if (p->head_dim == 64) return launch_forward<__nv_bfloat16, 64>(p, q, k, v, o, inv_l, s);
-    return launch_forward<__nv_bfloat16, 128>(p, q, k, v, o, inv_l, s);
-  } else {
-    if (p->head_dim == 64) return launch_forward<__half, 64>(p, q, k, v, o, inv_l, s);
-    return launch_forward<__half, 128>(p, q, k, v, o, inv_l, s);
-  }
+  return dispatch(p, [&](auto t, auto d) {
+    return launch_forward<typename decltype(t)::type, decltype(d)::value>(p, q, k, v, o, inv_l,
+                                                                          reinterpret_cast<cudaStream_t>(stream));
+  });
 }
 
 int fcsa_forward_bias(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
@@ -369,14 +570,10 @@ int fcsa_forward_bias(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_te
   if ((r = check_tensor(q, "q")) || (r = check_tensor(k, "k")) || (r = check_tensor(v, "v")) ||
       (r = check_tensor(o, "o")) || (r = check_bias(p, bias)))
     return r;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  if (p->dtype == FCSA_BF16) {
-    if (p->head_dim == 64) return launch_forward<__nv_bfloat16, 64, true>(p, q, k, v, o, inv_l, s, bias);
-    return launch_forward<__nv_bfloat16, 128, true>(p, q, k, v, o, inv_l, s, bias);
-  } else {
-    if (p->head_dim == 64) return launch_forward<__half, 64, true>(p, q, k, v, o, inv_l, s, bias);
-    return launch_forward<__half, 128, true>(p, q, k, v, o, inv_l, s, bias);
-  }
+  return dispatch(p, [&](auto t, auto d) {
+    return launch_forward<typename decltype(t)::type, decltype(d)::value, true>(
+        p, q, k, v, o, inv_l, reinterpret_cast<cudaStream_t>(stream), bias);
+  });
 }
 
 size_t fcsa_backward_workspace_bytes(const fcsa_problem* p) {
@@ -396,7 +593,9 @@ int fcsa_zeroed_init(void* zeroed, size_t bytes, void* stream) {
   return FCSA_OK;
 }
 
-static int backward_impl(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
+// Every backward entry point: dense or packed sequences (vl), with the fused l2norm backward over `groups` when
+// q_rnorm / k_rnorm are set (q, k are then the normalised tensors), or with a bias.
+static int backward_impl(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_tensor* q, const fcsa_tensor* k,
                          const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o,
                          const float* inv_l, const fcsa_tensor* dq, const fcsa_tensor* dk,
                          const fcsa_tensor* dv, void* workspace, size_t workspace_bytes, void* zeroed,
@@ -412,33 +611,26 @@ static int backward_impl(const fcsa_problem* p, const fcsa_tensor* q, const fcsa
       (r = check_tensor(dk, "dk")) || (r = check_tensor(dv, "dv")))
     return r;
   if (!inv_l) return fail(FCSA_ERR_INVALID, "inv_l: null");
-  const size_t need = fcsa_backward_workspace_bytes(p);
-  if (!workspace || workspace_bytes < need)
-    return fail(FCSA_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need, workspace_bytes);
+  const fcsa::BwdWorkspace w = bwd_layout(p, vl);
+  if (!workspace || workspace_bytes < w.total)
+    return fail(FCSA_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w.total, workspace_bytes);
   if (!aligned16(workspace)) return fail(FCSA_ERR_INVALID, "workspace not 16-byte aligned");
-  const size_t zneed = fcsa_backward_zeroed_bytes(p);
-  if (!zeroed || zeroed_bytes < zneed)
-    return fail(FCSA_ERR_WORKSPACE, "zeroed workspace too small: need %zu bytes, got %zu", zneed, zeroed_bytes);
+  if (!zeroed || zeroed_bytes < w.ztotal)
+    return fail(FCSA_ERR_WORKSPACE, "zeroed workspace too small: need %zu bytes, got %zu", w.ztotal, zeroed_bytes);
   if (!aligned16(zeroed)) return fail(FCSA_ERR_INVALID, "zeroed workspace not 16-byte aligned");
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  fcsa::BwdHostArgs h;
-  h.dtype_bf16 = p->dtype == FCSA_BF16;
+  if (p->out_f32 && (q_rnorm || k_rnorm))
+    return fail(FCSA_ERR_UNSUPPORTED, "out_f32 with the fused l2norm backward is not implemented (normalise outside)");
+  BwdHostArgs h;
   h.B = p->batch; h.H = p->heads; h.kv_heads = p->kv_heads; h.Nq = p->seq_q; h.Nk = p->seq_k;
-  h.D = p->head_dim; h.causal = p->causal ? 1 : 0;
+  h.causal = p->causal ? 1 : 0;
   h.window = kernel_window(p);
   h.scale = p->scale; h.shift = p->shift;
   h.mask = p->key_mask; h.mask_sb = p->key_mask_stride;
   h.q = *q; h.k = *k; h.v = *v; h.o = *o; h.d_o = *d_o; h.dq = *dq; h.dk = *dk; h.dv = *dv;
   h.inv_l = inv_l;
   h.out_f32 = p->out_f32 != 0;
-  if (h.out_f32 && (q_rnorm || k_rnorm))
-    return fail(FCSA_ERR_UNSUPPORTED, "out_f32 with the fused l2norm backward is not implemented (normalise outside)");
   h.workspace = workspace;
   h.zeroed = zeroed;
-  h.ev_start = g_ev[1][0];
-  h.ev_stop = g_ev[1][1];
-  h.ev_prep[0] = g_ev[3][0]; h.ev_prep[1] = g_ev[3][1];
-  h.ev_finish[0] = g_ev[4][0]; h.ev_finish[1] = g_ev[4][1];
   h.q_rnorm = q_rnorm;
   h.k_rnorm = k_rnorm;
   h.groups = groups;
@@ -447,14 +639,18 @@ static int backward_impl(const fcsa_problem* p, const fcsa_tensor* q, const fcsa
     h.bias_amax = bias->amax;
     h.dbias = d_bias_acc; h.dbias_sb = dsb; h.dbias_sh = dsh;
   }
-  int launches = 0;
-  const char* err = nullptr;
-  cudaError_t ce = cudaSuccess;
-  r = fcsa::run_backward(h, s, &launches, &err, &ce);
-  g_launches.fetch_add(launches);
-  if (r == FCSA_ERR_CUDA) return fail(r, "%s: %s", err ? err : "backward", cudaGetErrorString(ce));
-  if (r != FCSA_OK) return fail(r, "%s", err ? err : "backward failed");
-  return FCSA_OK;
+  if (vl) {
+    h.cu_q = vl->cu_seqlens_q; h.cu_k = vl->cu_seqlens_k;
+    h.total_q = vl->total_q; h.total_k = vl->total_k;
+  }
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  return dispatch(p, [&](auto t, auto d) {
+    using T = typename decltype(t)::type;
+    constexpr int D = decltype(d)::value;
+    if (vl) return run_backward_t<T, D, false, true>(h, w, s);   // (packed sequences take no bias)
+    if (bias) return run_backward_t<T, D, true>(h, w, s);
+    return run_backward_t<T, D>(h, w, s);
+  });
 }
 
 int fcsa_backward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
@@ -462,8 +658,8 @@ int fcsa_backward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor
                   const float* inv_l, const fcsa_tensor* dq, const fcsa_tensor* dk,
                   const fcsa_tensor* dv, void* workspace, size_t workspace_bytes, void* zeroed,
                   size_t zeroed_bytes, void* stream) {
-  return backward_impl(p, q, k, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed, zeroed_bytes,
-                       stream, nullptr, nullptr, 1);
+  return backward_impl(p, nullptr, q, k, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed,
+                       zeroed_bytes, stream, nullptr, nullptr, 1);
 }
 
 int fcsa_backward_bias(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
@@ -472,8 +668,8 @@ int fcsa_backward_bias(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_t
                        int64_t dsh, const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv,
                        void* workspace, size_t workspace_bytes, void* zeroed, size_t zeroed_bytes, void* stream) {
   if (!bias) return fail(FCSA_ERR_INVALID, "attn_bias: null");
-  return backward_impl(p, q, k, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed, zeroed_bytes,
-                       stream, nullptr, nullptr, 1, bias, d_bias_acc, dsb, dsh);
+  return backward_impl(p, nullptr, q, k, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed,
+                       zeroed_bytes, stream, nullptr, nullptr, 1, bias, d_bias_acc, dsb, dsh);
 }
 
 int fcsa_forward_fused(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
@@ -494,7 +690,7 @@ int fcsa_forward_fused(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_t
   if (g_ev[2][0]) cudaEventRecord(g_ev[2][0], s);
   const cudaError_t e = fcsa::launch_row_fwd(a, p->dtype == FCSA_BF16, false, s);
   if (g_ev[2][1]) cudaEventRecord(g_ev[2][1], s);
-  if ((r = row_pass_launched(e, "l2norm (q, k) launch"))) return r;
+  if ((r = launched(e, "l2norm (q, k) launch"))) return r;
   return fcsa_forward(p, &n->q_hat, &n->k_hat, v, o, inv_l, stream);
 }
 
@@ -508,7 +704,7 @@ int fcsa_backward_fused(const fcsa_problem* p, const fcsa_l2norm* n, const fcsa_
   if ((r = check_problem(p))) return r;
   if ((r = check_rows(false, p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, n->groups))) return r;
   if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
-  return backward_impl(p, &n->q_hat, &n->k_hat, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes,
+  return backward_impl(p, nullptr, &n->q_hat, &n->k_hat, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes,
                        zeroed, zeroed_bytes, stream, n->q_rnorm, n->k_rnorm, n->groups);
 }
 
@@ -523,8 +719,8 @@ int fcsa_f32_cast(int32_t dtype, int32_t batch, int32_t heads, int32_t rows, int
   if (groups > 0 && !rnorm) return fail(FCSA_ERR_INVALID, "f32 cast: rnorm is null");
   fcsa::RowArgs a = row_args(batch, head_dim, groups, mul, mul_reciprocal);
   a.t[0] = {heads, rows, *x, *y, {}, rnorm};
-  return row_pass_launched(fcsa::launch_row_fwd(a, dtype == FCSA_BF16, true, reinterpret_cast<cudaStream_t>(stream)),
-                           "f32 cast launch");
+  return launched(fcsa::launch_row_fwd(a, dtype == FCSA_BF16, true, reinterpret_cast<cudaStream_t>(stream)),
+                  "f32 cast launch");
 }
 
 int fcsa_f32_cast_backward(int32_t dtype, int32_t batch, int32_t heads, int32_t rows, int32_t head_dim,
@@ -539,8 +735,8 @@ int fcsa_f32_cast_backward(int32_t dtype, int32_t batch, int32_t heads, int32_t 
   if (!f32_rows(dx)) return fail(FCSA_ERR_INVALID, "f32 cast backward: dx rows must be 16-byte aligned float32");
   fcsa::RowArgs a = row_args(batch, head_dim, groups, mul, mul_reciprocal);
   a.t[0] = {heads, rows, *dy, groups > 0 ? *y : fcsa_tensor{}, *dx, const_cast<float*>(rnorm)};
-  return row_pass_launched(fcsa::launch_row_bwd(a, dtype == FCSA_BF16, true, reinterpret_cast<cudaStream_t>(stream)),
-                           "f32 cast backward launch");
+  return launched(fcsa::launch_row_bwd(a, dtype == FCSA_BF16, true, reinterpret_cast<cudaStream_t>(stream)),
+                  "f32 cast backward launch");
 }
 
 int fcsa_l2norm_forward(int32_t dtype, int32_t batch, int32_t heads, int32_t rows, int32_t head_dim,
@@ -551,8 +747,8 @@ int fcsa_l2norm_forward(int32_t dtype, int32_t batch, int32_t heads, int32_t row
   if ((r = check_tensor(x, "x")) || (r = check_tensor(y, "y"))) return r;
   fcsa::RowArgs a = row_args(batch, head_dim, groups);
   a.t[0] = {heads, rows, *x, *y, {}, rnorm};
-  return row_pass_launched(fcsa::launch_row_fwd(a, dtype == FCSA_BF16, false, reinterpret_cast<cudaStream_t>(stream)),
-                           "l2norm forward launch");
+  return launched(fcsa::launch_row_fwd(a, dtype == FCSA_BF16, false, reinterpret_cast<cudaStream_t>(stream)),
+                  "l2norm forward launch");
 }
 
 int fcsa_l2norm_backward(int32_t dtype, int32_t batch, int32_t heads, int32_t rows,
@@ -566,8 +762,8 @@ int fcsa_l2norm_backward(int32_t dtype, int32_t batch, int32_t heads, int32_t ro
   if (!rnorm) return fail(FCSA_ERR_INVALID, "rnorm: null");
   fcsa::RowArgs a = row_args(batch, head_dim, groups);
   a.t[0] = {heads, rows, *dy, *y, *dx, const_cast<float*>(rnorm)};
-  return row_pass_launched(fcsa::launch_row_bwd(a, dtype == FCSA_BF16, false, reinterpret_cast<cudaStream_t>(stream)),
-                           "l2norm backward launch");
+  return launched(fcsa::launch_row_bwd(a, dtype == FCSA_BF16, false, reinterpret_cast<cudaStream_t>(stream)),
+                  "l2norm backward launch");
 }
 
 size_t fcsa_decode_workspace_bytes(const fcsa_problem* p, int32_t n_new) {
@@ -607,17 +803,15 @@ int fcsa_decode(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* 
     a.t[n++] = {p->kv_heads, n_new, *k_new, *k_cache, {}, nullptr, cache_seqlens, p->seq_k, groups == 0 ? 1 : 0};
     a.t[n++] = {p->kv_heads, n_new, *v_new, *v_cache, {}, nullptr, cache_seqlens, p->seq_k, 1};
   }
-  if (n > 0 && (r = row_pass_launched(fcsa::launch_row_append(a, n, p->dtype == FCSA_BF16, s), "append pass launch")))
+  if (n > 0 && (r = launched(fcsa::launch_row_append(a, n, p->dtype == FCSA_BF16, s), "append pass launch")))
     return r;
 
   const fcsa_tensor* qa = groups > 0 ? &qhat : q;
   float* part = reinterpret_cast<float*>(static_cast<char*>(workspace) + qbytes);
-  if (p->dtype == FCSA_BF16) {
-    if (p->head_dim == 64) return launch_decode<__nv_bfloat16, 64>(p, sh, qa, k_cache, v_cache, cache_seqlens, n_new, o, part, s);
-    return launch_decode<__nv_bfloat16, 128>(p, sh, qa, k_cache, v_cache, cache_seqlens, n_new, o, part, s);
-  }
-  if (p->head_dim == 64) return launch_decode<__half, 64>(p, sh, qa, k_cache, v_cache, cache_seqlens, n_new, o, part, s);
-  return launch_decode<__half, 128>(p, sh, qa, k_cache, v_cache, cache_seqlens, n_new, o, part, s);
+  return dispatch(p, [&](auto t, auto d) {
+    return launch_decode<typename decltype(t)::type, decltype(d)::value>(p, sh, qa, k_cache, v_cache, cache_seqlens,
+                                                                         n_new, o, part, s);
+  });
 }
 
 int fcsa_forward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_tensor* q, const fcsa_tensor* k,
@@ -642,17 +836,14 @@ int fcsa_forward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, cons
     if (g_ev[2][0]) cudaEventRecord(g_ev[2][0], s);
     const cudaError_t e = fcsa::launch_row_fwd(a, p->dtype == FCSA_BF16, false, s);
     if (g_ev[2][1]) cudaEventRecord(g_ev[2][1], s);
-    if ((r = row_pass_launched(e, "l2norm (q, k) launch"))) return r;
+    if ((r = launched(e, "l2norm (q, k) launch"))) return r;
     qa = &n->q_hat;
     ka = &n->k_hat;
   }
-  if (p->dtype == FCSA_BF16) {
-    if (p->head_dim == 64) r = launch_forward<__nv_bfloat16, 64, false, true>(p, qa, ka, v, o, inv_l, s, nullptr, vl);
-    else r = launch_forward<__nv_bfloat16, 128, false, true>(p, qa, ka, v, o, inv_l, s, nullptr, vl);
-  } else {
-    if (p->head_dim == 64) r = launch_forward<__half, 64, false, true>(p, qa, ka, v, o, inv_l, s, nullptr, vl);
-    else r = launch_forward<__half, 128, false, true>(p, qa, ka, v, o, inv_l, s, nullptr, vl);
-  }
+  r = dispatch(p, [&](auto t, auto d) {
+    return launch_forward<typename decltype(t)::type, decltype(d)::value, false, true>(p, qa, ka, v, o, inv_l, s,
+                                                                                       nullptr, vl);
+  });
   if (r) return r;
   // o = 0 in the rows outside every sequence
   fcsa::TailArgs ta = {};
@@ -662,12 +853,12 @@ int fcsa_forward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, cons
 
 size_t fcsa_backward_fused_varlen_workspace_bytes(const fcsa_problem* p, const fcsa_varlen* vl) {
   if (check_varlen(p, vl)) return 0;
-  return varlen_layout(p, vl).total;
+  return bwd_layout(p, vl).total;
 }
 
 size_t fcsa_backward_fused_varlen_zeroed_bytes(const fcsa_problem* p, const fcsa_varlen* vl) {
   if (check_varlen(p, vl)) return 0;
-  return varlen_layout(p, vl).ztotal;
+  return bwd_layout(p, vl).ztotal;
 }
 
 int fcsa_backward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_l2norm* n,
@@ -677,49 +868,15 @@ int fcsa_backward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, con
   int r;
   if ((r = check_varlen(p, vl))) return r;
   if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
-  if (n->groups != 0) {
+  const bool fused = n->groups != 0;
+  if (fused) {
     if ((r = check_rows(false, p->dtype, 1, p->heads, vl->total_q, p->head_dim, n->groups))) return r;
     if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
   }
-  if ((r = check_tensor(&n->q_hat, "q")) || (r = check_tensor(&n->k_hat, "k")) || (r = check_tensor(v, "v")) ||
-      (r = check_tensor(o, "o")) || (r = check_tensor(d_o, "d_o")) || (r = check_tensor(dq, "dq")) ||
-      (r = check_tensor(dk, "dk")) || (r = check_tensor(dv, "dv")))
+  if ((r = backward_impl(p, vl, &n->q_hat, &n->k_hat, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed,
+                         zeroed_bytes, stream, fused ? n->q_rnorm : nullptr, fused ? n->k_rnorm : nullptr,
+                         fused ? n->groups : 1)))
     return r;
-  if (!inv_l) return fail(FCSA_ERR_INVALID, "inv_l: null");
-  const fcsa::BwdWorkspace w = varlen_layout(p, vl);
-  if (!workspace || workspace_bytes < w.total)
-    return fail(FCSA_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w.total, workspace_bytes);
-  if (!aligned16(workspace)) return fail(FCSA_ERR_INVALID, "workspace not 16-byte aligned");
-  if (!zeroed || zeroed_bytes < w.ztotal)
-    return fail(FCSA_ERR_WORKSPACE, "zeroed workspace too small: need %zu bytes, got %zu", w.ztotal, zeroed_bytes);
-  if (!aligned16(zeroed)) return fail(FCSA_ERR_INVALID, "zeroed workspace not 16-byte aligned");
-  fcsa::BwdHostArgs h;
-  h.dtype_bf16 = p->dtype == FCSA_BF16;
-  h.B = p->batch; h.H = p->heads; h.kv_heads = p->kv_heads; h.Nq = p->seq_q; h.Nk = p->seq_k;
-  h.D = p->head_dim; h.causal = p->causal ? 1 : 0;
-  h.window = kernel_window(p);
-  h.scale = p->scale; h.shift = p->shift;
-  h.mask = nullptr; h.mask_sb = 0;
-  h.q = n->q_hat; h.k = n->k_hat; h.v = *v; h.o = *o; h.d_o = *d_o; h.dq = *dq; h.dk = *dk; h.dv = *dv;
-  h.inv_l = inv_l;
-  h.workspace = workspace;
-  h.zeroed = zeroed;
-  h.ev_start = g_ev[1][0];
-  h.ev_stop = g_ev[1][1];
-  h.ev_prep[0] = g_ev[3][0]; h.ev_prep[1] = g_ev[3][1];
-  h.ev_finish[0] = g_ev[4][0]; h.ev_finish[1] = g_ev[4][1];
-  h.q_rnorm = n->groups != 0 ? n->q_rnorm : nullptr;
-  h.k_rnorm = n->groups != 0 ? n->k_rnorm : nullptr;
-  h.groups = n->groups != 0 ? n->groups : 1;
-  h.cu_q = vl->cu_seqlens_q; h.cu_k = vl->cu_seqlens_k;
-  h.total_q = vl->total_q; h.total_k = vl->total_k;
-  int launches = 0;
-  const char* err = nullptr;
-  cudaError_t ce = cudaSuccess;
-  r = fcsa::run_backward_varlen(h, reinterpret_cast<cudaStream_t>(stream), &launches, &err, &ce);
-  g_launches.fetch_add(launches);
-  if (r == FCSA_ERR_CUDA) return fail(r, "%s: %s", err ? err : "backward", cudaGetErrorString(ce));
-  if (r != FCSA_OK) return fail(r, "%s", err ? err : "backward failed");
   // zero gradients in the rows outside every sequence
   fcsa::TailArgs ta = {};
   ta.t[0] = {dq->ptr, dq->sh, dq->sn, p->heads, vl->total_q, vl->cu_seqlens_q};

@@ -101,16 +101,18 @@ struct Shapes {
   }
 };
 
-// window: sliding-window attention (0 = none); the library rejects a negative one
-fcsa_problem make_problem(const Shapes& sh, const Tensor& q, double scale, double shift, bool causal,
-                          const optional<Tensor>& mask_u8, bool out_f32 = false, int64_t window = 0) {
-  TORCH_CHECK(window >= 0 && window <= 0x7FFFFFFF, "window must be a non-negative int32 (0 = none), got ", window);
+// The problem of every entry point; `who` prefixes the message of a window out of range ("" / "decode: " / "varlen: ").
+// dtype: q's; window: sliding-window attention (0 = none); the library rejects a negative one.
+fcsa_problem build_problem(const char* who, const Tensor& q, int64_t B, int64_t H, int64_t kv_heads, int64_t Nq,
+                           int64_t Nk, int64_t D, double scale, double shift, bool causal,
+                           const optional<Tensor>& mask_u8, bool out_f32, int64_t window) {
+  TORCH_CHECK(window >= 0 && window <= 0x7FFFFFFF, who, "window must be a non-negative int32 (0 = none), got ", window);
   fcsa_problem p;
   p.out_f32 = out_f32 ? 1 : 0;
   p.window = (int32_t)window;
   p.dtype = dtype_code(q);
-  p.batch = (int32_t)sh.B; p.heads = (int32_t)sh.H; p.kv_heads = (int32_t)sh.kv_heads;
-  p.seq_q = (int32_t)sh.Nq; p.seq_k = (int32_t)sh.Nk; p.head_dim = (int32_t)sh.D;
+  p.batch = (int32_t)B; p.heads = (int32_t)H; p.kv_heads = (int32_t)kv_heads;
+  p.seq_q = (int32_t)Nq; p.seq_k = (int32_t)Nk; p.head_dim = (int32_t)D;
   p.causal = causal ? 1 : 0;
   p.scale = (float)scale; p.shift = (float)shift;
   if (mask_u8.has_value()) {
@@ -121,6 +123,13 @@ fcsa_problem make_problem(const Shapes& sh, const Tensor& q, double scale, doubl
     p.key_mask_stride = 0;
   }
   return p;
+}
+
+// the problem of q, k, v as Shapes canonicalised them
+fcsa_problem make_problem(const Shapes& sh,const Tensor& q, double scale, double shift, bool causal,
+                          const optional<Tensor>& mask_u8, bool out_f32, int64_t window) {
+  return build_problem("", q, sh.B, sh.H, sh.kv_heads, sh.Nq, sh.Nk, sh.D, scale, shift, causal, mask_u8, out_f32,
+                       window);
 }
 
 // key-padding mask (batch, seq_k), True = attend -> contiguous bytes
@@ -164,13 +173,16 @@ struct Workspaces {
 std::mutex g_ws_mutex;
 std::map<std::pair<int, void*>, Workspaces> g_ws;
 
-Workspaces workspaces_of_size(size_t need_s, size_t need_z, const Tensor& like, cudaStream_t stream) {
-  TORCH_CHECK(need_s > 0 && need_z > 0, "libfcsa_b200: ", fcsa_last_error());
+// The workspaces of (like's device, stream), grown to need_s scratch and need_z zeroed bytes.  A size of 0 is the
+// library's refusal of the problem.  with_zeroed = false (decode) needs the scratch only.
+Workspaces workspaces_of_size(size_t need_s, size_t need_z, const Tensor& like, cudaStream_t stream,
+                              bool with_zeroed = true) {
+  TORCH_CHECK(need_s > 0 && (need_z > 0 || !with_zeroed), "libfcsa_b200: ", fcsa_last_error());
   std::lock_guard<std::mutex> lock(g_ws_mutex);
   Workspaces& w = g_ws[{(int)like.get_device(), (void*)stream}];
   const auto opts = like.options().dtype(at::kByte);
   if (!w.scratch.defined() || (size_t)w.scratch.numel() < need_s) w.scratch = at::empty({(int64_t)need_s}, opts);
-  if (!w.zeroed.defined() || (size_t)w.zeroed.numel() < need_z) {
+  if (with_zeroed && (!w.zeroed.defined() || (size_t)w.zeroed.numel() < need_z)) {
     w.zeroed = at::empty({(int64_t)need_z}, opts);
     FCSA_CHECK(fcsa_zeroed_init(w.zeroed.data_ptr(), need_z, stream));
   }
@@ -418,7 +430,6 @@ std::tuple<Tensor, Tensor, Tensor, optional<Tensor>> backward(
 Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
               const optional<Tensor>& k_in, const optional<Tensor>& v_in, double scale, double shift, bool causal,
               int64_t groups, int64_t window) {
-  TORCH_CHECK(window >= 0 && window <= 0x7FFFFFFF, "decode: window must be a non-negative int32 (0 = none), got ", window);
   TORCH_CHECK(q_in.dim() == 4 && k_cache.dim() == 4 && v_cache.dim() == 4,
               "decode: q, k_cache, v_cache must be (batch, heads, seq, head_dim)");
   TORCH_CHECK(q_in.is_cuda() && k_cache.is_cuda() && v_cache.is_cuda(), "decode: CUDA tensors required");
@@ -456,26 +467,12 @@ Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, 
   }
   const c10::cuda::CUDAGuard guard(q_in.device());
   const Tensor q = tma_ready(q_in);
-  fcsa_problem p;
-  p.dtype = dtype_code(q);
-  p.batch = (int32_t)B; p.heads = (int32_t)H; p.kv_heads = (int32_t)Hk;
-  p.seq_q = (int32_t)Nq; p.seq_k = (int32_t)cap; p.head_dim = (int32_t)D;
-  p.causal = causal ? 1 : 0;
-  p.scale = (float)scale; p.shift = (float)shift;
-  p.key_mask = nullptr; p.key_mask_stride = 0;
-  p.out_f32 = 0; p.window = (int32_t)window;
+  const fcsa_problem p =
+      build_problem("decode: ", q, B, H, Hk, Nq, cap, D, scale, shift, causal, c10::nullopt, false, window);
   Tensor o = at::empty({B, H, Nq, D}, q.options());
   cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
-  const size_t need = fcsa_decode_workspace_bytes(&p, (int32_t)n_new);
-  TORCH_CHECK(need > 0, "libfcsa_b200: ", fcsa_last_error());
-  Tensor scratch;
-  {
-    std::lock_guard<std::mutex> lock(g_ws_mutex);
-    Workspaces& w = g_ws[{(int)q.get_device(), (void*)stream}];
-    if (!w.scratch.defined() || (size_t)w.scratch.numel() < need)
-      w.scratch = at::empty({(int64_t)need}, q.options().dtype(at::kByte));
-    scratch = w.scratch;
-  }
+  const Tensor scratch =
+      workspaces_of_size(fcsa_decode_workspace_bytes(&p, (int32_t)n_new), 0, q, stream, false).scratch;
   const fcsa_tensor tq = view4(q), tkc = view4(k_cache), tvc = view4(v_cache), to = view4(o);
   fcsa_tensor tk = {nullptr, 0, 0, 0}, tv = {nullptr, 0, 0, 0};
   if (has_new) { tk = view4(k); tv = view4(v); }
@@ -504,7 +501,6 @@ struct Varlen {
 
 Varlen varlen_problem(const Tensor& q, const Tensor& k, const Tensor& v, const Tensor& cu_q, const Tensor& cu_k,
                       int64_t max_q, int64_t max_k, double scale, double shift, bool causal, int64_t window) {
-  TORCH_CHECK(window >= 0 && window <= 0x7FFFFFFF, "varlen: window must be a non-negative int32 (0 = none), got ", window);
   TORCH_CHECK(q.dim() == 3 && k.dim() == 3 && v.dim() == 3,
               "varlen: q must be (total_q, heads, head_dim) and k, v (total_k, kv_heads, head_dim)");
   TORCH_CHECK(q.is_cuda() && k.is_cuda() && v.is_cuda(), "varlen: CUDA tensors required - this build has no CPU path");
@@ -524,14 +520,8 @@ Varlen varlen_problem(const Tensor& q, const Tensor& k, const Tensor& v, const T
               "varlen: max_seqlen_q / max_seqlen_k must be positive int32 values");
   TORCH_CHECK(q.size(0) <= 0x7FFFFFFF && k.size(0) <= 0x7FFFFFFF, "varlen: too many packed rows");
   Varlen r;
-  fcsa_problem& p = r.p;
-  p.dtype = dtype_code(q);
-  p.batch = (int32_t)(cu_q.size(0) - 1); p.heads = (int32_t)H; p.kv_heads = (int32_t)Hk;
-  p.seq_q = (int32_t)max_q; p.seq_k = (int32_t)max_k; p.head_dim = (int32_t)D;
-  p.causal = causal ? 1 : 0;
-  p.scale = (float)scale; p.shift = (float)shift;
-  p.key_mask = nullptr; p.key_mask_stride = 0;
-  p.out_f32 = 0; p.window = (int32_t)window;
+  r.p = build_problem("varlen: ", q, cu_q.size(0) - 1, H, Hk, max_q, max_k, D, scale, shift, causal, c10::nullopt,
+                      false, window);
   r.vl.cu_seqlens_q = cu_q.data_ptr<int32_t>();
   r.vl.cu_seqlens_k = cu_k.data_ptr<int32_t>();
   r.vl.total_q = (int32_t)q.size(0);

@@ -24,7 +24,7 @@ def sm_count():
 
 
 def group_split(B, H, Hk, Nk, sms, bias=False):
-    """Slices per group the backward chooses (mirror of bwd_group_split in csrc/bwd_kernel.cuh)."""
+    """Slices per group the backward chooses (mirror of bwd_group_split in csrc/fcsa_abi.cu)."""
     G = H // Hk
     if G == 1:
         return 1

@@ -386,7 +386,18 @@ def test_c_abi_refuses_stride0_tensor(fcsa):
     bad = _abi.FcsaTensor(x.data_ptr(), x.stride(0), 0, x.stride(2))
     rc = lib.fcsa_forward(_abi.ref(p), _abi.ref(good), _abi.ref(bad), _abi.ref(good), _abi.ref(good), None, None)
     assert rc == _abi.FCSA_ERR_INVALID and b"stride-0" in lib.fcsa_last_error()
+    # the backward's maps say the same, naming the operand: here a head-expanded d_o
+    inv_l = torch.ones(2, 4, 128, dtype=torch.float32, device="cuda")
+    grads = [torch.empty_like(x) for _ in range(3)]
+    tg = [_abi.FcsaTensor(t.data_ptr(), t.stride(0), t.stride(1), t.stride(2)) for t in grads]
+    ws = torch.empty(lib.fcsa_backward_workspace_bytes(_abi.ref(p)), dtype=torch.uint8, device="cuda")
+    zs = torch.zeros(lib.fcsa_backward_zeroed_bytes(_abi.ref(p)), dtype=torch.uint8, device="cuda")
+    rc = lib.fcsa_backward(_abi.ref(p), *([_abi.ref(good)] * 4), _abi.ref(bad), inv_l.data_ptr(),
+                           *(_abi.ref(t) for t in tg), ws.data_ptr(), ws.numel(), zs.data_ptr(), zs.numel(), None)
+    err = lib.fcsa_last_error()
+    assert rc == _abi.FCSA_ERR_INVALID and b"stride-0" in err and err.startswith(b"d_o:")
     torch.cuda.synchronize()
+    assert int(zs.count_nonzero()) == 0           # the zeroed workspace is left zero
 
 
 def test_zeroed_workspace_is_left_clean_across_shapes(fcsa):
