@@ -941,7 +941,7 @@ struct DqFinishVarlenArgs : DqFinishArgs {
 };
 
 // dq conversion (reference: the fp32 -> scalar_t cast of dq after its atomics, cu:1904): TPR = D / 8 consecutive lanes
-// per query row, 8 features each.  The accumulator is read from L2 (the reductions of the main kernel have just
+// per query row, 8 features each, and two rows per thread in the dense kernels (one in the VARLEN ones).  The accumulator is read from L2 (the reductions of the main kernel have just
 // produced it there), converted, and written back as zeros: it is zero between launches.
 // VARLEN: every row of a sequence's tiles is cleared, the padding rows past its end included.  Those lie inside the
 // accumulator's tensor map and receive dS K for masked queries: exact zeros for finite K, NaN when the neighbouring rows
@@ -952,9 +952,9 @@ bwd_dq_finish_kernel(const std::conditional_t<VARLEN, DqFinishVarlenArgs, DqFini
   pdl_launch_dependents();
   pdl_wait();
   constexpr int TPR = D / 8;
-  const long long t = (long long)blockIdx.x * 256 + threadIdx.x;
   if constexpr (VARLEN) {
     constexpr int QT = 64;
+    const long long t = (long long)blockIdx.x * 256 + threadIdx.x;
     const long long rowid = t / TPR;                       // over (sequences*heads) x padded
     const int c8 = (int)(t % TPR);
     const bool in_grid = rowid < (long long)a.B * a.H * a.padded;
@@ -986,38 +986,82 @@ bwd_dq_finish_kernel(const std::conditional_t<VARLEN, DqFinishVarlenArgs, DqFini
     *reinterpret_cast<uint4*>(dst) = pack16B<T>(g);
     return;
   }
-  const long long rowid = t / TPR;                         // over (batch*heads) x Nq
-  const int c8 = (int)(t % TPR);
-  const bool ok = rowid < (long long)a.B * a.H * a.Nq;     // whole rows of TPR lanes (shuffles stay in them)
-  const long long bh = ok ? rowid / a.Nq : 0;
-  const int row = ok ? (int)(rowid - bh * a.Nq) : 0;
-  const int b = (int)(bh / a.H), h = (int)(bh % a.H);
-  float* src = a.dq_acc + (bh * a.padded + row) * D + c8 * 8;
-  float4 lo = make_float4(0.f, 0.f, 0.f, 0.f), hi = lo;
-  if (ok) {
-    lo = ldg_cg128f(src);
-    hi = ldg_cg128f(src + 4);
-    *reinterpret_cast<float4*>(src) = make_float4(0.f, 0.f, 0.f, 0.f);
-    *reinterpret_cast<float4*>(src + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+  // Two rows per thread, 256 / TPR rows apart (a block covers 2 x 256 / TPR consecutive rows): every load of both rows
+  // is issued before any of them is used.  Row indices in 32 bits whenever the grid's rows fit (the divisions by Nq
+  // and H are then a few instructions instead of a 64-bit division routine each).
+  constexpr int RPB = 256 / TPR;
+  const long long nrows = (long long)a.B * a.H * a.Nq;
+  const bool small = nrows < 0x7FFFFFFFLL;
+  const int c8 = threadIdx.x % TPR;
+  long long bhs[2];
+  int rows[2];
+  bool oks[2];
+  float4 lo[2], hi[2];
+  uint4 yq[2];
+  float rn[2];
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    const long long rowid = ((long long)blockIdx.x * 2 + u) * RPB + threadIdx.x / TPR;    // over (batch*heads) x Nq
+    const bool ok = rowid < nrows;                         // whole rows of TPR lanes (shuffles stay in them)
+    long long bh = 0;
+    int row = 0;
+    if (ok) {
+      if (small) {
+        const unsigned r32 = (unsigned)rowid, q32 = r32 / (unsigned)a.Nq;
+        bh = q32;
+        row = (int)(r32 - q32 * (unsigned)a.Nq);
+      } else {
+        bh = rowid / a.Nq;
+        row = (int)(rowid - bh * a.Nq);
+      }
+    }
+    bhs[u] = bh;
+    rows[u] = row;
+    oks[u] = ok;
+    lo[u] = hi[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+    yq[u] = make_uint4(0, 0, 0, 0);
+    rn[u] = 0.f;
+    if (ok) {
+      const float* src = a.dq_acc + (bh * a.padded + row) * D + c8 * 8;
+      lo[u] = ldg_cg128f(src);
+      hi[u] = ldg_cg128f(src + 4);
+    }
   }
-  float g[8] = {lo.x * a.scale, lo.y * a.scale, lo.z * a.scale, lo.w * a.scale,
-                hi.x * a.scale, hi.y * a.scale, hi.z * a.scale, hi.w * a.scale};
-  if (a.q_rnorm != nullptr) {                             // uniform across the grid
-    float y[8];
-    unpack16B<T>(ok ? ldg_stream128(reinterpret_cast<const T*>(a.q_hat) + b * a.q_sb + h * a.q_sh +
-                                    (long long)row * a.q_sn + c8 * 8)
-                    : make_uint4(0, 0, 0, 0), y);
-    l2norm_bwd_group<8>(g, y, D / a.G, c8, ok ? a.q_rnorm + (((long long)b * a.H + h) * a.Nq + row) * a.G : nullptr,
-                        1.f);
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    if (!oks[u] || a.q_rnorm == nullptr) continue;
+    const int b = (int)(bhs[u] / a.H), h = (int)(bhs[u] - (long long)b * a.H);
+    yq[u] = ldg_stream128(reinterpret_cast<const T*>(a.q_hat) + b * a.q_sb + h * a.q_sh + (long long)rows[u] * a.q_sn +
+                          c8 * 8);
   }
-  if (!ok) return;
-  if (a.out_f32) {
-    float* dst = reinterpret_cast<float*>(a.dq) + b * a.sb + h * a.sh + (long long)row * a.sn + c8 * 8;
-    *reinterpret_cast<float4*>(dst) = make_float4(g[0], g[1], g[2], g[3]);
-    *reinterpret_cast<float4*>(dst + 4) = make_float4(g[4], g[5], g[6], g[7]);
-  } else {
-    T* dst = reinterpret_cast<T*>(a.dq) + b * a.sb + h * a.sh + (long long)row * a.sn + c8 * 8;
-    *reinterpret_cast<uint4*>(dst) = pack16B<T>(g);
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    const bool ok = oks[u];
+    const long long bh = bhs[u];
+    const int row = rows[u];
+    const int b = (int)(bh / a.H), h = (int)(bh - (long long)b * a.H);
+    if (ok) {
+      float* src = a.dq_acc + (bh * a.padded + row) * D + c8 * 8;
+      *reinterpret_cast<float4*>(src) = make_float4(0.f, 0.f, 0.f, 0.f);
+      *reinterpret_cast<float4*>(src + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    float g[8] = {lo[u].x * a.scale, lo[u].y * a.scale, lo[u].z * a.scale, lo[u].w * a.scale,
+                  hi[u].x * a.scale, hi[u].y * a.scale, hi[u].z * a.scale, hi[u].w * a.scale};
+    if (a.q_rnorm != nullptr) {                           // uniform across the grid
+      float y[8];
+      unpack16B<T>(yq[u], y);
+      l2norm_bwd_group<8>(g, y, D / a.G, c8, ok ? a.q_rnorm + (((long long)b * a.H + h) * a.Nq + row) * a.G : nullptr,
+                          1.f);
+    }
+    if (!ok) continue;
+    if (a.out_f32) {
+      float* dst = reinterpret_cast<float*>(a.dq) + b * a.sb + h * a.sh + (long long)row * a.sn + c8 * 8;
+      *reinterpret_cast<float4*>(dst) = make_float4(g[0], g[1], g[2], g[3]);
+      *reinterpret_cast<float4*>(dst + 4) = make_float4(g[4], g[5], g[6], g[7]);
+    } else {
+      T* dst = reinterpret_cast<T*>(a.dq) + b * a.sb + h * a.sh + (long long)row * a.sn + c8 * 8;
+      *reinterpret_cast<uint4*>(dst) = pack16B<T>(g);
+    }
   }
 }
 

@@ -499,7 +499,7 @@ int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream
     fa.q_hat = h.q.ptr; fa.q_sb = h.q.sb; fa.q_sh = h.q.sh; fa.q_sn = h.q.sn;
     fa.q_rnorm = h.q_rnorm; fa.G = h.groups; fa.out_f32 = h.out_f32 ? 1 : 0;
     const long long threads = (long long)h.B * h.H * (VARLEN ? fa.padded : h.Nq) * (D / 8);
-    const long long blocks = (threads + 255) / 256;
+    const long long blocks = VARLEN ? (threads + 255) / 256 : (threads + 511) / 512;   // dense: two rows per thread
     if (blocks > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
     if (g_ev[4][0]) cudaEventRecord(g_ev[4][0], stream);
     e = launch_pdl(bwd_dq_finish_kernel<T, D, VARLEN>, dim3((unsigned)blocks), dim3(256), 0, stream, fa);
