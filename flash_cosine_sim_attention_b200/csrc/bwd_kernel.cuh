@@ -43,6 +43,7 @@
 #include "l2norm_kernels.cuh"
 #include "sm90_primitives.cuh"
 #include "tensor_map.h"
+#include "tile_ranges.h"
 
 namespace fcsa {
 
@@ -111,12 +112,8 @@ inline BwdWorkspace bwd_workspace_layout(int B, int H, int kv_heads, int Nq, int
   return w;
 }
 
-// Packed sequences: the stats and the dq accumulator hold, per query head, `ntile` tiles of QT rows.  Sequence b starts
-// at tile base(b) = start_b / QT + b (start_b = its first query row), which needs no prefix sum on the device and leaves
-// room for ceil(len_b / QT) tiles before base(b + 1); every tile index stays below total_q / QT + B + 1.  dkv_acc is
-// [kv_heads][total_k][D] (dk, then dv).
-inline int varlen_tiles(int B, long long total_q) { return (int)(total_q / 64 + B + 1); }
-
+// Packed sequences: the stats and the dq accumulator hold, per query head, varlen_tiles tiles of QT rows, sequence b
+// from tile base(b) = varlen_tile_base (tile_ranges.h).  dkv_acc is [kv_heads][total_k][D] (dk, then dv).
 inline BwdWorkspace bwd_varlen_workspace_layout(int B, int H, int kv_heads, long long total_q, long long total_k,
                                                 int D) {
   BwdWorkspace w;
@@ -191,7 +188,7 @@ __global__ void __launch_bounds__(256) bwd_prep_kernel(const std::conditional_t<
     const SeqSpan sq = seq_span(a.cu_q, b, a.Nq, a.total_q);
     Nq = sq.len;
     padded = (Nq + QT - 1) / QT * QT;
-    tile0 = (long long)h * a.ntile + sq.start / QT + b;
+    tile0 = (long long)h * a.ntile + varlen_tile_base(sq.start, b);
     row_off = sq.start;
   }
   const float c2 = a.c2 + (a.shift_extra != nullptr ? fmaxf(__ldg(a.shift_extra), 0.f) * 1.4426950408889634f : 0.f);
@@ -458,27 +455,15 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     const SeqSpan sq = seq_span(a.cu_q, b, a.Nq, a.total_q), sk = seq_span(a.cu_k, b, a.Nk, a.total_k);
     Nq = sq.len; Nk = sk.len; q_row0 = sq.start; k_row0 = sk.start;
     nqt = (Nq + QT - 1) / QT;
-    qbase = q_row0 / QT + b;
+    qbase = varlen_tile_base(q_row0, b);
     if (key0 >= Nk) return;                   // a key tile past the end of its sequence
   }
-  const int off = Nk - Nq;
-  int i_lo = 0;
-  if (a.causal) {
-    // first query tile with a row that can see key0: QT*i + QT-1 + off >= key0
-    const int x = key0 - off - (QT - 1);
-    i_lo = x <= 0 ? 0 : (x + QT - 1) / QT;
-  }
-  int W = 0, i_end = nqt;                     // the window; the query tile after the last one visited
-  if constexpr (WINDOW) {
-    W = a.window;
-    if (!a.causal) {                          // first query tile with a row whose band reaches key0
-      const int x = key0 - off - (QT - 1) - (W - 1);
-      i_lo = x <= 0 ? 0 : (x + QT - 1) / QT;
-    }
-    const int last_row = key0 + 127 - off + W - 1;   // the last query row whose lower limit is at most key0 + 127
-    i_end = last_row < 0 ? 0 : min(nqt, last_row / QT + 1);
-  }
-  const int NI = max(0, i_end - i_lo);        // number of query tiles to visit per query head
+  const int off = diag_off(Nq, Nk);
+  int W = 0;                                  // the window
+  if constexpr (WINDOW) W = a.window;
+  const TileRange qr = query_tiles<WINDOW>(key0, off, nqt, a.causal, W);
+  const int i_lo = qr.lo, i_end = qr.hi;      // the query tiles [i_lo, i_end) visited per query head
+  const int NI = tile_count(qr);              // number of query tiles to visit per query head
   const int NT = hpc * NI;                    // flat tile index i: head h0 + i / NI, query tile i_lo + i % NI
 
   if (wg == 0) {
@@ -520,7 +505,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       if (rw == 0) tma_prefetch_desc(&tm_dq);
       for (int i = rw; i < NT; i += 2) {
         const int n = i >> 1, sb = n % NDQ;        // the warpgroup's n-th tile
-        const int hh = HEAD_LOOP ? i / NI : 0, qt = i_lo + i - hh * NI;
+        const HeadTile ht = head_tile(i, i_lo, NI, HEAD_LOOP);
+        const int hh = ht.head, qt = ht.qt;
         const uint32_t src = sDQ + (NDQ * rw + sb) * Cfg::kDQ;
         mbar_wait(BAR(DQ_FULL + NDQ * rw + sb), (n / NDQ) & 1);
 #pragma unroll
@@ -550,7 +536,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   int lo_off = 0, hi_off = 0;
   if constexpr (WINDOW) {
     lo_off = a.causal ? -off : -off - W + 1;
-    hi_off = W - 1 - off;
+    hi_off = window_hi_off(off, W);
   }
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
@@ -700,7 +686,6 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   float dv[D / 2], dk[D / 2];
 #pragma unroll
   for (int i = 0; i < D / 2; ++i) dv[i] = dk[i] = 0.f;
-  // (packed sequences: a head's last tile ends at ceil(Nq / QT) * QT, so row0 + QT < Nq says whether row0 is before it)
   // the producer loads K and V whatever NI; the epilogue reads K (l2norm backward) even when no query tile is visited
   mbar_wait(BAR(KV_FULL), 0);
 
@@ -759,12 +744,9 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     if (NT > 0) {
       mbar_wait(BAR(FULL), 0);
       issue_s_dp(s, dp, sQ, sDO);
-      // i runs over the flat (head, query tile) sequence; row0 restarts at i_lo * QT with every head, after the last
-      // tile (window: after tile i_end - 1, i.e. once row0 + QT passes key0 + 127 + hi_off, the last row seeing a key)
-      auto next_in_head = [&](int row0) {
-        return row0 + QT < (VARLEN ? Nq : a.nqt * QT) && (!WINDOW || row0 + QT <= key0 + 127 + hi_off);
-      };
-      for (int i = 0, row0 = i_lo * QT; i < NT; ++i, row0 = (!HEAD_LOOP || next_in_head(row0)) ? row0 + QT : i_lo * QT) {
+      // i runs over the flat (head, query tile) sequence; row0 restarts at i_lo * QT with every head (next_row0)
+      for (int i = 0, row0 = i_lo * QT; i < NT; ++i,
+               row0 = HEAD_LOOP ? next_row0<WINDOW>(row0, i_lo, VARLEN ? Nq : a.nqt * QT, key0, hi_off) : row0 + QT) {
         const int st = i % NST;
         const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
         wgmma_wait<0>();                        // S^T, dP^T of tile i; dV, dK of tile i - 1; dQ of tile i - 2
@@ -812,8 +794,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   } else {
     for (int i = 0; i < NT; ++i) {
       const int st = i % NST;
-      const int hh = HEAD_LOOP ? i / NI : 0;    // head h0 + hh, query tile i_lo + i % NI
-      const int row0 = (i_lo + i - hh * NI) * QT;
+      const HeadTile ht = head_tile(i, i_lo, NI, HEAD_LOOP);
+      const int hh = ht.head, row0 = ht.qt * QT;
       const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
       mbar_wait(BAR(FULL + st), (i / NST) & 1);
       float s[QT / 2], dp[QT / 2];
@@ -964,7 +946,7 @@ bwd_dq_finish_kernel(const std::conditional_t<VARLEN, DqFinishVarlenArgs, DqFini
     const SeqSpan sq = seq_span(a.cu_q, b, a.Nq, a.total_q);
     const bool own = in_grid && r < (sq.len + QT - 1) / QT * QT;    // a row of the sequence's tiles
     const bool ok = in_grid && r < sq.len;                          // ... and of the sequence (whole rows of lanes)
-    float* src = a.dq_acc + (((long long)h * a.ntile + sq.start / QT + b) * QT + r) * D + c8 * 8;
+    float* src = a.dq_acc + (((long long)h * a.ntile + varlen_tile_base(sq.start, b)) * QT + r) * D + c8 * 8;
     const long long row = (long long)sq.start + r;                  // the packed row
     float4 lo = make_float4(0.f, 0.f, 0.f, 0.f), hi = lo;
     if (own) {

@@ -18,6 +18,7 @@
 #pragma once
 
 #include "sm90_primitives.cuh"
+#include "tile_ranges.h"
 
 namespace fcsa {
 
@@ -51,24 +52,6 @@ struct DecodeCfg {
   static constexpr int kCtasPerSm = D == 64 ? 2 : 1;
   static_assert(kSmem * kCtasPerSm <= 232448, "decode kernel shared memory");
 };
-
-// Splits per work item: 1 when the items alone fill the SMs, otherwise the fewest that do, at most one per key tile
-// of the capacity.  (tests/test_decode_host.py mirrors this rule.)  With a window, `cap` is decode_window_keys.
-inline int decode_split(long long items, int cap, int sm_count) {
-  if (items >= sm_count) return 1;
-  const long long want = (sm_count + items - 1) / items;
-  const long long tiles = (cap + 127) / 128;
-  return (int)(want < tiles ? want : tiles);
-}
-
-// A bound on the keys whose tiles one row block can see under a window W: its rows span at most 64 queries, so its
-// keys lie in a range of 64 + W - 2 (causal) or 64 + 2 W - 3 keys, which touches at most ceil(range / 128) + 1 tiles.
-// The split rule then bounds a block's tiles by the window instead of the capacity.
-inline int decode_window_keys(int cap, int window, bool causal) {
-  const long long range = 64LL + (causal ? 1 : 2) * (long long)window;
-  const long long keys = range + 128;
-  return (int)(keys < cap ? keys : cap);
-}
 
 // WINDOW: sliding-window attention (Windowed<DecodeArgs>::window = W).  A row block's visible tiles start at the tile of
 // its smallest lower limit; the split cuts [t_lo, t_hi) into n_split chunks.
@@ -118,22 +101,13 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
   // visible keys and this split's key tiles (uniform over the CTA)
   const int L = min(max(a.seqlens[b], 0), a.cap);
   const int Tb = min(L + a.n_new, a.cap);
-  const int off = Tb - a.Nq;
-  int nt = (Tb + 127) >> 7;
-  if (a.causal) {
-    const int last_col = r_last / a.G + off;
-    nt = last_col < 0 ? 0 : min(nt, (last_col >> 7) + 1);
-  }
-  int W = 0, t_lo = 0;                        // the window and the block's first visible tile
-  if constexpr (WINDOW) {
-    W = a.window;
-    const int last_col = r_last / a.G + off + (a.causal ? 0 : W - 1);
-    nt = last_col < 0 ? 0 : min((Tb + 127) >> 7, (last_col >> 7) + 1);
-    const int first_col = r0 / a.G + off - W + 1;
-    t_lo = first_col <= 0 ? 0 : min(first_col >> 7, nt);
-  }
-  const int j0 = t_lo + (int)((long long)(nt - t_lo) * split / a.n_split);
-  const int j1 = t_lo + (int)((long long)(nt - t_lo) * (split + 1) / a.n_split);
+  const int off = diag_off(a.Nq, Tb);
+  int W = 0;                                  // the window
+  if constexpr (WINDOW) W = a.window;
+  // the tiles the block's queries r0 / G .. r_last / G see (the forward's rule with Nk = T_b), and this split's chunk
+  const TileRange chunk =
+      split_chunk(key_tiles<WINDOW>(r0 / a.G, r_last / a.G, off, Tb, a.causal, W), split, a.n_split);
+  const int j0 = chunk.lo, j1 = chunk.hi;
 
   if (wg == 0) {
     // =============================== TMA producer ===============================

@@ -171,7 +171,7 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
   a.causal = p->causal ? 1 : 0;
   a.has_mask = p->key_mask ? 1 : 0;
   a.group = p->heads / p->kv_heads;
-  a.n_qblk = (p->seq_q + Cfg::kBlockM - 1) / Cfg::kBlockM;
+  a.n_qblk = fcsa::row_blocks(p->seq_q, Cfg::kBlockM);
   const float log2e = 1.4426950408889634f;
   a.c1 = p->scale * log2e;
   a.c2 = p->shift * log2e;
@@ -253,7 +253,7 @@ int decode_shape(const fcsa_problem* p, DecodeShape* s) {
   const cudaError_t e = fcsa::device_sm_count(&sms);
   if (e != cudaSuccess) return cuda_fail(e, "cudaDeviceGetAttribute(multiProcessorCount)");
   s->R = (p->heads / p->kv_heads) * p->seq_q;
-  s->n_rb = (s->R + 63) / 64;
+  s->n_rb = fcsa::row_blocks(s->R, 64);
   s->items = (long long)p->batch * p->kv_heads * s->n_rb;
   const int w = kernel_window(p);
   s->n_split = fcsa::decode_split(s->items, w > 0 ? fcsa::decode_window_keys(p->seq_k, w, p->causal != 0) : p->seq_k, sms);
@@ -368,21 +368,6 @@ struct BwdHostArgs {
   const int* cu_k = nullptr;
   int total_q = 0, total_k = 0;
 };
-
-// Slices per key/value-head group (query heads per CTA = G / split).  One CTA per group keeps dk / dv in registers
-// (no accumulator, no finish pass, bitwise reproducible), but the grid then has B * kv_heads * key tiles CTAs; below
-// one CTA per SM the group is split into the fewest slices that fill the device.  Keys/values shared by all heads
-// (kv_heads == 1) and the BIAS kernels (no registers to spare for the head loop) take one query head per CTA.
-int bwd_group_split(int B, int H, int kv_heads, int Nk, bool bias, int sm_count) {
-  const int G = H / kv_heads;
-  if (G == 1) return 1;
-  if (bias || kv_heads == 1) return G;
-  const long long unsplit = (long long)((Nk + 127) / 128) * B * kv_heads;
-  if (unsplit >= sm_count) return 1;
-  for (int s = 2; s < G; ++s)
-    if (G % s == 0 && unsplit * s >= sm_count) return s;
-  return G;
-}
 
 // The backward's launches: preprocess, main kernel, dq finish, and for split groups the dk / dv finish (and the l2norm
 // backward of dk).  w: the workspaces' layout (bwd_layout).

@@ -19,6 +19,7 @@
 #pragma once
 
 #include "sm90_primitives.cuh"
+#include "tile_ranges.h"
 
 namespace fcsa {
 
@@ -59,8 +60,8 @@ struct FwdVarlenArgs : FwdArgs {
 // another's products more often than with two (DESIGN.md 4.1).  D = 128 (O alone is 64 registers) keeps two.
 template <int D>
 struct FwdCfg {
-  static constexpr int kConsumers = (D == 64) ? 3 : 2;                 // consumer warpgroups, 64 query rows each
-  static constexpr int kBlockM = 64 * kConsumers;                      // query rows of one CTA
+  static constexpr int kBlockM = fwd_block_rows(D);                    // query rows of one CTA
+  static constexpr int kConsumers = kBlockM / 64;                      // consumer warpgroups, 64 query rows each
   static constexpr int kThreads = 128 * (1 + kConsumers);              // + the producer warpgroup
   static constexpr int kProducerRegs = kConsumers == 3 ? kProducerRegs3 : fcsa::kProducerRegs;
   static constexpr int kConsumerRegs = kConsumers == 3 ? kConsumerRegs3 : fcsa::kConsumerRegs;
@@ -139,20 +140,11 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     Nq = sq.len; Nk = sk.len; q_row0 = sq.start; k_row0 = sk.start;
     if (m0 >= Nq) return;                                     // a query block past the end of its sequence
   }
-  const int off = Nk - Nq;
-  int NT = (Nk + 127) >> 7;                                   // key tiles this block visits
-  if (a.causal) {
-    const int last_col = min(m0 + BM - 1, Nq - 1) + off;
-    NT = last_col < 0 ? 0 : min(NT, (last_col >> 7) + 1);
-  }
-  int W = 0, j_lo = 0;                                        // the window and the first key tile visited
-  if constexpr (WINDOW) {
-    W = a.window;
-    const int last_col = min(m0 + BM - 1, Nq - 1) + off + (a.causal ? 0 : W - 1);
-    NT = last_col < 0 ? 0 : min((Nk + 127) >> 7, (last_col >> 7) + 1);
-    const int first_col = m0 + off - W + 1;                   // the lower limit of the block's first row
-    j_lo = first_col <= 0 ? 0 : min(first_col >> 7, NT);
-  }
+  const int off = diag_off(Nq, Nk);
+  int W = 0;                                                  // the window
+  if constexpr (WINDOW) W = a.window;
+  const TileRange blk = block_key_tiles<WINDOW>(m0, BM, Nq, Nk, off, a.causal, W);
+  const int j_lo = blk.lo, NT = blk.hi;                       // the key tiles [j_lo, NT) this block visits
 
   if (wg == 0) {
     // =============================== TMA producer ===============================
@@ -214,21 +206,9 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       if (!a.causal) lim[hf] = min(Nk - 1, row_a + 8 * hf + off + W - 1);
     }
   }
-  // The key tiles [jw_lo, jw_hi) this warpgroup's own 64 rows see: the block's rules applied to its first and last
-  // row.  On the block's other tiles every p of these rows is 0 (with 192-row blocks, the trailing causal tiles of
-  // the first warpgroups and all tiles of rows past the end), so the warpgroup only passes their ring slots on.
-  const int r0 = m0 + 64 * w;
-  int jw_lo = j_lo, jw_hi = NT;
-  if (r0 >= Nq) {
-    jw_hi = 0;
-  } else if (a.causal || WINDOW) {
-    const int last_col = min(r0 + 63, Nq - 1) + off + (a.causal ? 0 : W - 1);
-    jw_hi = last_col < 0 ? 0 : (last_col >> 7) + 1;
-  }
-  if constexpr (WINDOW) {
-    const int first_col = r0 + off - W + 1;
-    if (first_col > 0) jw_lo = max(j_lo, first_col >> 7);
-  }
+  // the key tiles [jw_lo, jw_hi) this warpgroup's own 64 rows see; it only passes the ring slots of the others on
+  const TileRange wgt = warpgroup_key_tiles<WINDOW>(m0 + 64 * w, j_lo, NT, Nq, off, a.causal, W);
+  const int jw_lo = wgt.lo, jw_hi = wgt.hi;
 
   float o[D / 2];
 #pragma unroll

@@ -1,18 +1,12 @@
 """CPU: the key/value-cache logic of the transformer on the plain attention (float64), the split rule of the decode
-kernel (a Python mirror that the GPU tests tie to the kernel through its launch count), and the argument checks of
-flash_cosine_sim_attention_with_kv_cache that need no device."""
+kernel (csrc/tile_ranges.h through tests/tile_ranges.py; the GPU tests tie it to the launches through their count),
+and the argument checks of flash_cosine_sim_attention_with_kv_cache that need no device."""
 import math
 
 import pytest
 import torch
 
-
-def decode_split(items, cap, sms):
-    """Key splits per work item (mirror of decode_split in csrc/decode_kernel.cuh): 1 when the work items fill the
-    SMs, otherwise the fewest that do, at most the key tiles of the capacity."""
-    if items >= sms:
-        return 1
-    return min(math.ceil(sms / items), math.ceil(cap / 128))
+from tile_ranges import decode_split
 
 
 @pytest.mark.parametrize("items,cap,sms,want", [

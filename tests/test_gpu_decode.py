@@ -8,7 +8,7 @@ test_gpu_parity.py and the element-wise bound at C = 2.  Cache rows the call mus
 so a stray write, or a NaN value row leaking into P V, shows up.
 
 The split count (key ranges per work item) is chosen on the host from the SM count; tests that target one side of
-the rule compute it with the Python mirror (test_decode_host.decode_split) and check it through the number of
+the rule compute it with the library's own rule (tile_ranges.decode_split) and check it through the number of
 launches: append pass + decode kernel, + the combine kernel when it splits."""
 import math
 
@@ -16,7 +16,7 @@ import pytest
 import torch
 
 from elementwise_bounds import FMT, attention_bounds, check_bound, kernel_shift
-from test_decode_host import decode_split
+from tile_ranges import decode_split
 from test_gpu_parity import TOL_OUT, fcsa, record, rel_err  # noqa: F401
 
 pytestmark = pytest.mark.gpu

@@ -15,25 +15,13 @@ import torch
 
 from gqa_reference import gqa_attention
 from test_gpu_parity import ROUND, TOL_GRAD, TOL_OUT, bound_check, fcsa, make_inputs, record, rel_err  # noqa: F401
+from tile_ranges import group_split
 
 pytestmark = pytest.mark.gpu
 
 
 def sm_count():
     return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-
-
-def group_split(B, H, Hk, Nk, sms, bias=False):
-    """Slices per group the backward chooses (mirror of bwd_group_split in csrc/fcsa_abi.cu)."""
-    G = H // Hk
-    if G == 1:
-        return 1
-    if bias or Hk == 1:
-        return G
-    unsplit = math.ceil(Nk / 128) * B * Hk
-    if unsplit >= sms:
-        return 1
-    return next((s for s in range(2, G) if G % s == 0 and unsplit * s >= sms), G)
 
 
 def loop_batch(Hk, Nk):

@@ -24,8 +24,8 @@ import torch
 
 import logit_range
 from elementwise_bounds import C, FMT, attention_bounds, check_bound, kernel_shift, ratio
-from test_decode_host import decode_split
-from test_gpu_gqa import group_split, sm_count
+from test_gpu_gqa import sm_count
+from tile_ranges import decode_split, group_split
 from test_gpu_parity import TOL_GRAD, TOL_OUT, fcsa, float32_ds_scale, float32_operands, record  # noqa: F401
 from window_bounds import window_attention_bounds
 

@@ -4,7 +4,8 @@ the relative-to-max tolerances of test_gpu_parity.py:
 * a sweep of sequence lengths around multiples of 64 that makes forward CTAs visit 1 to 7 key tiles (past both K/V
   rings) and backward CTAs visit 1 to 8 query tiles (past the 4- and 3-stage Q/dO rings, the D = 64 drain with
   either dQ owner), plus grouped-query loop-path CTAs whose flat (head, query tile) sequence restarts at every
-  residue mod 2 and mod 3; the coverage is computed by a mirror of the kernels' tile arithmetic and asserted;
+  residue mod 2 and mod 3; the coverage is computed from the kernels' tile arithmetic (tests/tile_ranges.py) and
+  asserted for each head dim's forward block;
 * the BIAS instantiations past one ring, with d_bias;
 * fp16 biases at the edges of the shifted exponent range;
 * padding-suffix key masks, with whole masked key tiles;
@@ -14,39 +15,30 @@ import torch
 
 from elementwise_bounds import C, U, attention_bounds, check_bound, kernel_shift
 from gqa_reference import gqa_attention
-from test_gpu_gqa import gqa_check, group_split, loop_batch, sm_count
+from test_gpu_gqa import gqa_check, loop_batch, sm_count
 from test_gpu_parity import (ROUND, TOL_GRAD, TOL_OUT, bound_check, check, fcsa, float32_operands,  # noqa: F401
                              make_inputs, record, rel_err)
 from oracle import cosine_sim_attention_oracle as oracle
+from tile_ranges import block_range, bwd_range, fwd_block_rows, group_split
 
 gpu = pytest.mark.gpu        # every test here but the coverage check of the sweep needs the H100
 
-QT, KT = 64, 128          # backward query tile rows, key tile (forward and backward)
+KT = 128                  # key tile (forward and backward)
 
 
-# ---- mirror of the kernels' tile arithmetic -------------------------------------------------------------------
-def fwd_key_tiles(Nq, Nk, causal):
-    """Key tiles each forward CTA (128 query rows) visits (fcsa_fwd_kernel's NT)."""
-    out = []
-    for m0 in range(0, Nq, 128):
-        nt = (Nk + 127) // 128
-        if causal:
-            last_col = min(m0 + 127, Nq - 1) + Nk - Nq
-            nt = 0 if last_col < 0 else min(nt, (last_col >> 7) + 1)
-        out.append(nt)
-    return out
+# ---- the tile counts of the kernels' work items -----------------------------------------------------------------
+def fwd_key_tiles(Nq, Nk, causal, D):
+    """Key tiles each forward CTA of head dim D visits (fcsa_fwd_kernel's NT)."""
+    bm = fwd_block_rows(D)
+    return [int(block_range(m0, bm, Nq, Nk, None, causal)[1][0]) for m0 in range(0, Nq, bm)]
 
 
 def bwd_query_tiles(Nq, Nk, causal, hpc=1):
-    """(NI, NT) of each backward CTA (one 128-key tile, hpc query heads): fcsa_bwd_kernel's i_lo / NI / NT."""
-    nqt = (Nq + QT - 1) // QT
+    """(NI, NT) of each backward CTA (one 128-key tile, hpc query heads): fcsa_bwd_kernel's NI / NT."""
     out = []
-    for jt in range((Nk + KT - 1) // KT):
-        i_lo = 0
-        if causal:
-            x = jt * KT - (Nk - Nq) - (QT - 1)
-            i_lo = 0 if x <= 0 else (x + QT - 1) // QT
-        ni = max(0, nqt - i_lo)
+    for key0 in range(0, Nk, KT):
+        i_lo, i_end = bwd_range(key0, Nq, Nk, None, causal)
+        ni = max(0, int(i_end[0] - i_lo[0]))
         out.append((ni, hpc * ni))
     return out
 
@@ -66,9 +58,10 @@ def gqa_nq(ni):
 
 
 def test_sweep_covers_every_tile_count():
-    fwd = {nt for nq, nk, c in SWEEP for nt in fwd_key_tiles(nq, nk, c)}
+    for D in (64, 128):                                      # 1 .. 6 key tiles: past the 4- and 2-stage rings
+        fwd = {nt for nq, nk, c in SWEEP for nt in fwd_key_tiles(nq, nk, c, D)}
+        assert set(range(1, 7)) <= fwd, (D, fwd)
     bwd = {nt for nq, nk, c in SWEEP for _, nt in bwd_query_tiles(nq, nk, c)}
-    assert set(range(1, 7)) <= fwd, fwd                      # 1 .. 6 key tiles: past the 4- and 2-stage rings
     assert set(range(1, 9)) <= bwd, bwd                      # NT = 1 .. 8, both dQ owners of the last tile
     gqa = [bwd_query_tiles(gqa_nq(ni), 256, False, hpc) for ni, hpc in GQA_LOOP]
     assert all(len({ni_ for ni_, _ in t}) == 1 for t in gqa)

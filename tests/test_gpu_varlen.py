@@ -9,7 +9,8 @@ import pytest
 import torch
 
 from elementwise_bounds import FMT, attention_bounds, check_bound, kernel_shift
-from test_gpu_gqa import group_split, sm_count
+from test_gpu_gqa import sm_count
+from tile_ranges import group_split
 from test_gpu_parity import TOL_GRAD, TOL_OUT, fcsa, record, rel_err  # noqa: F401
 
 pytestmark = pytest.mark.gpu

@@ -13,7 +13,8 @@ import torch
 
 from elementwise_bounds import FMT, check_bound, kernel_shift
 from window_bounds import window_attention_bounds
-from test_gpu_gqa import group_split, loop_batch, sm_count
+from test_gpu_gqa import loop_batch, sm_count
+from tile_ranges import group_split
 from test_gpu_parity import TOL_GRAD, TOL_OUT, fcsa, float32_ds_scale, float32_operands, make_inputs, record  # noqa: F401
 
 pytestmark = pytest.mark.gpu

@@ -1,5 +1,5 @@
 """CPU: packed variable-length attention without a device - the Python API's rejections, the C ABI's argument checks
-and workspace sizes through ctypes, a mirror of the tile-padded layout of the backward's stats and dq accumulator,
+and workspace sizes through ctypes, the tile-padded layout of the backward's stats and dq accumulator,
 and the transformer's packed path with the plain attention in float64."""
 import itertools
 import os
@@ -10,6 +10,7 @@ import torch
 
 from flash_cosine_sim_attention_b200 import _abi, flash_cosine_sim_attention_varlen
 from flash_cosine_sim_attention_b200.transformer import CosineSimCausalTransformer
+from tile_ranges import tiles
 
 
 def args(total=10, H=2, Hk=2, D=64, dtype=torch.bfloat16):
@@ -144,14 +145,6 @@ def test_abi_argument_checks(lib):
 
 
 # ---- the tile-padded layout ----------------------------------------------------------------------------------------
-def tiles(lengths):
-    """Mirror of the backward's layout: sequence b's query tiles are base(b) .. base(b) + ceil(len_b / 64) - 1 with
-    base(b) = cu[b] // 64 + b; returns (the tile ranges, tiles per head)."""
-    cu = [0] + list(itertools.accumulate(lengths))
-    ranges = [(cu[b] // 64 + b, cu[b] // 64 + b + (n + 63) // 64) for b, n in enumerate(lengths)]
-    return ranges, cu[-1] // 64 + len(lengths) + 1
-
-
 def assert_disjoint_and_inside(lengths):
     ranges, ntile = tiles(lengths)
     for (lo, hi), (lo2, _) in zip(ranges, ranges[1:]):

@@ -1,7 +1,7 @@
 """CPU: sliding-window attention on the host side.
 
-* A mirror of the tile ranges the three kernels visit under a window (csrc/fwd_kernel.cuh, bwd_kernel.cuh,
-  decode_kernel.cuh), checked against the band rule for every window up to Nq + Nk, causal and not: every visible
+* The tile ranges the backward and decode kernels visit under a window (csrc/tile_ranges.h through
+  tests/tile_ranges.py; the forward's are in test_fwd_blocks_host.py), checked against the band rule for every window up to Nq + Nk, causal and not: every visible
   (query, key) pair lies in a visited tile, and every visited tile holds at least one visible pair (a work item that
   visits nothing is the one exception).  The backward's HEAD_LOOP row0 sequence and the decode split are included.
 * plain_cosine_sim_attention(window=...) in float64 against an explicit band mask, with GQA and merged 3-D layouts.
@@ -16,6 +16,7 @@ import pytest
 import torch
 
 from elementwise_bounds import C, attention_bounds, check_bound, kernel_shift
+from tile_ranges import bwd_range, bwd_row0_sequence, decode_range, decode_window_keys
 from window_bounds import window_attention_bounds
 
 QT = 64
@@ -48,79 +49,12 @@ def visited(lo, hi, nt):
     return (t >= lo[:, None]) & (t < hi[:, None])
 
 
-# ---- mirrors of the kernels' arithmetic (numpy arrays over the window W; every division is of a non-negative value)
-def fwd_range(m0, nq, nk, w, causal):
-    """fcsa_fwd_kernel: key tiles [j_lo, NT) of the query block starting at m0."""
-    off = nk - nq
-    last_col = min(m0 + 127, nq - 1) + off + (0 if causal else w - 1)
-    NT = np.where(last_col < 0, 0, np.minimum((nk + 127) >> 7, np.maximum(last_col, 0) // 128 + 1))
-    first_col = m0 + off - w + 1
-    j_lo = np.where(first_col <= 0, 0, np.minimum(np.maximum(first_col, 0) // 128, NT))
-    return j_lo, NT
-
-
-def bwd_range(key0, nq, nk, w, causal):
-    """fcsa_bwd_kernel: query tiles [i_lo, i_end) of the key tile starting at key0."""
-    off = nk - nq
-    nqt = (nq + QT - 1) // QT
-    x = key0 - off - (QT - 1) - (0 if causal else w - 1)
-    i_lo = np.where(x <= 0, 0, (np.maximum(x, 0) + QT - 1) // QT)
-    last_row = key0 + 127 - off + w - 1
-    i_end = np.where(last_row < 0, 0, np.minimum(nqt, np.maximum(last_row, 0) // QT + 1))
-    return i_lo, i_end
-
-
-def bwd_row0_sequence(key0, nq, nk, w, causal, hpc):
-    """The STAGED consumer loop's row0 over the flat (head, query tile) sequence, as the kernel steps it, and the
-    dQ reducer's query tile qt = i_lo + i - hh NI: lists of per-window arrays."""
-    off = nk - nq
-    i_lo, i_end = bwd_range(key0, nq, nk, w, causal)
-    NI = np.maximum(0, i_end - i_lo)
-    hi_off = w - 1 - off
-    row0 = i_lo * QT
-    rows, qts = [], []
-    for i in range(int((hpc * NI).max(initial=0))):
-        rows.append(np.where(i < hpc * NI, row0, -1))
-        hh = np.where(NI > 0, i // np.maximum(NI, 1), 0)
-        qts.append(np.where(i < hpc * NI, i_lo + i - hh * NI, -1))
-        nxt = (row0 + QT < nq) & (row0 + QT <= key0 + 127 + hi_off)
-        row0 = np.where(nxt, row0 + QT, i_lo * QT)
-    return rows, qts, i_lo, NI
-
-
-def decode_range(r0, R, G, Tb, nq, w, causal, n_split):
-    """fcsa_decode_kernel: the [j0, j1) of every split of the row block starting at row r0."""
-    off = Tb - nq
-    r_last = min(r0 + 63, R - 1)
-    last_col = r_last // G + off + (0 if causal else w - 1)
-    nt = np.where(last_col < 0, 0, np.minimum((Tb + 127) >> 7, np.maximum(last_col, 0) // 128 + 1))
-    first_col = r0 // G + off - w + 1
-    t_lo = np.where(first_col <= 0, 0, np.minimum(np.maximum(first_col, 0) // 128, nt))
-    return [(t_lo + (nt - t_lo) * s // n_split, t_lo + (nt - t_lo) * (s + 1) // n_split) for s in range(n_split)]
-
-
-def decode_window_keys(cap, window, causal):
-    """Mirror of decode_window_keys (csrc/decode_kernel.cuh)."""
-    return np.minimum(64 + (1 if causal else 2) * window + 128, cap)
-
-
 def check_tiles(vis_tiles, lo, hi):
     """Visited tiles == tiles with a visible pair, except that a work item with no visible pair may visit nothing."""
     n, nt = vis_tiles.shape
     got = visited(np.broadcast_to(lo, (n,)), np.broadcast_to(hi, (n,)), nt)
     empty = ~vis_tiles.any(1)
     assert ((got == vis_tiles) | (empty[:, None] & ~got)).all()
-
-
-@pytest.mark.parametrize("causal", [True, False])
-@pytest.mark.parametrize("nq", LENGTHS)
-def test_forward_tile_range(nq, causal):
-    for nk in LENGTHS:
-        w = np.arange(1, nq + nk)                 # windows of Nq + Nk and more run the unwindowed kernels
-        vis = band(nq, nk, w, causal)
-        for m0 in range(0, nq, 128):
-            blk = vis[:, m0:m0 + 128]
-            check_tiles(tiles_hit(blk, 2, 128), *fwd_range(m0, nq, nk, w, causal))
 
 
 @pytest.mark.parametrize("causal", [True, False])
