@@ -40,10 +40,9 @@
 #include <type_traits>
 
 #include "../../include/fcsa_b200.h"
+#include "key_tile.cuh"
 #include "l2norm_kernels.cuh"
-#include "sm90_primitives.cuh"
 #include "tensor_map.h"
-#include "tile_ranges.h"
 
 namespace fcsa {
 
@@ -393,9 +392,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   constexpr int QCHUNK = QT * 128;         // bytes of one 64-feature chunk of a Q / dO stage
   constexpr int NST = Cfg::NST;
 
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
+  uint8_t* smem = smem_1024();
   const uint32_t sK = smem_u32(smem + Cfg::kOffK);
   const uint32_t sV = smem_u32(smem + Cfg::kOffV);
   const uint32_t sQ = smem_u32(smem + Cfg::kOffQ);
@@ -411,6 +408,9 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   constexpr int KV_FULL = 0, FULL = 1, EMPTY = FULL + NST, DQ_FULL = EMPTY + NST, DQ_EMPTY = DQ_FULL + 2 * NDQ,
                 DS_FULL = DQ_EMPTY + 2 * NDQ, DS_EMPTY = DS_FULL + NDS, NBARS = DS_EMPTY + NDS;
   static_assert(NBARS * 8 <= 256, "barrier area");
+  const Ring<NST> qring = {BAR(FULL), BAR(EMPTY)};            // Q, dO and the stats of a query tile
+  const Ring<NDS> dsr = {BAR(DS_FULL), BAR(DS_EMPTY)};        // STAGED: the dS^T slots
+  auto dq_ring = [&](int wg_) { return Ring<NDQ>{BAR(DQ_FULL + NDQ * wg_), BAR(DQ_EMPTY + NDQ * wg_)}; };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;
@@ -435,18 +435,10 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
   if (threadIdx.x == 0) {
     mbar_init(BAR(KV_FULL), 1);
-    for (int s = 0; s < NST; ++s) {
-      mbar_init(BAR(FULL + s), 1);
-      mbar_init(BAR(EMPTY + s), 256);
-    }
-    for (int s = 0; s < 2 * NDQ; ++s) {
-      mbar_init(BAR(DQ_FULL + s), 128);
-      mbar_init(BAR(DQ_EMPTY + s), 1);
-    }
-    for (int s = 0; s < NDS; ++s) {
-      mbar_init(BAR(DS_FULL + s), 128);
-      mbar_init(BAR(DS_EMPTY + s), 128);
-    }
+    qring.init(1, 256);
+    dq_ring(0).init(128, 1);                  // filled by a consumer warpgroup, emptied by its reducer thread
+    dq_ring(1).init(128, 1);
+    dsr.init(128, 128);
     fence_mbar_init();
   }
   __syncthreads();
@@ -485,15 +477,15 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         if constexpr (VARLEN) tile0 = (long long)h * a.ntile + qbase;
         const float* stats_h = a.stats + tile0 * 2 * QT;
         for (int qt = i_lo; qt < i_end; ++qt, ++i) {
-          const int st = i % NST;
-          mbar_wait(BAR(EMPTY + st), ((i / NST) & 1) ^ 1);
-          mbar_expect_tx(BAR(FULL + st), 2 * Cfg::kQ + 8 * QT);
+          const int st = qring.acquire(i);
+          const uint32_t full = qring.full_bar(st);
+          mbar_expect_tx(full, 2 * Cfg::kQ + 8 * QT);
 #pragma unroll
           for (int ch = 0; ch < KCH; ++ch) {
-            tma_load_4d(sQ + st * Cfg::kQ + ch * QCHUNK, &tm_q, BAR(FULL + st), ch * 64, q_row0 + qt * QT, h, tb);
-            tma_load_4d(sDO + st * Cfg::kQ + ch * QCHUNK, &tm_do, BAR(FULL + st), ch * 64, q_row0 + qt * QT, h, tb);
+            tma_load_4d(sQ + st * Cfg::kQ + ch * QCHUNK, &tm_q, full, ch * 64, q_row0 + qt * QT, h, tb);
+            tma_load_4d(sDO + st * Cfg::kQ + ch * QCHUNK, &tm_do, full, ch * 64, q_row0 + qt * QT, h, tb);
           }
-          bulk_load_1d(sStats + st * 8 * QT, stats_h + (long long)qt * 2 * QT, 8 * QT, BAR(FULL + st));
+          bulk_load_1d(sStats + st * 8 * QT, stats_h + (long long)qt * 2 * QT, 8 * QT, full);
         }
       }
     } else if (STAGED && (warp == 1 || warp == 2) && elect_one()) {
@@ -502,19 +494,19 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       // and are not written; with packed sequences the rows of a tail tile past the sequence's end are inside it,
       // and the dq finish kernel clears them)
       const int rw = warp - 1;
+      const Ring<NDQ> dqr = dq_ring(rw);
       if (rw == 0) tma_prefetch_desc(&tm_dq);
       for (int i = rw; i < NT; i += 2) {
-        const int n = i >> 1, sb = n % NDQ;        // the warpgroup's n-th tile
+        const int n = i >> 1;                      // the warpgroup's n-th tile
         const HeadTile ht = head_tile(i, i_lo, NI, HEAD_LOOP);
         const int hh = ht.head, qt = ht.qt;
-        const uint32_t src = sDQ + (NDQ * rw + sb) * Cfg::kDQ;
-        mbar_wait(BAR(DQ_FULL + NDQ * rw + sb), (n / NDQ) & 1);
+        const uint32_t src = sDQ + (NDQ * rw + dqr.wait(n)) * Cfg::kDQ;
 #pragma unroll
         for (int c = 0; c < D / 32; ++c)
           tma_reduce_add_4d(&tm_dq, src + c * (QT * 128), c * 32, (qbase + qt) * QT, h0 + hh, tb);
         bulk_commit();
         bulk_wait_read<0>();
-        mbar_arrive(BAR(DQ_EMPTY + NDQ * rw + sb));
+        dqr.release(n);
       }
       bulk_wait<0>();                          // every reduction performed before the dq finish kernel reads
     }
@@ -656,16 +648,12 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 #pragma unroll
     for (int kk = 0; kk < QT / 16; ++kk) {
       const uint32_t af[4] = {pf[4 * kk], pf[4 * kk + 1], pf[4 * kk + 2], pf[4 * kk + 3]};
-      const uint64_t db = gmma_desc_sw128(sDOs + kk * 2048, QCHUNK, 1024);
-      if constexpr (D == 64) wgmma_rs_n64<T, 1>(dv, af, db, 1u);
-      else wgmma_rs_n128<T, 1>(dv, af, db, 1u);
+      wgmma_rs<T, 1>(dv, af, gmma_desc_sw128(sDOs + kk * 2048, QCHUNK, 1024), 1u);
     }
 #pragma unroll
     for (int kk = 0; kk < QT / 16; ++kk) {
       const uint32_t af[4] = {dsf[4 * kk], dsf[4 * kk + 1], dsf[4 * kk + 2], dsf[4 * kk + 3]};
-      const uint64_t db = gmma_desc_sw128(sQs + kk * 2048, QCHUNK, 1024);
-      if constexpr (D == 64) wgmma_rs_n64<T, 1>(dk, af, db, 1u);
-      else wgmma_rs_n128<T, 1>(dk, af, db, 1u);
+      wgmma_rs<T, 1>(dk, af, gmma_desc_sw128(sQs + kk * 2048, QCHUNK, 1024), 1u);
     }
   };
   // dQ = dS K.  STAGED: contraction over all 128 keys of the CTA (dsbuf = a dS^T slot, whose two warpgroup halves
@@ -678,8 +666,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     for (int kk = 0; kk < NKK; ++kk) {
       const uint64_t da = gmma_desc_sw128(dsbuf + kk * 2048, 8192, 1024);     // dS: queries contiguous (MN-major)
       const uint64_t db = gmma_desc_sw128(sKd + kk * 2048, 16384, 1024);      // K: features contiguous (MN-major)
-      if constexpr (D == 64) wgmma_ss_n64<T, 1, 1>(dq, da, db, kk > 0 ? 1u : 0u);
-      else wgmma_ss_n128<T, 1, 1>(dq, da, db, kk > 0 ? 1u : 0u);
+      wgmma_ss<T, 1, 1>(dq, da, db, kk > 0 ? 1u : 0u);
     }
   };
 
@@ -713,9 +700,10 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 #pragma unroll
     for (int k = 0; k < D / 2; ++k) dq[k] = 0.f;
     auto ds_slot = [&](int i) { return sDS + 2 * (i % NDS) * Cfg::kDS; };
+    const Ring<NDQ> dqr = dq_ring(w);
     auto stage_dq = [&](int i) {              // i & 1 == w
-      const int n = i >> 1, sb = n % NDQ;
-      mbar_wait(BAR(DQ_EMPTY + NDQ * w + sb), ((n / NDQ) & 1) ^ 1);   // the reducer has read the buffer's last tile
+      const int n = i >> 1;
+      const int sb = dqr.acquire(n);          // the reducer has read the buffer's last tile
       const uint32_t dst = sDQ + (NDQ * w + sb) * Cfg::kDQ + dq_thr;
 #pragma unroll
       for (int jb = 0; jb < D / 8; ++jb) {
@@ -724,15 +712,15 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         sts64f(o + 1024, dq[4 * jb + 2], dq[4 * jb + 3]);
       }
       fence_proxy_async_smem();
-      mbar_arrive(BAR(DQ_FULL + NDQ * w + sb));
+      dqr.commit(n);
     };
     // dQ(i) retired: release its dS^T slot, stage the tile
     auto retire_dq = [&](int i) {
-      mbar_arrive(BAR(DS_EMPTY + i % NDS));
+      dsr.release(i);
       stage_dq(i);
     };
     auto issue_owned_dq = [&](int i) {        // i & 1 == w
-      mbar_wait(BAR(DS_FULL + i % NDS), (i / NDS) & 1);
+      dsr.wait(i);
       issue_dq(dq, ds_slot(i));
     };
 
@@ -742,7 +730,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     fence_regs(dk);
     fence_regs(dq);
     if (NT > 0) {
-      mbar_wait(BAR(FULL), 0);
+      qring.wait(0);
       issue_s_dp(s, dp, sQ, sDO);
       // i runs over the flat (head, query tile) sequence; row0 restarts at i_lo * QT with every head (next_row0)
       for (int i = 0, row0 = i_lo * QT; i < NT; ++i,
@@ -758,21 +746,20 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         fence_regs(pf);
         fence_regs(dsf);
         if (i >= 2 && ((i - 2) & 1) == w) retire_dq(i - 2);
-        if (i > 0) mbar_arrive(BAR(EMPTY + (i - 1) % NST));   // Q, dO and the stats of tile i - 1 are no longer read
+        if (i > 0) qring.release(i - 1);        // Q, dO and the stats of tile i - 1 are no longer read
         const bool own = (i & 1) == w;
-        if (own && i >= NDS) mbar_wait(BAR(DS_EMPTY + i % NDS), ((i - NDS) / NDS) & 1);
+        if (own && i >= NDS) dsr.acquire(i);
         elementwise_tile(s, dp, pf, dsf, row0, sStats + st * 8 * QT, ds_slot(i) + w * Cfg::kDS);
         // the slot arithmetic below is redone from an opaque copy of i rather than kept live through the elementwise
         // stage (the BIAS kernels have no register to spare there)
         int io = i;
         asm volatile("" : "+r"(io));
-        if ((io & 1) != w) mbar_arrive(BAR(DS_FULL + io % NDS));
+        if ((io & 1) != w) dsr.commit(io);
         issue_dv_dk(pf, dsf, sQs, sDOs, dv, dk);
         if (io >= 1 && (io & 1) != w) issue_owned_dq(io - 1);
         wgmma_commit();
         if (i + 1 < NT) {
-          const int sn = (i + 1) % NST;
-          mbar_wait(BAR(FULL + sn), ((i + 1) / NST) & 1);
+          const int sn = qring.wait(i + 1);
           issue_s_dp(s, dp, sQ + sn * Cfg::kQ, sDO + sn * Cfg::kQ);
         }
       }
@@ -782,7 +769,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       fence_regs(dk);
       fence_regs(dq);
       if (NT >= 2 && ((NT - 2) & 1) == w) retire_dq(NT - 2);
-      mbar_arrive(BAR(EMPTY + (NT - 1) % NST));
+      qring.release(NT - 1);
       if (((NT - 1) & 1) == w) {
         issue_owned_dq(NT - 1);
         wgmma_commit();
@@ -793,11 +780,10 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     }
   } else {
     for (int i = 0; i < NT; ++i) {
-      const int st = i % NST;
       const HeadTile ht = head_tile(i, i_lo, NI, HEAD_LOOP);
       const int hh = ht.head, row0 = ht.qt * QT;
+      const int st = qring.wait(i);
       const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
-      mbar_wait(BAR(FULL + st), (i / NST) & 1);
       float s[QT / 2], dp[QT / 2];
       issue_s_dp(s, dp, sQs, sDOs);
       wgmma_wait<0>();
@@ -819,7 +805,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       fence_regs(dv);
       fence_regs(dk);
       fence_regs(dq);
-      mbar_arrive(BAR(EMPTY + st));             // Q, dO and the stats of this stage are no longer read
+      qring.release(i);                         // Q, dO and the stats of this stage are no longer read
 
       // ---- dQ partial tile -> fp32 accumulator (rows = queries, columns = features) ----
       long long tile0 = ((long long)b * a.H + h0 + hh) * a.nqt;     // the accumulator tile of query tile 0

@@ -9,7 +9,7 @@
 //     64 = one wgmma M tile.  All G query heads of a group therefore share every K / V tile load.
 //   * warpgroup 0 : TMA producer (one thread): 128-key K and V tiles of the split's key range through mbarrier rings
 //   * warpgroup 1 : the 64 rows.  Q (8 or 16 KB) is loaded with ordinary loads into the 128-byte-swizzled layout;
-//                   per key tile S = Q K^T -> P = exp2(S*c1 - c2), masked -> O += P V, all as in the forward
+//                   per key tile the forward's step (key_tile.cuh): S = Q K^T -> P = exp2(S*c1 - c2) -> O += P V
 //   * visible length T_b = min(cache_seqlens[b] + n_new, capacity); query i sees key j iff j < T_b and, causal,
 //     j <= i + T_b - Nq (the forward's bottom-right rule with Nk = T_b).  The ceil(T_b / 128) tiles a block can see
 //     are cut into n_split contiguous chunks on the device, so a cache allocated at full length costs nothing.
@@ -17,8 +17,7 @@
 //     decode_combine_kernel forms o = sum_s O_s / max(sum_s l_s, 1e-37) in split order: o is bitwise reproducible.
 #pragma once
 
-#include "sm90_primitives.cuh"
-#include "tile_ranges.h"
+#include "key_tile.cuh"
 
 namespace fcsa {
 
@@ -62,9 +61,7 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
   using Cfg = DecodeCfg<D>;
   constexpr int S = Cfg::kStages, TILE = Cfg::kTile, DCH = D / 64;
 
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
+  uint8_t* smem = smem_1024();
   const uint32_t sQ = smem_u32(smem + Cfg::kOffQ);
   const uint32_t sK = smem_u32(smem + Cfg::kOffK);
   const uint32_t sV = smem_u32(smem + Cfg::kOffV);
@@ -72,6 +69,7 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
   auto BAR = [&](int i) { return bar0 + 8u * i; };
   constexpr int K_FULL = 0, K_EMPTY = K_FULL + S, V_FULL = K_EMPTY + S, V_EMPTY = V_FULL + S, NBARS = V_EMPTY + S;
   static_assert(NBARS * 8 <= 256, "barrier area");
+  const Ring<S> kr = {BAR(K_FULL), BAR(K_EMPTY)}, vr = {BAR(V_FULL), BAR(V_EMPTY)};
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;
@@ -87,12 +85,8 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
   const int r_last = min(r0 + 63, a.R - 1);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) {
-      mbar_init(BAR(K_FULL + s), 1);
-      mbar_init(BAR(K_EMPTY + s), 128);
-      mbar_init(BAR(V_FULL + s), 1);
-      mbar_init(BAR(V_EMPTY + s), 128);
-    }
+    kr.init(1, 128);
+    vr.init(1, 128);
     fence_mbar_init();
   }
   __syncthreads();
@@ -115,20 +109,7 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
     if (warp == 0 && elect_one() && j1 > j0) {
       tma_prefetch_desc(&tm_k);
       tma_prefetch_desc(&tm_v);
-      for (int j = j0; j < j1; ++j) {
-        const int s = (j - j0) % S;
-        const uint32_t par = (((j - j0) / S) & 1) ^ 1;
-        mbar_wait(BAR(K_EMPTY + s), par);
-        mbar_expect_tx(BAR(K_FULL + s), TILE);
-#pragma unroll
-        for (int ch = 0; ch < DCH; ++ch)
-          tma_load_4d(sK + s * TILE + ch * 16384, &tm_k, BAR(K_FULL + s), ch * 64, j * 128, hk, b);
-        mbar_wait(BAR(V_EMPTY + s), par);
-        mbar_expect_tx(BAR(V_FULL + s), TILE);
-#pragma unroll
-        for (int ch = 0; ch < DCH; ++ch)
-          tma_load_4d(sV + s * TILE + ch * 16384, &tm_v, BAR(V_FULL + s), ch * 64, j * 128, hk, b);
-      }
+      load_kv_tiles<D>(&tm_k, &tm_v, kr, vr, sK, sV, j0, j1, 0, hk, b);
     }
     return;
   }
@@ -160,24 +141,14 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
     named_bar_sync(1, 128);
   }
 
-  // last visible column of each of the thread's rows (-1: a padding row past R)
-  int lim[2];
+  // the visible key columns of each of the thread's rows (none for a padding row past R)
+  ColRange lim[2];
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     const int r = r0 + row_a + 8 * hf;
-    lim[hf] = r >= a.R ? -1 : (a.causal ? min(Tb - 1, r / a.G + off) : Tb - 1);
+    lim[hf] = r >= a.R ? ColRange{0, -1} : row_key_cols<WINDOW>(r / a.G, off, Tb, a.causal, W);
   }
-  int lo[2] = {0, 0};                         // WINDOW: first visible column of each row, and the band's upper side
-  if constexpr (WINDOW) {
-#pragma unroll
-    for (int hf = 0; hf < 2; ++hf) {
-      const int r = r0 + row_a + 8 * hf;
-      lo[hf] = r / a.G + off - W + 1;
-      if (!a.causal && r < a.R) lim[hf] = min(Tb - 1, r / a.G + off + W - 1);
-    }
-  }
-  const int first_lim = r0 / a.G + off;       // the block's smallest causal limit
-  const float c1 = a.c1, nc2 = -a.c2;
+  const float c1 = a.c1;
 
   float o[D / 2];
 #pragma unroll
@@ -185,56 +156,19 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
   float l[2] = {0.f, 0.f};
 
   for (int j = j0; j < j1; ++j) {
-    const int s = (j - j0) % S;
-    const uint32_t par = ((j - j0) / S) & 1;
-    // ---- S = Q K^T (64 x 128, fp32) ----
+    const int n = j - j0;                     // the rings' use
     float sacc[64];
-    mbar_wait(BAR(K_FULL + s), par);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk) {
-      const uint32_t qo = (kk >> 2) * 8192 + (kk & 3) * 32;
-      const uint32_t ko = (kk >> 2) * 16384 + (kk & 3) * 32;
-      wgmma_ss_n128<T, 0, 0>(sacc, gmma_desc_sw128(sQ + qo, 16, 1024), gmma_desc_sw128(sK + s * TILE + ko, 16, 1024),
-                             kk > 0 ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(sacc);
-    mbar_arrive(BAR(K_EMPTY + s));
+    const int s = kr.wait(n);
+    qk_tile<T, D>(sacc, sQ, 8192, sK + s * TILE);
+    kr.release(n);
 
-    // ---- P = exp2(S*c1 - c2), masked (a select: cache rows past T_b may hold anything); 16-bit P as A fragments --
+    // (a select: cache rows past T_b may hold anything)
     const int col0 = j * 128;
-    bool need_mask = (col0 + 127 >= Tb) || (a.causal && col0 + 127 > first_lim);
-    if constexpr (WINDOW)      // a column below the block's largest lower limit, or past its smallest upper one
-      need_mask = need_mask || col0 < r_last / a.G + off - W + 1 || col0 + 127 > first_lim + W - 1;
+    const bool need_mask = !tile_visible<WINDOW>(r0 / a.G, r_last / a.G, col0, col0 + 127, off, Tb, a.causal, W);
     uint32_t pf[32];
-    auto exp_tile = [&](auto masked_tag) {
-      constexpr bool MASKED = decltype(masked_tag)::value;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int hf = i & 1;
-        const int col = col0 + 8 * (i >> 1) + cq;
-        float p0 = ex2_approx(fmaf(sacc[2 * i], c1, nc2));
-        float p1 = ex2_approx(fmaf(sacc[2 * i + 1], c1, nc2));
-        if constexpr (MASKED) {
-          if constexpr (WINDOW) {
-            p0 = col <= lim[hf] && col >= lo[hf] ? p0 : 0.f;
-            p1 = col + 1 <= lim[hf] && col + 1 >= lo[hf] ? p1 : 0.f;
-          } else {
-            p0 = col <= lim[hf] ? p0 : 0.f;
-            p1 = col + 1 <= lim[hf] ? p1 : 0.f;
-          }
-        }
-        l[hf] += p0 + p1;
-        pf[i] = pack2<T>(p0, p1);
-      }
-    };
-    if (need_mask) exp_tile(std::true_type{});
-    else exp_tile(std::false_type{});
+    exp_tile<T, WINDOW>(need_mask, sacc, pf, l, c1, col0, cq, lim, ShiftOnly{-a.c2}, AllKeys{});
 
-    // ---- O += P V ----
-    mbar_wait(BAR(V_FULL + s), par);
+    vr.wait(n);
     if (col0 + 128 > Tb) {
       // the tile runs past T_b: its rows there are zeroed (P = 0 there, but 0 * NaN would not be 0)
       const int valid = Tb - col0;
@@ -246,38 +180,21 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
       fence_proxy_async_smem();
       named_bar_sync(1, 128);
     }
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      const uint32_t af[4] = {pf[4 * kk], pf[4 * kk + 1], pf[4 * kk + 2], pf[4 * kk + 3]};
-      const uint64_t dv = gmma_desc_sw128(sV + s * TILE + kk * 2048, 16384, 1024);
-      if constexpr (D == 64) wgmma_rs_n64<T, 1>(o, af, dv, 1u);
-      else wgmma_rs_n128<T, 1>(o, af, dv, 1u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(o);
-    fence_regs(pf);
-    mbar_arrive(BAR(V_EMPTY + s));
+    pv_tile<T>(o, pf, sV + s * TILE);
+    vr.release(n);
   }
 
   // ---- epilogue --------------------------------------------------------------------------
 #pragma unroll
-  for (int hf = 0; hf < 2; ++hf) {
-    l[hf] += __shfl_xor_sync(0xFFFFFFFFu, l[hf], 1);
-    l[hf] += __shfl_xor_sync(0xFFFFFFFFu, l[hf], 2);
-  }
+  for (int hf = 0; hf < 2; ++hf) l[hf] = quad_sum(l[hf]);
   if (a.n_split == 1) {
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
       const int r = r0 + row_a + 8 * hf;
       if (r >= a.R) continue;
       const int i = r / a.G, h = hk * a.G + (r - i * a.G);
-      const float inv = 1.0f / fmaxf(l[hf], 1e-37f);
-      T* orow = static_cast<T*>(a.o) + b * a.o_sb + h * a.o_sh + (long long)i * a.o_sn;
-#pragma unroll
-      for (int jb = 0; jb < D / 8; ++jb)
-        *reinterpret_cast<uint32_t*>(orow + 8 * jb + cq) = pack2<T>(o[4 * jb + 2 * hf] * inv, o[4 * jb + 2 * hf + 1] * inv);
+      store_row(static_cast<T*>(a.o) + b * a.o_sb + h * a.o_sh + (long long)i * a.o_sn, o, hf, cq,
+                1.0f / fmaxf(l[hf], 1e-37f));
     }
     return;
   }
@@ -289,9 +206,7 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     const int row = row_a + 8 * hf;
-#pragma unroll
-    for (int jb = 0; jb < D / 8; ++jb)
-      *reinterpret_cast<float2*>(po + row * D + 8 * jb + cq) = make_float2(o[4 * jb + 2 * hf], o[4 * jb + 2 * hf + 1]);
+    store_row(po + row * D, o, hf, cq, 1.f);
     if ((lane & 3) == 0) pl[row] = l[hf];
   }
 }

@@ -18,8 +18,7 @@
 //                   (D = 64) drift out of phase, so one's exps overlap another's products more often than two do.
 #pragma once
 
-#include "sm90_primitives.cuh"
-#include "tile_ranges.h"
+#include "key_tile.cuh"
 
 namespace fcsa {
 
@@ -77,6 +76,14 @@ struct FwdCfg {
   static_assert(kSmem <= 232448, "forward kernel shared memory");
 };
 
+// The exp stage's key padding mask (key_tile.cuh): key col is kept iff its byte in the batch's mask row is nonzero.
+struct PaddingMask {
+  const uint8_t* row;
+  bool has;
+  __device__ __forceinline__ bool on() const { return has; }
+  __device__ __forceinline__ bool operator()(int col) const { return row[col] != 0; }
+};
+
 template <bool VARLEN, bool WINDOW>
 using FwdArgsOf = std::conditional_t<WINDOW, Windowed<std::conditional_t<VARLEN, FwdVarlenArgs, FwdArgs>>,
                                      std::conditional_t<VARLEN, FwdVarlenArgs, FwdArgs>>;
@@ -92,9 +99,7 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   using Cfg = FwdCfg<D>;
   constexpr int S = Cfg::kStages, TILE = Cfg::kTile, DCH = D / 64, BM = Cfg::kBlockM;
 
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
+  uint8_t* smem = smem_1024();
   const uint32_t sQ = smem_u32(smem + Cfg::kOffQ);
   const uint32_t sK = smem_u32(smem + Cfg::kOffK);
   const uint32_t sV = smem_u32(smem + Cfg::kOffV);
@@ -103,6 +108,7 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   constexpr int Q_FULL = 0, K_FULL = 1, K_EMPTY = K_FULL + S, V_FULL = K_EMPTY + S, V_EMPTY = V_FULL + S,
                 NBARS = V_EMPTY + S;
   static_assert(NBARS * 8 <= 256, "barrier area");
+  const Ring<S> kr = {BAR(K_FULL), BAR(K_EMPTY)}, vr = {BAR(V_FULL), BAR(V_EMPTY)};
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;
@@ -125,12 +131,8 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
   if (threadIdx.x == 0) {
     mbar_init(BAR(Q_FULL), 1);
-    for (int s = 0; s < S; ++s) {
-      mbar_init(BAR(K_FULL + s), 1);
-      mbar_init(BAR(K_EMPTY + s), 128 * Cfg::kConsumers);
-      mbar_init(BAR(V_FULL + s), 1);
-      mbar_init(BAR(V_EMPTY + s), 128 * Cfg::kConsumers);
-    }
+    kr.init(1, 128 * Cfg::kConsumers);
+    vr.init(1, 128 * Cfg::kConsumers);
     fence_mbar_init();
   }
   __syncthreads();
@@ -156,20 +158,7 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       mbar_expect_tx(BAR(Q_FULL), Cfg::kQ);
 #pragma unroll
       for (int ch = 0; ch < DCH; ++ch) tma_load_4d(sQ + ch * BM * 128, &tm_q, BAR(Q_FULL), ch * 64, q_row0 + m0, h, tb);
-      for (int j = j_lo; j < NT; ++j) {
-        const int s = (j - j_lo) % S;
-        const uint32_t par = (((j - j_lo) / S) & 1) ^ 1;
-        mbar_wait(BAR(K_EMPTY + s), par);
-        mbar_expect_tx(BAR(K_FULL + s), TILE);
-#pragma unroll
-        for (int ch = 0; ch < DCH; ++ch)
-          tma_load_4d(sK + s * TILE + ch * 16384, &tm_k, BAR(K_FULL + s), ch * 64, k_row0 + j * 128, hk, tb);
-        mbar_wait(BAR(V_EMPTY + s), par);
-        mbar_expect_tx(BAR(V_FULL + s), TILE);
-#pragma unroll
-        for (int ch = 0; ch < DCH; ++ch)
-          tma_load_4d(sV + s * TILE + ch * 16384, &tm_v, BAR(V_FULL + s), ch * 64, k_row0 + j * 128, hk, tb);
-      }
+      load_kv_tiles<D>(&tm_k, &tm_v, kr, vr, sK, sV, j_lo, NT, k_row0, hk, tb);
     }
     return;
   }
@@ -193,19 +182,22 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       brow[hf] = reinterpret_cast<const T*>(a.bias) + (long long)b * a.bias_sb + (long long)h * a.bias_sh +
                  (long long)min(row_a + 8 * hf, a.Nq - 1) * a.bias_sn;
   }
-  // last visible column of each row (causal / ragged end)
-  int lim[2];
+  // the visible key columns of each of the thread's rows (the selects of a masked tile)
+  ColRange lim[2];
 #pragma unroll
-  for (int hf = 0; hf < 2; ++hf) lim[hf] = a.causal ? min(Nk - 1, row_a + 8 * hf + off) : Nk - 1;
-  // WINDOW: first visible column of each row, and the non-causal band's upper side
-  int lo[2] = {0, 0};
-  if constexpr (WINDOW) {
-#pragma unroll
-    for (int hf = 0; hf < 2; ++hf) {
-      lo[hf] = row_a + 8 * hf + off - W + 1;
-      if (!a.causal) lim[hf] = min(Nk - 1, row_a + 8 * hf + off + W - 1);
+  for (int hf = 0; hf < 2; ++hf) lim[hf] = row_key_cols<WINDOW>(row_a + 8 * hf, off, Nk, a.causal, W);
+  // the additive term (with BIAS: + bias * log2e) and the key padding mask of the exp stage
+  auto add = [&](int hf, int col) {
+    if constexpr (BIAS) {
+      uint32_t bw = 0;
+      if (col < a.Nk) bw = __ldg(reinterpret_cast<const unsigned int*>(brow[hf] + col));
+      const float2 bf = unpack2<T>(bw);
+      return make_float2(fmaf(bf.x, 1.4426950408889634f, nc2), fmaf(bf.y, 1.4426950408889634f, nc2));
+    } else {
+      return make_float2(nc2, nc2);
     }
-  }
+  };
+  const PaddingMask keys = {a.mask + (long long)b * a.mask_sb, a.has_mask != 0};
   // the key tiles [jw_lo, jw_hi) this warpgroup's own 64 rows see; it only passes the ring slots of the others on
   const TileRange wgt = warpgroup_key_tiles<WINDOW>(m0 + 64 * w, j_lo, NT, Nq, off, a.causal, W);
   const int jw_lo = wgt.lo, jw_hi = wgt.hi;
@@ -218,88 +210,27 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const uint32_t sQw = sQ + w * 64 * 128;     // this warpgroup's 64 rows inside every 64-feature chunk of Q
 
   for (int j = j_lo; j < NT; ++j) {
-    const int s = (j - j_lo) % S;
-    const uint32_t par = ((j - j_lo) / S) & 1;
-    if (j < jw_lo || j >= jw_hi) {            // (after the FULL wait: an arrival must count for this use of the slot)
-      mbar_wait(BAR(K_FULL + s), par);
-      mbar_arrive(BAR(K_EMPTY + s));
-      mbar_wait(BAR(V_FULL + s), par);
-      mbar_arrive(BAR(V_EMPTY + s));
+    const int n = j - j_lo;                   // the rings' use
+    if (j < jw_lo || j >= jw_hi) {
+      kr.pass(n);
+      vr.pass(n);
       continue;
     }
-    // ---- S = Q K^T (64 x 128, fp32) ----
     float sacc[64];
-    mbar_wait(BAR(K_FULL + s), par);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < D / 16; ++kk) {
-      const uint32_t ko = (kk & 3) * 32;       // + the 64-feature chunk (kk >> 2) below
-      wgmma_ss_n128<T, 0, 0>(sacc, gmma_desc_sw128(sQw + (kk >> 2) * BM * 128 + ko, 16, 1024),
-                             gmma_desc_sw128(sK + s * TILE + (kk >> 2) * 16384 + ko, 16, 1024), kk > 0 ? 1u : 0u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(sacc);
-    mbar_arrive(BAR(K_EMPTY + s));
+    const int s = kr.wait(n);
+    qk_tile<T, D>(sacc, sQw, BM * 128, sK + s * TILE);
+    kr.release(n);
 
-    // ---- P = exp2(S*c1 - c2 [+ bias*log2e]), masked; row sums in fp32; 16-bit P as A fragments ----
+    // (the warpgroup's 64 rows unclipped: rows past Nq are never stored, and a later last row only masks more)
     const int col0 = j * 128;
-    bool need_mask = a.has_mask || (col0 + 127 >= Nk) || (a.causal && col0 + 127 > m0 + 64 * w + off);
-    // (window: a column below the warpgroup's largest lower limit, or past its smallest upper one)
-    if constexpr (WINDOW)
-      need_mask = need_mask || col0 < m0 + 64 * w + 63 + off - W + 1 || col0 + 127 > m0 + 64 * w + off + W - 1;
+    const bool need_mask =
+        a.has_mask || !tile_visible<WINDOW>(m0 + 64 * w, m0 + 64 * w + 63, col0, col0 + 127, off, Nk, a.causal, W);
     uint32_t pf[32];
-    auto exp_tile = [&](auto masked_tag) {
-      constexpr bool MASKED = decltype(masked_tag)::value;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int hf = i & 1;                                 // row_a or row_a + 8
-        const int col = col0 + 8 * (i >> 1) + cq;
-        float add0 = nc2, add1 = nc2;
-        if constexpr (BIAS) {
-          uint32_t bw = 0;
-          if (col < a.Nk) bw = __ldg(reinterpret_cast<const unsigned int*>(brow[hf] + col));
-          const float2 bf = unpack2<T>(bw);
-          add0 = fmaf(bf.x, 1.4426950408889634f, nc2);
-          add1 = fmaf(bf.y, 1.4426950408889634f, nc2);
-        }
-        float p0 = ex2_approx(fmaf(sacc[2 * i], c1, add0));
-        float p1 = ex2_approx(fmaf(sacc[2 * i + 1], c1, add1));
-        if constexpr (MASKED) {
-          bool v0 = col <= lim[hf], v1 = col + 1 <= lim[hf];
-          if constexpr (WINDOW) {
-            v0 = v0 && col >= lo[hf];
-            v1 = v1 && col + 1 >= lo[hf];
-          }
-          if (a.has_mask) {
-            v0 = v0 && a.mask[(long long)b * a.mask_sb + col] != 0;
-            v1 = v1 && a.mask[(long long)b * a.mask_sb + col + 1] != 0;
-          }
-          p0 = v0 ? p0 : 0.f;
-          p1 = v1 ? p1 : 0.f;
-        }
-        l[hf] += p0 + p1;
-        pf[i] = pack2<T>(p0, p1);
-      }
-    };
-    if (need_mask) exp_tile(std::true_type{});
-    else exp_tile(std::false_type{});
+    exp_tile<T, WINDOW>(need_mask, sacc, pf, l, c1, col0, cq, lim, add, keys);
 
-    // ---- O += P V ----
-    mbar_wait(BAR(V_FULL + s), par);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 8; ++kk) {
-      const uint32_t af[4] = {pf[4 * kk], pf[4 * kk + 1], pf[4 * kk + 2], pf[4 * kk + 3]};
-      const uint64_t dv = gmma_desc_sw128(sV + s * TILE + kk * 2048, 16384, 1024);
-      if constexpr (D == 64) wgmma_rs_n64<T, 1>(o, af, dv, 1u);
-      else wgmma_rs_n128<T, 1>(o, af, dv, 1u);
-    }
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(o);
-    fence_regs(pf);
-    mbar_arrive(BAR(V_EMPTY + s));
+    vr.wait(n);
+    pv_tile<T>(o, pf, sV + s * TILE);
+    vr.release(n);
   }
 
   // ---- epilogue: O * 1/max(l, eps) -> global ----------------------------------------------
@@ -308,30 +239,14 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   // makes legitimately tiny row sums).
   float inv[2];
 #pragma unroll
-  for (int hf = 0; hf < 2; ++hf) {
-    float x = l[hf];
-    x += __shfl_xor_sync(0xFFFFFFFFu, x, 1);
-    x += __shfl_xor_sync(0xFFFFFFFFu, x, 2);
-    inv[hf] = 1.0f / fmaxf(x, 1e-37f);
-  }
+  for (int hf = 0; hf < 2; ++hf) inv[hf] = 1.0f / fmaxf(quad_sum(l[hf]), 1e-37f);
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     const int row = row_a + 8 * hf;
     if (row >= Nq) continue;
     const long long o_off = (long long)tb * a.o_sb + (long long)h * a.o_sh + (long long)(q_row0 + row) * a.o_sn;
-    if (a.o_f32) {
-      float* orow = reinterpret_cast<float*>(a.o) + o_off;
-#pragma unroll
-      for (int jb = 0; jb < D / 8; ++jb)
-        *reinterpret_cast<float2*>(orow + 8 * jb + cq) =
-            make_float2(o[4 * jb + 2 * hf] * inv[hf], o[4 * jb + 2 * hf + 1] * inv[hf]);
-    } else {
-      T* orow = reinterpret_cast<T*>(a.o) + o_off;
-#pragma unroll
-      for (int jb = 0; jb < D / 8; ++jb)
-        *reinterpret_cast<uint32_t*>(orow + 8 * jb + cq) =
-            pack2<T>(o[4 * jb + 2 * hf] * inv[hf], o[4 * jb + 2 * hf + 1] * inv[hf]);
-    }
+    if (a.o_f32) store_row(reinterpret_cast<float*>(a.o) + o_off, o, hf, cq, inv[hf]);
+    else store_row(reinterpret_cast<T*>(a.o) + o_off, o, hf, cq, inv[hf]);
     if ((lane & 3) == 0 && a.inv_l != nullptr) {
       if constexpr (VARLEN) a.inv_l[(long long)h * a.total_q + q_row0 + row] = inv[hf];
       else a.inv_l[((long long)b * a.H + h) * a.Nq + row] = inv[hf];

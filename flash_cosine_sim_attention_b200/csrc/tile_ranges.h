@@ -1,5 +1,6 @@
-// Which tiles a work item visits, and the host rules that size the grids from the same quantities: the one
-// definition, for the three attention kernels (device), the launch code (host) and the CPU tests
+// Which tiles a work item visits, which of them the forward and decode must mask per element, and the host rules that
+// size the grids from the same quantities: the one definition, for the three attention kernels (device), the launch
+// code (host) and the CPU tests
 // (tests/tile_ranges_host.cpp compiles this header with the host compiler alone).
 //
 // Visibility is the public rule: query i sees key j iff j <= i + (Nk - Nq) when causal (bottom-right aligned), and,
@@ -85,6 +86,31 @@ FCSA_TILE_FN TileRange warpgroup_key_tiles(int r0, int blk_lo, int blk_hi, int N
 FCSA_TILE_FN TileRange split_chunk(TileRange t, int split, int n_split) {
   return {t.lo + (int)((long long)(t.hi - t.lo) * split / n_split),
           t.lo + (int)((long long)(t.hi - t.lo) * (split + 1) / n_split)};
+}
+
+// ---- the masks of the forward and decode exp stages --------------------------------------------------------------
+// The key columns [lo, hi] (inclusive) that query i sees among Nk keys: the per-element limits of a masked tile.
+struct ColRange {
+  int lo, hi;
+};
+template <bool WINDOW>
+FCSA_TILE_FN ColRange row_key_cols(int i, int off, int Nk, int causal, int W) {
+  ColRange c = {0, causal ? tile_min(Nk - 1, i + off) : Nk - 1};
+  if constexpr (WINDOW) {
+    c.lo = i + off - W + 1;
+    if (!causal) c.hi = tile_min(Nk - 1, i + off + W - 1);
+  }
+  return c;
+}
+
+// True iff every key of [k_first, k_last] exists and is visible to every query of [q_first, q_last]: such a tile
+// needs no per-element selects.  Only the corners decide: the causal limit and the window's upper side are smallest
+// for the first query, the window's lower side largest for the last.
+template <bool WINDOW>
+FCSA_TILE_FN bool tile_visible(int q_first, int q_last, int k_first, int k_last, int off, int Nk, int causal, int W) {
+  bool all = k_last < Nk && !(causal && k_last > q_first + off);
+  if constexpr (WINDOW) all = all && !(k_first < q_last + off - W + 1 || k_last > q_first + off + W - 1);
+  return all;
 }
 
 // ---- query tiles of a key tile (backward) --------------------------------------------------------------------------

@@ -34,6 +34,8 @@ def _lib():
         "fcsa_decode_chunk": [i, i, i, i, i, i, i, i, i, p, p],
         "fcsa_query_tiles": [i, i, i, i, i, i, p, p],
         "fcsa_bwd_row0_sequence": [i, i, i, i, i, i, i, i, p, p],
+        "fcsa_row_key_cols": [i, i, i, i, i, p, p],
+        "fcsa_tile_visible": [p, p, i, i, i, i, i, i, p],
         "fcsa_varlen_tile_base": [i, i],
         "fcsa_varlen_tiles": [i, ctypes.c_longlong],
         "fcsa_fwd_block_rows": [i],
@@ -107,6 +109,24 @@ def decode_range(r0, R, G, Tb, nq, w, causal, n_split):
     r_last = min(r0 + 63, R - 1)
     return [_ranges(_lib().fcsa_decode_chunk, w, r0 // G, r_last // G, nq, Tb, int(causal), s, n_split)
             for s in range(n_split)]
+
+
+def row_key_cols(nq, nk, w, causal):
+    """The forward's and decode's per-element limits: the key columns [lo, hi] each query sees, as (W, nq) arrays."""
+    b, e = _span(w)
+    lo, hi = np.empty((e - b, nq), np.int32), np.empty((e - b, nq), np.int32)
+    _lib().fcsa_row_key_cols(nq, nk, int(causal), b, e, lo, hi)
+    return lo, hi
+
+
+def tile_visible(q_first, q_last, nq, nk, w, causal):
+    """Whether query rows [q_first[r], q_last[r]] see every key of each 128-key tile (the tile needs no masks):
+    (W, ranges, key tiles) bool."""
+    b, e = _span(w)
+    q_first, q_last = np.ascontiguousarray(q_first, np.int32), np.ascontiguousarray(q_last, np.int32)
+    out = np.empty((e - b, len(q_first), (nk + 127) // 128), np.int32)
+    _lib().fcsa_tile_visible(q_first, q_last, len(q_first), nq, nk, int(causal), b, e, out)
+    return out.astype(bool)
 
 
 def decode_window_keys(cap, window, causal):

@@ -69,6 +69,31 @@ void fcsa_bwd_row0_sequence(int key0, int nq, int nk, int causal, int hpc, int w
   }
 }
 
+// The key columns [lo, hi] every query i < nq sees among nk keys, under every window: lo[w][i], hi[w][i].
+void fcsa_row_key_cols(int nq, int nk, int causal, int w_begin, int w_end, int* lo, int* hi) {
+  for (int w = w_begin; w < (w_begin ? w_end : 1); ++w)
+    for (int i = 0; i < nq; ++i) {
+      const ColRange c = w_begin ? row_key_cols<true>(i, diag_off(nq, nk), nk, causal, w)
+                                 : row_key_cols<false>(i, diag_off(nq, nk), nk, causal, 0);
+      lo[(long long)(w - w_begin) * nq + i] = c.lo, hi[(long long)(w - w_begin) * nq + i] = c.hi;
+    }
+}
+
+// Whether the query rows [q_first[r], q_last[r]] see every key of key tile t, under every window: out[w][r][t] for
+// the ceil(nk / 128) tiles of 128 keys.
+void fcsa_tile_visible(const int* q_first, const int* q_last, int n_ranges, int nq, int nk, int causal, int w_begin,
+                       int w_end, int* out) {
+  const int nt = (nk + 127) / 128;
+  for (int w = w_begin; w < (w_begin ? w_end : 1); ++w)
+    for (int r = 0; r < n_ranges; ++r)
+      for (int t = 0; t < nt; ++t) {
+        const int off = diag_off(nq, nk), k0 = 128 * t;
+        out[((long long)(w - w_begin) * n_ranges + r) * nt + t] =
+            w_begin ? tile_visible<true>(q_first[r], q_last[r], k0, k0 + 127, off, nk, causal, w)
+                    : tile_visible<false>(q_first[r], q_last[r], k0, k0 + 127, off, nk, causal, 0);
+      }
+}
+
 int fcsa_varlen_tile_base(int start, int b) { return varlen_tile_base(start, b); }
 int fcsa_varlen_tiles(int B, long long total_q) { return varlen_tiles(B, total_q); }
 int fcsa_fwd_block_rows(int D) { return fwd_block_rows(D); }
