@@ -46,6 +46,10 @@ EXPORTED_SYMBOLS = (
     "fcsa_backward_fused_varlen_workspace_bytes",
     "fcsa_backward_fused_varlen_zeroed_bytes",
     "fcsa_backward_fused_varlen",
+    "fcsa_backward_fused_deterministic_workspace_bytes",
+    "fcsa_backward_fused_deterministic",
+    "fcsa_backward_fused_deterministic_varlen_workspace_bytes",
+    "fcsa_backward_fused_deterministic_varlen",
 )
 
 
@@ -158,6 +162,16 @@ def load():
     lib.fcsa_backward_fused_varlen.restype = c_int32
     lib.fcsa_backward_fused_varlen.argtypes = [PP, PV, PN, PT, PT, PT, c_void_p, PT, PT, PT, c_void_p, c_size_t,
                                                c_void_p, c_size_t, c_void_p]
+    lib.fcsa_backward_fused_deterministic_workspace_bytes.restype = c_size_t
+    lib.fcsa_backward_fused_deterministic_workspace_bytes.argtypes = [PP]
+    lib.fcsa_backward_fused_deterministic.restype = c_int32
+    lib.fcsa_backward_fused_deterministic.argtypes = [PP, PN, PT, PT, PT, c_void_p, PT, PT, PT, c_void_p, c_size_t,
+                                                      c_void_p]
+    lib.fcsa_backward_fused_deterministic_varlen_workspace_bytes.restype = c_size_t
+    lib.fcsa_backward_fused_deterministic_varlen_workspace_bytes.argtypes = [PP, PV]
+    lib.fcsa_backward_fused_deterministic_varlen.restype = c_int32
+    lib.fcsa_backward_fused_deterministic_varlen.argtypes = [PP, PV, PN, PT, PT, PT, c_void_p, PT, PT, PT, c_void_p,
+                                                             c_size_t, c_void_p]
     lib.fcsa_set_kernel_events.restype = c_int32
     lib.fcsa_set_kernel_events.argtypes = [c_int32, c_void_p, c_void_p]
     _lib = lib

@@ -310,13 +310,14 @@ __device__ __forceinline__ float4 ldg_cg128f(const float* p) {
 // l2norm backward of one key row in the backward epilogue: dk = (dk_hat - k_hat <k_hat, dk_hat>_group) * rnorm_group.
 // The thread holds features 8 jb + cq + {0, 1} (g[2 jb], g[2 jb + 1]) of the row; the row's other features are in the
 // other three lanes of its quad.  k_hat comes from the resident K tile (row address sk_row, 128B swizzle, 64-feature
-// chunks 16 KB apart).  All lanes of the warp must call it (quad shuffles); `in` = the key exists.
+// chunks 16 KB apart).  All lanes of the warp must call it (quad shuffles); `in` = the key exists.  k_rnorm has
+// `groups` floats per row; the key's row is krow0 + key.  (The dQ kernel applies it to a row of its resident Q tile.)
 template <typename T, int D>
-__device__ __forceinline__ void l2norm_bwd_key_row(float (&g)[D / 4], const BwdArgs& a, uint32_t sk_row, long long krow0,
-                                                   int key, bool in) {
+__device__ __forceinline__ void l2norm_bwd_key_row(float (&g)[D / 4], const float* k_rnorm, int groups, uint32_t sk_row,
+                                                   long long krow0, int key, bool in) {
   const int lane = threadIdx.x & 31;
   const int r8 = (lane >> 2) & 7, cq = 2 * (lane & 3);
-  const int gs = D / a.groups;                  // features per group (a power of two)
+  const int gs = D / groups;                    // features per group (a power of two)
   float y[D / 4], dot[D / 4];
 #pragma unroll
   for (int jb = 0; jb < D / 8; ++jb) {
@@ -355,7 +356,7 @@ __device__ __forceinline__ void l2norm_bwd_key_row(float (&g)[D / 4], const BwdA
     for (int jb = 0; jb < D / 8; ++jb) dot[2 * jb] = dot[2 * jb + 1] = q[jb];
   }
   const int lg = __ffs(gs) - 1;
-  const float* rn = a.k_rnorm + (krow0 + (in ? key : 0)) * a.groups;     // k_rnorm row krow0 + key
+  const float* rn = k_rnorm + (krow0 + (in ? key : 0)) * groups;         // k_rnorm row krow0 + key
   // one load per feature pair (a pair shares its group unless gs = 1); the pairs of one group hit the same L1 line
 #pragma unroll
   for (int jb = 0; jb < D / 8; ++jb) {
@@ -376,7 +377,11 @@ using BwdArgsOf = std::conditional_t<WINDOW, Windowed<std::conditional_t<VARLEN,
 // VARLEN: packed sequences (BwdVarlenArgs); `b` is then the sequence, and its lengths replace Nq / Nk.
 // WINDOW: sliding-window attention (Windowed<>::window = W): a key tile visits query tiles [i_lo, i_end) instead of
 // [i_lo, nqt), i_end being the tile after the last query row whose lower limit reaches key0 + 127.
-template <typename T, int D, bool BIAS = false, bool HEAD_LOOP = false, bool VARLEN = false, bool WINDOW = false>
+// DQ = false: dK and dV only (the deterministic backward, whose dq comes from fcsa_dq_kernel).  No dS^T in shared
+// memory, no dQ product, no reducer warps, no dq accumulator; both head dims run the in-order loop, and the host
+// launches it with split = 1, so dk / dv always leave through the direct epilogue.
+template <typename T, int D, bool BIAS = false, bool HEAD_LOOP = false, bool VARLEN = false, bool WINDOW = false,
+          bool DQ = true>
 __global__ void __launch_bounds__(384, 1)
 fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                 const __grid_constant__ CUtensorMap tm_v, const __grid_constant__ CUtensorMap tm_do,
@@ -385,8 +390,9 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   static_assert(!(BIAS && HEAD_LOOP), "BIAS launches have one query head per CTA");
   static_assert(!(BIAS && VARLEN), "packed sequences take no bias");
   static_assert(!(BIAS && WINDOW), "a window takes no bias");
+  static_assert(DQ || !BIAS, "the dK / dV-only kernel takes no bias");
   using Cfg = BwdCfg<D>;
-  constexpr bool STAGED = Cfg::kStaged;
+  constexpr bool STAGED = Cfg::kStaged && DQ;
   constexpr int QT = Cfg::QT;              // query rows per tile
   constexpr int KCH = D / 64;              // 64-feature chunks of every operand tile
   constexpr int QCHUNK = QT * 128;         // bytes of one 64-feature chunk of a Q / dO stage
@@ -615,7 +621,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         const float ds0 = p0 * (dp[2 * e] + ndl.x), ds1 = p1 * (dp[2 * e + 1] + ndl.y);
         pf[e] = pack2<T>(p0, p1);
         dsf[e] = pack2<T>(ds0, ds1);
-        sts32(ds_addr + 1024 * hf, dsf[e]);
+        if constexpr (DQ) sts32(ds_addr + 1024 * hf, dsf[e]);
         if constexpr (BIAS) {
           // d bias = dS (reference cu:1574-1576): fp32 reduction
           if (a.dbias != nullptr) {
@@ -637,8 +643,10 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
                  row0 + QT - 1 <= key0 + 64 * w + hi_off;
     if (!BIAS && interior) elementwise(false, s, dp, pf, dsf, row0, stc3, dsbuf);
     else elementwise(true, s, dp, pf, dsf, row0, stc3, dsbuf);
-    fence_proxy_async_smem();
-    named_bar_sync(1 + w, 128);               // the warpgroup's whole dS^T tile is in shared memory
+    if constexpr (DQ) {
+      fence_proxy_async_smem();
+      named_bar_sync(1 + w, 128);             // the warpgroup's whole dS^T tile is in shared memory
+    }
   };
 
   // dV += P^T dO, dK += dS^T Q (A from registers)
@@ -798,6 +806,12 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       wgmma_wait<0>();                          // the dQ accumulator only fits once the A fragments are dead
       fence_regs(pf);
       fence_regs(dsf);
+      if constexpr (!DQ) {
+        fence_regs(dv);
+        fence_regs(dk);
+        qring.release(i);                       // Q, dO and the stats of this stage are no longer read
+        continue;
+      }
       float dq[D / 2];
       issue_dq(dq, dsbuf);
       wgmma_commit();
@@ -825,7 +839,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
   // ---- epilogue: dV and dK * scale of the warpgroup's 64 keys ---------------------------------
   // (no early exit for keys at or beyond Nk: the l2norm backward below shuffles within the quad of a key row)
-  const bool to_acc = a.split > 1;
+  const bool to_acc = DQ && a.split > 1;
   long long krow0 = ((long long)b * a.kv_heads + hk) * a.Nk;     // the row of key 0 in k_rnorm and dk_acc / dv_acc
   if constexpr (VARLEN) {
     // the key span is read again rather than kept in registers through the main loop
@@ -875,7 +889,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         g[2 * jb] = dk[4 * jb + 2 * hf] * a.scale;
         g[2 * jb + 1] = dk[4 * jb + 2 * hf + 1] * a.scale;
       }
-      if (a.k_rnorm != nullptr) l2norm_bwd_key_row<T, D>(g, a, sK + (64 * w + kr + 8 * hf) * 128, krow0, key, in);
+      if (a.k_rnorm != nullptr)
+        l2norm_bwd_key_row<T, D>(g, a.k_rnorm, a.groups, sK + (64 * w + kr + 8 * hf) * 128, krow0, key, in);
       if (in) {
 #pragma unroll
         for (int jb = 0; jb < D / 8; ++jb)

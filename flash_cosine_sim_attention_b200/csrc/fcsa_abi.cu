@@ -20,6 +20,7 @@
 #include "../../include/fcsa_b200.h"
 #include "bwd_kernel.cuh"
 #include "decode_kernel.cuh"
+#include "dq_kernel.cuh"
 #include "fwd_kernel.cuh"
 #include "l2norm_kernels.cuh"
 #include "tensor_map.h"
@@ -27,7 +28,7 @@
 namespace {
 
 thread_local char g_err[512] = "";
-cudaEvent_t g_ev[5][2] = {};   // 0 forward, 1 backward, 2 l2norm(q,k), 3 backward preprocess, 4 dq finish
+cudaEvent_t g_ev[5][2] = {};   // 0 forward, 1 backward, 2 l2norm(q,k), 3 backward preprocess, 4 dq finish / dQ kernel
 std::atomic<long long> g_launches{0};
 
 int fail(int code, const char* fmt, ...) {
@@ -342,6 +343,9 @@ fcsa::BwdWorkspace bwd_layout(const fcsa_problem* p, const fcsa_varlen* vl) {
   return fcsa::bwd_workspace_layout(p->batch, p->heads, p->kv_heads, p->seq_q, p->seq_k, p->head_dim);
 }
 
+// The deterministic backward's scratch: the stats alone (no dq accumulator, and no dk / dv accumulators: split = 1)
+size_t bwd_deterministic_bytes(const fcsa::BwdWorkspace& w) { return w.dkv_off; }
+
 // The backward's arguments, filled from the problem and the caller's tensors by backward_impl
 struct BwdHostArgs {
   int B, H, kv_heads, Nq, Nk, causal;
@@ -352,7 +356,9 @@ struct BwdHostArgs {
   const float* inv_l;
   bool out_f32;                     // o (read), dq, dk, dv (written) are float32
   void* workspace;                  // scratch
-  void* zeroed;                     // zero on entry, zero again on exit (dq accumulator)
+  void* zeroed;                     // zero on entry, zero again on exit (dq accumulator); unused when deterministic
+  // the deterministic route: dK / dV with split = 1 (fcsa_bwd_kernel<DQ = false>), then fcsa_dq_kernel
+  bool deterministic = false;
   // fused l2norm backward (q, k above are then the NORMALISED tensors and dq, dk the gradients
   // w.r.t. the raw ones); both null = plain backward
   const float* q_rnorm;
@@ -369,8 +375,47 @@ struct BwdHostArgs {
   int total_q = 0, total_k = 0;
 };
 
+// The dQ kernel of the deterministic backward, after the dK / dV kernel: one CTA per (block of dq_block_rows query
+// rows, batch, query head); packed sequences: blocks of the longest sequence.
+template <typename T, int D, bool VARLEN>
+int launch_dq(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, const float* stats, cudaStream_t stream) {
+  using Cfg = fcsa::DqCfg<D>;
+  const int tB = VARLEN ? 1 : h.B, tNq = VARLEN ? h.total_q : h.Nq, tNk = VARLEN ? h.total_k : h.Nk;
+  CUtensorMap tq, tk, tv, tdo;
+  int r;
+  if ((r = map_operand<T, D>(&tq, "q", h.q, tB, h.H, tNq, Cfg::kBlockM)) ||
+      (r = map_operand<T, D>(&tk, "k", h.k, tB, h.kv_heads, tNk, 128)) ||
+      (r = map_operand<T, D>(&tv, "v", h.v, tB, h.kv_heads, tNk, 128)) ||
+      (r = map_operand<T, D>(&tdo, "d_o", h.d_o, tB, h.H, tNq, Cfg::kBlockM)))
+    return r;
+  fcsa::DqArgsOf<VARLEN, true> a;
+  a.window = h.window;
+  if constexpr (VARLEN) {
+    a.cu_q = h.cu_q; a.cu_k = h.cu_k; a.total_q = h.total_q; a.total_k = h.total_k; a.ntile = w.nqt;
+  }
+  a.B = h.B; a.H = h.H; a.Nq = h.Nq; a.Nk = h.Nk; a.causal = h.causal; a.has_mask = h.mask ? 1 : 0;
+  a.group = h.H / h.kv_heads;
+  a.n_qblk = fcsa::row_blocks(h.Nq, Cfg::kBlockM);
+  a.nqt = w.nqt;
+  a.c1 = h.scale * 1.4426950408889634f; a.scale = h.scale;
+  a.mask = h.mask; a.mask_sb = h.mask_sb;
+  a.stats = stats;
+  a.out_f32 = h.out_f32 ? 1 : 0;
+  a.dq = h.dq.ptr; a.dq_sb = h.dq.sb; a.dq_sh = h.dq.sh; a.dq_sn = h.dq.sn;
+  a.q_rnorm = h.q_rnorm; a.groups = h.groups;
+  const long long grid = (long long)a.n_qblk * h.B * h.H;
+  if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
+  const auto launch = [&](auto kern) {
+    return launch_attention<decltype(kern)::value>("dQ", g_ev[4], grid, Cfg::kThreads, Cfg::kSmem, stream, tq, tk, tv,
+                                                   tdo, a);
+  };
+  return a.window > 0 ? launch(kernel_c<fcsa::fcsa_dq_kernel<T, D, VARLEN, true>>{})
+                      : launch(kernel_c<fcsa::fcsa_dq_kernel<T, D, VARLEN>>{});
+}
+
 // The backward's launches: preprocess, main kernel, dq finish, and for split groups the dk / dv finish (and the l2norm
-// backward of dk).  w: the workspaces' layout (bwd_layout).
+// backward of dk).  Deterministic: preprocess, the dK / dV kernel with split = 1, the dQ kernel.  w: the workspaces'
+// layout (bwd_layout).
 template <typename T, int D, bool BIAS = false, bool VARLEN = false>
 int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream_t stream) {
   using namespace fcsa;
@@ -387,7 +432,7 @@ int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream
   cudaError_t e;
   int r;
   int split = 1;
-  if (h.kv_heads < h.H) {
+  if (h.kv_heads < h.H && !h.deterministic) {
     int sms = 0;
     e = device_sm_count(&sms);
     if (e != cudaSuccess) return cuda_fail(e, "cudaDeviceGetAttribute(multiProcessorCount)");
@@ -435,7 +480,7 @@ int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream
     // sequences: [1][H][ntile * QT][D], every tile inside the map)
     memset(&tdq, 0, sizeof(tdq));
     const long long acc_sh = (long long)w.nqt * Cfg::QT * D;
-    if (Cfg::kStaged &&
+    if (Cfg::kStaged && !h.deterministic &&
         (r = make_tensor_map_bhnd(&tdq, dq_acc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, tB, h.H, VARLEN ? w.nqt * Cfg::QT : h.Nq,
                                   D, h.H * acc_sh, acc_sh, D, Cfg::QT, 32)))
       return fail(FCSA_ERR_CUDA, "dq accumulator: cuTensorMapEncodeTiled failed (%d)", r);
@@ -465,15 +510,23 @@ int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream
       return launch_attention<decltype(kern)::value>("backward", g_ev[1], items, Cfg::kThreads, Cfg::kSmem, stream,
                                                      tq, tk, tv, tdo, tdq, a);
     };
+    // DQ = false: the dK / dV kernel of the deterministic route
+    const auto launch_main = [&](auto dq) {
+      constexpr bool DQ = decltype(dq)::value;
+      if (a.hpc > 1)   // HEAD_LOOP
+        return a.window > 0 ? launch(kernel_c<fcsa_bwd_kernel<T, D, false, true, VARLEN, true, DQ>>{})
+                            : launch(kernel_c<fcsa_bwd_kernel<T, D, false, true, VARLEN, false, DQ>>{});
+      return a.window > 0 ? launch(kernel_c<fcsa_bwd_kernel<T, D, false, false, VARLEN, true, DQ>>{})
+                          : launch(kernel_c<fcsa_bwd_kernel<T, D, false, false, VARLEN, false, DQ>>{});
+    };
     if constexpr (BIAS)   // (one query head per CTA, no window)
       r = launch(kernel_c<fcsa_bwd_kernel<T, D, true>>{});
-    else if (a.hpc > 1)   // HEAD_LOOP
-      r = a.window > 0 ? launch(kernel_c<fcsa_bwd_kernel<T, D, false, true, VARLEN, true>>{})
-                       : launch(kernel_c<fcsa_bwd_kernel<T, D, false, true, VARLEN>>{});
     else
-      r = a.window > 0 ? launch(kernel_c<fcsa_bwd_kernel<T, D, false, false, VARLEN, true>>{})
-                       : launch(kernel_c<fcsa_bwd_kernel<T, D, false, false, VARLEN>>{});
+      r = h.deterministic ? launch_main(std::false_type{}) : launch_main(std::true_type{});
     if (r) return r;
+  }
+  if constexpr (!BIAS) {
+    if (h.deterministic) return launch_dq<T, D, VARLEN>(h, w, stats, stream);
   }
   // 3. finish
   {
@@ -579,13 +632,14 @@ int fcsa_zeroed_init(void* zeroed, size_t bytes, void* stream) {
 }
 
 // Every backward entry point: dense or packed sequences (vl), with the fused l2norm backward over `groups` when
-// q_rnorm / k_rnorm are set (q, k are then the normalised tensors), or with a bias.
+// q_rnorm / k_rnorm are set (q, k are then the normalised tensors), or with a bias.  deterministic: the route without
+// atomics, which needs the stats alone as scratch and no zeroed workspace (zeroed is ignored).
 static int backward_impl(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_tensor* q, const fcsa_tensor* k,
                          const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o,
                          const float* inv_l, const fcsa_tensor* dq, const fcsa_tensor* dk,
                          const fcsa_tensor* dv, void* workspace, size_t workspace_bytes, void* zeroed,
                          size_t zeroed_bytes, void* stream,
-                         const float* q_rnorm, const float* k_rnorm, int groups,
+                         const float* q_rnorm, const float* k_rnorm, int groups, bool deterministic,
                          const fcsa_bias* bias = nullptr, float* d_bias_acc = nullptr, int64_t dsb = 0,
                          int64_t dsh = 0) {
   int r;
@@ -597,12 +651,15 @@ static int backward_impl(const fcsa_problem* p, const fcsa_varlen* vl, const fcs
     return r;
   if (!inv_l) return fail(FCSA_ERR_INVALID, "inv_l: null");
   const fcsa::BwdWorkspace w = bwd_layout(p, vl);
-  if (!workspace || workspace_bytes < w.total)
-    return fail(FCSA_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w.total, workspace_bytes);
+  const size_t need = deterministic ? bwd_deterministic_bytes(w) : w.total;
+  if (!workspace || workspace_bytes < need)
+    return fail(FCSA_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need, workspace_bytes);
   if (!aligned16(workspace)) return fail(FCSA_ERR_INVALID, "workspace not 16-byte aligned");
-  if (!zeroed || zeroed_bytes < w.ztotal)
-    return fail(FCSA_ERR_WORKSPACE, "zeroed workspace too small: need %zu bytes, got %zu", w.ztotal, zeroed_bytes);
-  if (!aligned16(zeroed)) return fail(FCSA_ERR_INVALID, "zeroed workspace not 16-byte aligned");
+  if (!deterministic) {
+    if (!zeroed || zeroed_bytes < w.ztotal)
+      return fail(FCSA_ERR_WORKSPACE, "zeroed workspace too small: need %zu bytes, got %zu", w.ztotal, zeroed_bytes);
+    if (!aligned16(zeroed)) return fail(FCSA_ERR_INVALID, "zeroed workspace not 16-byte aligned");
+  }
   if (p->out_f32 && (q_rnorm || k_rnorm))
     return fail(FCSA_ERR_UNSUPPORTED, "out_f32 with the fused l2norm backward is not implemented (normalise outside)");
   BwdHostArgs h;
@@ -615,7 +672,8 @@ static int backward_impl(const fcsa_problem* p, const fcsa_varlen* vl, const fcs
   h.inv_l = inv_l;
   h.out_f32 = p->out_f32 != 0;
   h.workspace = workspace;
-  h.zeroed = zeroed;
+  h.zeroed = deterministic ? nullptr : zeroed;
+  h.deterministic = deterministic;
   h.q_rnorm = q_rnorm;
   h.k_rnorm = k_rnorm;
   h.groups = groups;
@@ -644,7 +702,7 @@ int fcsa_backward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor
                   const fcsa_tensor* dv, void* workspace, size_t workspace_bytes, void* zeroed,
                   size_t zeroed_bytes, void* stream) {
   return backward_impl(p, nullptr, q, k, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed,
-                       zeroed_bytes, stream, nullptr, nullptr, 1);
+                       zeroed_bytes, stream, nullptr, nullptr, 1, false);
 }
 
 int fcsa_backward_bias(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
@@ -654,7 +712,7 @@ int fcsa_backward_bias(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_t
                        void* workspace, size_t workspace_bytes, void* zeroed, size_t zeroed_bytes, void* stream) {
   if (!bias) return fail(FCSA_ERR_INVALID, "attn_bias: null");
   return backward_impl(p, nullptr, q, k, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed,
-                       zeroed_bytes, stream, nullptr, nullptr, 1, bias, d_bias_acc, dsb, dsh);
+                       zeroed_bytes, stream, nullptr, nullptr, 1, false, bias, d_bias_acc, dsb, dsh);
 }
 
 int fcsa_forward_fused(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
@@ -690,7 +748,29 @@ int fcsa_backward_fused(const fcsa_problem* p, const fcsa_l2norm* n, const fcsa_
   if ((r = check_rows(false, p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, n->groups))) return r;
   if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
   return backward_impl(p, nullptr, &n->q_hat, &n->k_hat, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes,
-                       zeroed, zeroed_bytes, stream, n->q_rnorm, n->k_rnorm, n->groups);
+                       zeroed, zeroed_bytes, stream, n->q_rnorm, n->k_rnorm, n->groups, false);
+}
+
+size_t fcsa_backward_fused_deterministic_workspace_bytes(const fcsa_problem* p) {
+  if (check_problem(p)) return 0;
+  return bwd_deterministic_bytes(bwd_layout(p, nullptr));
+}
+
+int fcsa_backward_fused_deterministic(const fcsa_problem* p, const fcsa_l2norm* n, const fcsa_tensor* v,
+                                      const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
+                                      const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv,
+                                      void* workspace, size_t workspace_bytes, void* stream) {
+  if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
+  int r;
+  if ((r = check_problem(p))) return r;
+  const bool fused = n->groups != 0;
+  if (fused) {
+    if ((r = check_rows(false, p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, n->groups))) return r;
+    if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
+  }
+  return backward_impl(p, nullptr, &n->q_hat, &n->k_hat, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes,
+                       nullptr, 0, stream, fused ? n->q_rnorm : nullptr, fused ? n->k_rnorm : nullptr,
+                       fused ? n->groups : 1, true);
 }
 
 int fcsa_f32_cast(int32_t dtype, int32_t batch, int32_t heads, int32_t rows, int32_t head_dim, int32_t groups,
@@ -846,10 +926,12 @@ size_t fcsa_backward_fused_varlen_zeroed_bytes(const fcsa_problem* p, const fcsa
   return bwd_layout(p, vl).ztotal;
 }
 
-int fcsa_backward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_l2norm* n,
-                               const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
-                               const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv, void* workspace,
-                               size_t workspace_bytes, void* zeroed, size_t zeroed_bytes, void* stream) {
+// fcsa_backward_fused_varlen and its deterministic twin (zeroed unused)
+static int backward_varlen_impl(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_l2norm* n,
+                                const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
+                                const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv, void* workspace,
+                                size_t workspace_bytes, void* zeroed, size_t zeroed_bytes, void* stream,
+                                bool deterministic) {
   int r;
   if ((r = check_varlen(p, vl))) return r;
   if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
@@ -860,7 +942,7 @@ int fcsa_backward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, con
   }
   if ((r = backward_impl(p, vl, &n->q_hat, &n->k_hat, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed,
                          zeroed_bytes, stream, fused ? n->q_rnorm : nullptr, fused ? n->k_rnorm : nullptr,
-                         fused ? n->groups : 1)))
+                         fused ? n->groups : 1, deterministic)))
     return r;
   // zero gradients in the rows outside every sequence
   fcsa::TailArgs ta = {};
@@ -868,6 +950,28 @@ int fcsa_backward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, con
   ta.t[1] = {dk->ptr, dk->sh, dk->sn, p->kv_heads, vl->total_k, vl->cu_seqlens_k};
   ta.t[2] = {dv->ptr, dv->sh, dv->sn, p->kv_heads, vl->total_k, vl->cu_seqlens_k};
   return launch_varlen_tail(p, ta, 3, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int fcsa_backward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_l2norm* n,
+                               const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
+                               const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv, void* workspace,
+                               size_t workspace_bytes, void* zeroed, size_t zeroed_bytes, void* stream) {
+  return backward_varlen_impl(p, vl, n, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed, zeroed_bytes,
+                              stream, false);
+}
+
+size_t fcsa_backward_fused_deterministic_varlen_workspace_bytes(const fcsa_problem* p, const fcsa_varlen* vl) {
+  if (check_varlen(p, vl)) return 0;
+  return bwd_deterministic_bytes(bwd_layout(p, vl));
+}
+
+int fcsa_backward_fused_deterministic_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_l2norm* n,
+                                             const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o,
+                                             const float* inv_l, const fcsa_tensor* dq, const fcsa_tensor* dk,
+                                             const fcsa_tensor* dv, void* workspace, size_t workspace_bytes,
+                                             void* stream) {
+  return backward_varlen_impl(p, vl, n, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, nullptr, 0, stream,
+                              true);
 }
 
 }  // extern "C"

@@ -167,7 +167,10 @@ inline int varlen_tiles(int B, long long total_q) { return (int)(total_q / 64 + 
 // Query rows of one forward CTA: three consumer warpgroups of 64 rows for D = 64, two for D = 128 (FwdCfg).
 constexpr int fwd_block_rows(int D) { return D == 64 ? 192 : 128; }
 
-// Blocks of `rows` rows that cover n rows: the forward's query blocks, decode's row blocks.
+// Query rows of one CTA of the deterministic backward's dQ kernel: two consumer warpgroups of 64 rows.
+constexpr int dq_block_rows = 128;
+
+// Blocks of `rows` rows that cover n rows: the forward's query blocks, the dQ kernel's, decode's row blocks.
 inline int row_blocks(int n, int rows) { return (n + rows - 1) / rows; }
 
 // Decode splits per work item: 1 when the items alone fill the SMs, otherwise the fewest that do, at most one per key

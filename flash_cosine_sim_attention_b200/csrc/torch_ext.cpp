@@ -325,6 +325,8 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> forward_ex(
 //   groups > 0 (with q_rnorm, k_rnorm): q, k are the NORMALISED tensors forward_ex returned and dq, dk
 //                       are gradients w.r.t. the raw ones (l2norm backward fused)
 //   bias_prepared + bias_grad: d_bias accumulated in fp32, returned in `bias_dtype_like`'s dtype / shape
+//   deterministic     : the backward without atomics (fcsa_backward_fused_deterministic): bitwise reproducible
+//                       dq, dk, dv; scratch only, no zeroed workspace; no bias
 // returns (dq, dk, dv, d_bias or undefined)
 // ------------------------------------------------------------------------------------------------
 std::tuple<Tensor, Tensor, Tensor, Tensor> backward_ex(
@@ -332,7 +334,7 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> backward_ex(
     const Tensor& v_in, const optional<Tensor>& q_rnorm, const optional<Tensor>& k_rnorm,
     const optional<Tensor>& mask, const optional<Tensor>& bias_prepared, bool bias_batch_dim,
     const optional<Tensor>& bias_amax, bool bias_grad, const optional<Tensor>& bias_like, double scale, double shift,
-    bool causal, int64_t groups, bool out_f32, int64_t window) {
+    bool causal, int64_t groups, bool out_f32, int64_t window, bool deterministic) {
   const Shapes sh(q_in, k_in, v_in);
   const c10::cuda::CUDAGuard guard(q_in.device());
   const Tensor q = tma_ready(q_in), k = tma_ready(k_in), v = tma_ready(v_in), o = tma_ready(o_in),
@@ -348,15 +350,31 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> backward_ex(
   Tensor dk = at::empty(k.sizes(), gopt);
   Tensor dv = at::empty(v.sizes(), gopt);
   cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
-  const Workspaces ws = backward_workspaces(p, q, stream);
   const fcsa_tensor tq = view4(q), tk = view4(k), tv = view4(v), to = view4(o), tdo = view4(d_o), tdq = view4(dq),
                     tdk = view4(dk), tdv = view4(dv);
-  void* wsp = ws.scratch.data_ptr();
-  void* zsp = ws.zeroed.data_ptr();
-  const size_t wsn = (size_t)ws.scratch.numel(), zsn = (size_t)ws.zeroed.numel();
   const bool has_bias = bias_prepared.has_value() && bias_prepared->defined();
   const bool fused = q_rnorm.has_value() && q_rnorm->defined();
   Tensor db;
+  if (deterministic) {
+    TORCH_CHECK(!has_bias, "backward_ex: the deterministic backward takes no attn_bias");
+    const Tensor scratch =
+        workspaces_of_size(fcsa_backward_fused_deterministic_workspace_bytes(&p), 0, q, stream, false).scratch;
+    fcsa_l2norm n;
+    n.groups = fused ? (int32_t)groups : 0;
+    n.q_hat = tq; n.k_hat = tk;
+    n.q_rnorm = n.k_rnorm = nullptr;
+    if (fused) {
+      TORCH_CHECK(k_rnorm.has_value() && k_rnorm->defined() && groups > 0, "backward_ex: bad fused-l2norm arguments");
+      n.q_rnorm = q_rnorm->data_ptr<float>(); n.k_rnorm = k_rnorm->data_ptr<float>();
+    }
+    FCSA_CHECK(fcsa_backward_fused_deterministic(&p, &n, &tv, &to, &tdo, inv_l.data_ptr<float>(), &tdq, &tdk, &tdv,
+                                                 scratch.data_ptr(), (size_t)scratch.numel(), stream));
+    return {dq, dk, dv, db};
+  }
+  const Workspaces ws = backward_workspaces(p, q, stream);
+  void* wsp = ws.scratch.data_ptr();
+  void* zsp = ws.zeroed.data_ptr();
+  const size_t wsn = (size_t)ws.scratch.numel(), zsn = (size_t)ws.zeroed.numel();
   if (fused) {
     TORCH_CHECK(!has_bias && k_rnorm.has_value() && k_rnorm->defined() && groups > 0, "backward_ex: bad fused-l2norm arguments");
     fcsa_l2norm n;
@@ -414,7 +432,8 @@ std::tuple<Tensor, Tensor, Tensor, optional<Tensor>> backward(
   optional<Tensor> bias_prepared;
   if (has_bias) bias_prepared = prep_bias(*attn_bias, sh, q.scalar_type(), attn_bias_batch_dim);
   auto r = backward_ex(d_out, o, l, q, k, v, c10::nullopt, c10::nullopt, mask, bias_prepared, attn_bias_batch_dim,
-                       c10::nullopt, has_bias && attn_bias->requires_grad(), attn_bias, scale, scale, causal, 0, false, 0);
+                       c10::nullopt, has_bias && attn_bias->requires_grad(), attn_bias, scale, scale, causal, 0, false, 0,
+                       false);
   optional<Tensor> db;
   if (std::get<3>(r).defined()) db = std::get<3>(r);
   return {std::get<0>(r), std::get<1>(r), std::get<2>(r), db};
@@ -560,12 +579,13 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> forward_varlen(
   return {o, inv_l, qn, kn, rq, rk};
 }
 
-// gradients of forward_varlen w.r.t. the raw q, k (groups > 0: q, k are the normalised tensors it returned) and v
+// gradients of forward_varlen w.r.t. the raw q, k (groups > 0: q, k are the normalised tensors it returned) and v;
+// deterministic: fcsa_backward_fused_deterministic_varlen (scratch only)
 std::tuple<Tensor, Tensor, Tensor> backward_varlen(
     const Tensor& d_out, const Tensor& o_in, const Tensor& inv_l, const Tensor& q_in, const Tensor& k_in,
     const Tensor& v_in, const optional<Tensor>& q_rnorm, const optional<Tensor>& k_rnorm, const Tensor& cu_q,
     const Tensor& cu_k, int64_t max_q, int64_t max_k, double scale, double shift, bool causal, int64_t groups,
-    int64_t window) {
+    int64_t window, bool deterministic) {
   const c10::cuda::CUDAGuard guard(q_in.device());
   const Tensor q = tma_ready(q_in), k = tma_ready(k_in), v = tma_ready(v_in), o = tma_ready(o_in),
                d_o = tma_ready(d_out);
@@ -579,8 +599,6 @@ std::tuple<Tensor, Tensor, Tensor> backward_varlen(
   Tensor dk = at::empty(k.sizes(), k.options());
   Tensor dv = at::empty(v.sizes(), v.options());
   cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
-  const Workspaces ws = workspaces_of_size(fcsa_backward_fused_varlen_workspace_bytes(&vr.p, &vr.vl),
-                                           fcsa_backward_fused_varlen_zeroed_bytes(&vr.p, &vr.vl), q, stream);
   fcsa_l2norm n;
   n.groups = (int32_t)groups;
   n.q_hat = view_packed(q); n.k_hat = view_packed(k);
@@ -592,6 +610,16 @@ std::tuple<Tensor, Tensor, Tensor> backward_varlen(
   }
   const fcsa_tensor tv = view_packed(v), to = view_packed(o), tdo = view_packed(d_o), tdq = view_packed(dq),
                     tdk = view_packed(dk), tdv = view_packed(dv);
+  if (deterministic) {
+    const Tensor scratch = workspaces_of_size(fcsa_backward_fused_deterministic_varlen_workspace_bytes(&vr.p, &vr.vl), 0,
+                                              q, stream, false).scratch;
+    FCSA_CHECK(fcsa_backward_fused_deterministic_varlen(&vr.p, &vr.vl, &n, &tv, &to, &tdo, inv_l.data_ptr<float>(),
+                                                        &tdq, &tdk, &tdv, scratch.data_ptr(),
+                                                        (size_t)scratch.numel(), stream));
+    return {dq, dk, dv};
+  }
+  const Workspaces ws = workspaces_of_size(fcsa_backward_fused_varlen_workspace_bytes(&vr.p, &vr.vl),
+                                           fcsa_backward_fused_varlen_zeroed_bytes(&vr.p, &vr.vl), q, stream);
   FCSA_CHECK(fcsa_backward_fused_varlen(&vr.p, &vr.vl, &n, &tv, &to, &tdo, inv_l.data_ptr<float>(), &tdq, &tdk, &tdv,
                                         ws.scratch.data_ptr(), (size_t)ws.scratch.numel(), ws.zeroed.data_ptr(),
                                         (size_t)ws.zeroed.numel(), stream));
@@ -628,7 +656,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("backward", &backward, "Flash Cosine-Sim Attention Backward");
   m.def("debug", &debug, "Debug");
   namespace py = pybind11;
-  // (window: a trailing argument, default 0 = no window, after the positional ones every caller passes)
+  // (window, deterministic: trailing arguments, default 0 = no window / false, after the positional ones every caller
+  // passes)
   m.def("forward_ex", &forward_ex, "forward with explicit shift / fused l2norm / prepared bias", py::arg("q"),
         py::arg("k"), py::arg("v"), py::arg("mask"), py::arg("bias_prepared"), py::arg("bias_batch_dim"),
         py::arg("bias_amax"), py::arg("scale"), py::arg("shift"), py::arg("causal"), py::arg("l2norm_groups"),
@@ -637,7 +666,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("q"), py::arg("k"), py::arg("v"), py::arg("q_rnorm"), py::arg("k_rnorm"), py::arg("mask"),
         py::arg("bias_prepared"), py::arg("bias_batch_dim"), py::arg("bias_amax"), py::arg("bias_grad"),
         py::arg("bias_like"), py::arg("scale"), py::arg("shift"), py::arg("causal"), py::arg("groups"),
-        py::arg("out_f32"), py::arg("window") = 0);
+        py::arg("out_f32"), py::arg("window") = 0, py::arg("deterministic") = false);
   m.def("prepare_bias", &prepare_bias, "attn_bias -> padded, aligned tensor in the problem dtype");
   m.def("f32_cast", &f32_cast, "float32 -> (l2norm +) scaled cast to the 16-bit operand dtype");
   m.def("f32_cast_backward", &f32_cast_backward, "backward of f32_cast: float32 gradient w.r.t. the float32 input");
@@ -650,7 +679,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("backward_varlen", &backward_varlen, "backward of forward_varlen", py::arg("d_out"), py::arg("o"),
         py::arg("inv_l"), py::arg("q"), py::arg("k"), py::arg("v"), py::arg("q_rnorm"), py::arg("k_rnorm"),
         py::arg("cu_q"), py::arg("cu_k"), py::arg("max_q"), py::arg("max_k"), py::arg("scale"), py::arg("shift"),
-        py::arg("causal"), py::arg("groups"), py::arg("window") = 0);
+        py::arg("causal"), py::arg("groups"), py::arg("window") = 0, py::arg("deterministic") = false);
   m.def("decode", &decode, "new queries against a key/value cache, appending k / v at cache_seqlens", py::arg("q"),
         py::arg("k_cache"), py::arg("v_cache"), py::arg("cache_seqlens"), py::arg("k"), py::arg("v"), py::arg("scale"),
         py::arg("shift"), py::arg("causal"), py::arg("groups"), py::arg("window") = 0);

@@ -292,7 +292,7 @@ class _FusedCosineSimAttention(Function):
     """One autograd node for l2norm(q), l2norm(k) -> attention, all in CUDA kernels."""
 
     @staticmethod
-    def forward(ctx, q, k, v, mask, scale, causal, groups, l2norm_qk, shift_groups=0, window=0):
+    def forward(ctx, q, k, v, mask, scale, causal, groups, l2norm_qk, shift_groups=0, window=0, deterministic=False):
         ext = _ext()
         # shift_groups > 0: q, k arrive already normalised over that many groups (padded head dims)
         shift = (_choose_shift(q.dtype, scale, shift_groups, True) if shift_groups > 0
@@ -304,16 +304,17 @@ class _FusedCosineSimAttention(Function):
             if not l2norm_qk:
                 qn, kn = q, k
             ctx.save_for_backward(o, inv_l, qn, kn, v, mask, rq, rk)
-            ctx.params = (scale, shift, causal, groups, l2norm_qk, window)
+            ctx.params = (scale, shift, causal, groups, l2norm_qk, window, deterministic)
         return o
 
     @staticmethod
     def backward(ctx, do):
         o, inv_l, qn, kn, v, mask, rq, rk = ctx.saved_tensors
-        scale, shift, causal, groups, l2norm_qk, window = ctx.params
+        scale, shift, causal, groups, l2norm_qk, window, deterministic = ctx.params
         dq, dk, dv, _ = _ext().backward_ex(do, o, inv_l, qn, kn, v, rq, rk, mask, None, False, None, False, None,
-                                           scale, shift, causal, groups if l2norm_qk else 0, False, window)
-        return dq, dk, dv, None, None, None, None, None, None, None
+                                           scale, shift, causal, groups if l2norm_qk else 0, False, window,
+                                           deterministic)
+        return dq, dk, dv, None, None, None, None, None, None, None, None
 
 
 class _L2Norm(Function):
@@ -349,6 +350,17 @@ def _check_window(window, attn_bias, name):
     if exists(attn_bias):
         raise NotImplementedError(f"{name}: window with attn_bias is not supported (the bias kernels take no window)")
     return min(window, 2 ** 31 - 1)
+
+
+def _check_deterministic(deterministic, attn_bias, name):
+    """The `deterministic` keyword of the training entry points: a bool.  Rejected before any launch: anything else,
+    and True together with attn_bias (its gradient is summed with atomics)."""
+    if not isinstance(deterministic, bool):
+        raise TypeError(f"{name}: deterministic must be a bool, got {deterministic!r}")
+    if deterministic and exists(attn_bias):
+        raise NotImplementedError(f"{name}: deterministic=True with attn_bias is not supported (the bias gradient is "
+                                  "summed with atomics)")
+    return deterministic
 
 
 def _band(nq, nk, window, causal, device):
@@ -483,7 +495,7 @@ class _Float32OnHalfKernels(Function):
 
     @staticmethod
     def forward(ctx, q, k, v, mask, attn_bias, scale, causal, attn_bias_batch_dim, shift, half, use_amax, norm_groups,
-                window=0):
+                window=0, deterministic=False):
         ext = _ext()
         D = q.shape[-1]
         Dp = D if D in _KERNEL_HEAD_DIMS else (64 if D < 64 else 128)        # 16 / 32 / 96: zero-padded features
@@ -503,27 +515,28 @@ class _Float32OnHalfKernels(Function):
         if needs_grad:
             ctx.save_for_backward(o, inv_l, qh, kh, vh, mask, bias, amax, sv, rq, rk)
             ctx.params = (scale, shift, causal, batch_dim, D, exists(attn_bias) and ctx.needs_input_grad[4], norm_groups,
-                          window)
+                          window, deterministic)
         return o[..., :D] * sv
 
     @staticmethod
     def backward(ctx, g):
         o, inv_l, qh, kh, vh, mask, bias, amax, sv, rq, rk = ctx.saved_tensors
-        scale, shift, causal, batch_dim, D, bias_grad, norm_groups, window = ctx.params
+        scale, shift, causal, batch_dim, D, bias_grad, norm_groups, window, deterministic = ctx.params
         # o = o_kernel * sv, so d(o_kernel) = g * sv; it enters the kernels as fp16 scaled into [1, 2):
         # g * sv / sg with sg = pg * sv, pg = pow2 scale of g  ->  the cast pass computes g / pg
         pg = _pow2_scale(g, 1)
         gh, _ = _cast16(g, qh.dtype, 0, pg, True, qh.shape[-1])
         dq, dk, dv, db = _ext().backward_ex(gh, o, inv_l, qh, kh, vh, None, None, mask, bias, batch_dim, amax,
-                                            bias_grad, None, scale, shift, causal, 0, True, window)
+                                            bias_grad, None, scale, shift, causal, 0, True, window, deterministic)
         sg = pg * sv                                          # undo the gradient scale; dv also undoes v / sv
         dq = _uncast16(dq, qh, rq, norm_groups, sg, False, D)
         dk = _uncast16(dk, kh, rk, norm_groups, sg, False, D)
         dv = _uncast16(dv, None, None, 0, pg, False, D)
-        return dq, dk, dv, None, (db * sg if bias_grad else None), None, None, None, None, None, None, None, None
+        return dq, dk, dv, None, (db * sg if bias_grad else None), None, None, None, None, None, None, None, None, None
 
 
-def _float32_on_half_kernels(q, k, v, mask, attn_bias, scale, groups, causal, l2norm_qk, attn_bias_batch_dim, window=0):
+def _float32_on_half_kernels(q, k, v, mask, attn_bias, scale, groups, causal, l2norm_qk, attn_bias_batch_dim, window=0,
+                             deterministic=False):
     D = q.shape[-1]
     assert D % groups == 0, "groups must divide the head dim"
     # fp16 (11-bit significand, like tf32) whenever its exponent range holds exp(scale * q.k); bf16 (8 bits, fp32's
@@ -543,7 +556,7 @@ def _float32_on_half_kernels(q, k, v, mask, attn_bias, scale, groups, causal, l2
     shift = _choose_shift(h, scale, groups if l2norm_qk else 1, l2norm_qk)
     return _Float32OnHalfKernels.apply(q, k, v, mask, attn_bias, float(scale), bool(causal), bool(attn_bias_batch_dim),
                                        float(shift), h, bool(l2norm_qk and h == torch.float16), int(norm_groups),
-                                       int(window))
+                                       int(window), deterministic)
 
 
 _warned = set()
@@ -556,7 +569,8 @@ def _warn_once(key, msg):
 
 
 def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, groups=1, causal=False,
-                               l2norm_qk=True, attn_bias_batch_dim=False, l2norm_groups=None, window=None):
+                               l2norm_qk=True, attn_bias_batch_dim=False, l2norm_groups=None, window=None,
+                               deterministic=False):
     """Fused cosine-similarity attention (reference py:308-334, same arguments and meaning;
     `l2norm_groups` is accepted as an alias of `groups`).
 
@@ -564,6 +578,10 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
     alignment of causal masking) and d = i + off - j, key j is visible to query i iff 0 <= d < W with causal=True (the
     query itself and the W - 1 keys before it) and iff |d| < W otherwise, on top of `mask`.  The kernels skip the key
     tiles outside the band, so a causal pass costs O(n * W).  Rows that see no key give 0.  Not with attn_bias.
+
+    deterministic: True runs the backward without atomics (a dK / dV kernel and a dQ kernel that sum in a fixed
+    order), so dq, dk and dv are bitwise the same from run to run and a batch element's do not depend on the rest of
+    the batch.  Slower than the default backward; the forward is the same.  Not with attn_bias.
 
     Every supported input runs the hand-written sm_90a kernels: float16 / bfloat16 natively, float32 at
     tf32-class operand precision on the fp16 kernels (see _float32_on_half_kernels), head dims 64 and 128
@@ -573,6 +591,7 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
         groups = l2norm_groups
     assert not (causal and exists(mask)), "mask should not be supplied if causality is needed"
     window = _check_window(window, attn_bias, "flash_cosine_sim_attention")
+    deterministic = _check_deterministic(deterministic, attn_bias, "flash_cosine_sim_attention")
     if not q.is_cuda:
         raise RuntimeError(
             "flash_cosine_sim_attention: CUDA tensors required - this build has no CPU path "
@@ -589,7 +608,7 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
         raise RuntimeError("flash_cosine_sim_attention: attn_bias must be a CUDA tensor")
     if q.dtype == torch.float32:
         return _float32_on_half_kernels(q, k, v, mask, attn_bias, scale, groups, causal, l2norm_qk, attn_bias_batch_dim,
-                                        window)
+                                        window, deterministic)
     if q.dtype not in _KERNEL_DTYPES:
         raise TypeError(f"flash_cosine_sim_attention: dtype {q.dtype} is not supported (float16, bfloat16, float32)")
     _warn_fp16_overflow(q.dtype, scale, groups, l2norm_qk)
@@ -610,7 +629,7 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
                                               bool(attn_bias_batch_dim), float(shift), amax)
         else:
             o = _FusedCosineSimAttention.apply(pad(q), pad(k), pad(v), mask, float(scale), bool(causal), 1, False,
-                                               int(groups) if l2norm_qk else 0, window)
+                                               int(groups) if l2norm_qk else 0, window, deterministic)
         return o[..., :D]
     if exists(attn_bias):
         # additive bias: l2norm kernels (with their own backward), then the BIAS instantiations of the
@@ -628,7 +647,7 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
     gs = q.shape[-1] // groups
     assert (gs & (gs - 1)) == 0, "groups must divide the head dim into power-of-two chunks"
     return _FusedCosineSimAttention.apply(q, k, v, mask, float(scale), bool(causal), int(groups), bool(l2norm_qk), 0,
-                                          window)
+                                          window, deterministic)
 
 
 def _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias):
@@ -715,7 +734,7 @@ class _FusedVarlenAttention(Function):
     """One autograd node for packed sequences: l2norm(q), l2norm(k) -> attention, all in CUDA kernels."""
 
     @staticmethod
-    def forward(ctx, q, k, v, cu_q, cu_k, max_q, max_k, scale, causal, groups, l2norm_qk, window=0):
+    def forward(ctx, q, k, v, cu_q, cu_k, max_q, max_k, scale, causal, groups, l2norm_qk, window=0, deterministic=False):
         shift = _choose_shift(q.dtype, scale, groups, l2norm_qk)
         g = groups if l2norm_qk else 0
         needs_grad = any(ctx.needs_input_grad[:3])
@@ -725,16 +744,16 @@ class _FusedVarlenAttention(Function):
             if not l2norm_qk:
                 qn, kn = q, k
             ctx.save_for_backward(o, inv_l, qn, kn, v, rq, rk, cu_q, cu_k)
-            ctx.params = (max_q, max_k, scale, shift, causal, g, window)
+            ctx.params = (max_q, max_k, scale, shift, causal, g, window, deterministic)
         return o
 
     @staticmethod
     def backward(ctx, do):
         o, inv_l, qn, kn, v, rq, rk, cu_q, cu_k = ctx.saved_tensors
-        max_q, max_k, scale, shift, causal, g, window = ctx.params
+        max_q, max_k, scale, shift, causal, g, window, deterministic = ctx.params
         dq, dk, dv = _ext().backward_varlen(do, o, inv_l, qn, kn, v, rq, rk, cu_q, cu_k, max_q, max_k, scale, shift,
-                                            causal, g, window)
-        return (dq, dk, dv) + (None,) * 9
+                                            causal, g, window, deterministic)
+        return (dq, dk, dv) + (None,) * 10
 
 
 class _EmptyVarlenAttention(Function):
@@ -798,7 +817,8 @@ def _check_varlen_args(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_se
 
 
 def flash_cosine_sim_attention_varlen(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale=8,
-                                      groups=1, causal=False, l2norm_qk=True, mask=None, attn_bias=None, window=None):
+                                      groups=1, causal=False, l2norm_qk=True, mask=None, attn_bias=None, window=None,
+                                      deterministic=False):
     """Cosine-sim attention over packed variable-length sequences (training: forward and backward).
 
     q: (total_q, heads, head_dim); k, v: (total_k, kv_heads, head_dim), kv_heads dividing heads (query head h reads kv
@@ -815,12 +835,15 @@ def flash_cosine_sim_attention_varlen(q, k, v, cu_seqlens_q, cu_seqlens_k, max_s
     [cu[-1], total), e.g. the unused end of a fixed-size packing buffer) give o = 0 and zero gradients.  Packed tensors
     with no query or no key rows give zeros (and zero gradients) without a kernel launch.  float16 / bfloat16 and head dims 64 and 128 only; no float32, mask or
     attn_bias.  window: sliding-window attention as in flash_cosine_sim_attention, with each sequence's own lengths.
+    deterministic: the backward of flash_cosine_sim_attention(deterministic=True); a sequence's gradients are then
+    also bitwise independent of the other sequences in the pack.
     Returns o (total_q, heads, head_dim)."""
     window = _check_window(window, attn_bias, "flash_cosine_sim_attention_varlen")
+    deterministic = _check_deterministic(deterministic, attn_bias, "flash_cosine_sim_attention_varlen")
     _check_varlen_args(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, groups, mask, attn_bias)
     _warn_fp16_overflow(q.dtype, scale, groups, l2norm_qk)
     if q.shape[0] == 0 or k.shape[0] == 0:
         return _EmptyVarlenAttention.apply(q, k, v)
     return _FusedVarlenAttention.apply(q, k, v, cu_seqlens_q, cu_seqlens_k, max(int(max_seqlen_q), 1),
                                        max(int(max_seqlen_k), 1), float(scale), bool(causal), int(groups),
-                                       bool(l2norm_qk), window)
+                                       bool(l2norm_qk), window, deterministic)

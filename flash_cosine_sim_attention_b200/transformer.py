@@ -127,13 +127,14 @@ class Attention(nn.Module):
         q = self.to_q(x).view(n, self.heads, -1)
         k, v = self.to_k(x).view(n, self.kv_heads, -1), self.to_v(x).view(n, self.kv_heads, -1)
         if self.use_cuda_kernel:
-            unsupported = sorted(set(self.kernel_kwargs) - {"l2norm_qk"})
+            unsupported = sorted(set(self.kernel_kwargs) - {"l2norm_qk", "deterministic"})
             if unsupported:
                 raise NotImplementedError(f"packed documents do not support the attention keywords {unsupported}")
             m = n if max_seqlen is None else int(max_seqlen)
             o = flash_cosine_sim_attention_varlen(q, k, v, cu_seqlens, cu_seqlens, m, m, scale=self.scale,
                                                   groups=self.l2norm_groups, causal=True,
-                                                  l2norm_qk=self.kernel_kwargs.get("l2norm_qk", True), window=self.window)
+                                                  l2norm_qk=self.kernel_kwargs.get("l2norm_qk", True), window=self.window,
+                                                  deterministic=self.kernel_kwargs.get("deterministic", False))
         else:
             # the reference: one call per document (reads the boundaries on the host)
             bounds = cu_seqlens.tolist()
@@ -159,8 +160,9 @@ class Attention(nn.Module):
         if L + n > cache.capacity:
             raise ValueError(f"key/value cache full: {L} + {n} tokens exceed its capacity {cache.capacity}")
         # the uncached CUDA path hands these keywords to flash_cosine_sim_attention; with a cache only l2norm_qk has a
-        # meaning, and a silently dropped one would make cached and uncached outputs differ
-        unsupported = sorted(set(self.kernel_kwargs) - {"l2norm_qk"}) if self.use_cuda_kernel else []
+        # meaning, and a silently dropped one would make cached and uncached outputs differ.  `deterministic` only
+        # concerns the backward, and the cache is inference only: it changes no output here.
+        unsupported = sorted(set(self.kernel_kwargs) - {"l2norm_qk", "deterministic"}) if self.use_cuda_kernel else []
         if unsupported:
             raise NotImplementedError(f"the key/value cache does not support the attention keywords {unsupported}")
         if self.use_cuda_kernel and k.dtype == torch.float32:

@@ -134,7 +134,9 @@ int fcsa_zeroed_init(void* zeroed, size_t bytes, void* stream);
  * Reproducibility: o, dk, dv are bitwise reproducible from run to run when kv_heads == heads, and for
  * grouped-query problems whose backward grid keeps each group in one CTA (enough batch * kv_heads *
  * key tiles to fill the device, no bias).  Otherwise dk/dv are summed over CTAs with fp32 atomics and
- * may differ in the last bits between runs, like dq always may.
+ * may differ in the last bits between runs, like dq always may.  fcsa_backward_fused_deterministic and
+ * fcsa_backward_fused_deterministic_varlen (below) have no such reduction: dq, dk, dv are bitwise
+ * reproducible for every problem they take.
  */
 int fcsa_backward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
                   const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o,
@@ -189,6 +191,26 @@ int fcsa_backward_fused(const fcsa_problem* p, const fcsa_l2norm* n, const fcsa_
                         const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv,
                         void* workspace, size_t workspace_bytes, void* zeroed, size_t zeroed_bytes,
                         void* stream);
+
+/* ---- deterministic backward ------------------------------------------------------------------------
+ * The gradients of fcsa_backward_fused without a floating-point reduction whose order depends on
+ * scheduling: dq, dk, dv are bitwise the same from run to run, and batch element b's are the same
+ * whatever the batch around it.  Three launches: the preprocess, a dK / dV kernel with one CTA per
+ * (key tile, batch, kv head) that keeps every query head of the group (no dk / dv accumulators), and a
+ * dQ kernel that sums each query block's key tiles in ascending order in registers (no dq accumulator).
+ * The rounding points are fcsa_backward's, so the results agree with it within its error bounds; dk, dv
+ * are bitwise fcsa_backward's wherever that keeps each group in one CTA.
+ *   n->groups == 0: q, k (n->q_hat, n->k_hat) are used as given and the rnorms are ignored; > 0: the
+ *                   l2norm backward is applied as in fcsa_backward_fused.
+ * Takes out_f32 (with groups == 0), window and key_mask as fcsa_backward does; no bias.  `workspace`:
+ * fcsa_backward_fused_deterministic_workspace_bytes(p) bytes of scratch (the per-row constants only),
+ * contents irrelevant on entry.  No zeroed workspace.
+ */
+size_t fcsa_backward_fused_deterministic_workspace_bytes(const fcsa_problem* p);
+int fcsa_backward_fused_deterministic(const fcsa_problem* p, const fcsa_l2norm* n, const fcsa_tensor* v,
+                                      const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
+                                      const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv,
+                                      void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- float32 front end ---------------------------------------------------------------------------
  * The reference dispatches Float in forward and backward (cu:1702-1703, 1832-1834).  Here float32 callers run the
@@ -247,7 +269,7 @@ int fcsa_backward_bias(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_t
  * or fcsa_backward (which = 1) records the cudaEvent_t `start` / `stop` on the launch stream
  * immediately before / after its dominant kernel (the wgmma attention kernel, not the
  * pre/post passes); which = 2, 3, 4 do the same for the l2norm(q,k) pass of fcsa_forward_fused, the
- * backward preprocess and the dq finish pass.  An event between two launches suspends their programmatic
+ * backward preprocess and the dq finish pass (the dQ kernel in the deterministic backward).  An event between two launches suspends their programmatic
  * dependent launch, so a hooked run is for attribution, not for the headline time.  Pass NULL, NULL to clear.  State is process-wide (autograd calls the
  * backward from its own thread), so use it from single-stream measurement code only.
  */
@@ -317,6 +339,14 @@ int fcsa_backward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, con
                                const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
                                const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv, void* workspace,
                                size_t workspace_bytes, void* zeroed, size_t zeroed_bytes, void* stream);
+/* The deterministic backward (see fcsa_backward_fused_deterministic) over packed sequences: a sequence's gradients are
+ * bitwise the same whatever the other sequences of the pack.  Scratch only, a pure function like the above. */
+size_t fcsa_backward_fused_deterministic_varlen_workspace_bytes(const fcsa_problem* p, const fcsa_varlen* vl);
+int fcsa_backward_fused_deterministic_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_l2norm* n,
+                                             const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o,
+                                             const float* inv_l, const fcsa_tensor* dq, const fcsa_tensor* dk,
+                                             const fcsa_tensor* dv, void* workspace, size_t workspace_bytes,
+                                             void* stream);
 
 #ifdef __cplusplus
 }
