@@ -10,14 +10,16 @@ so a stray write, or a NaN value row leaking into P V, shows up.
 The split count (key ranges per work item) is chosen on the host from the SM count; tests that target one side of
 the rule compute it with the library's own rule (tile_ranges.decode_split) and check it through the number of
 launches: append pass + decode kernel, + the combine kernel when it splits."""
+import functools
 import math
 
 import pytest
 import torch
 
 from elementwise_bounds import FMT, attention_bounds, check_bound, kernel_shift
-from tile_ranges import decode_split
+from tile_ranges import decode_split, decode_window_keys
 from test_gpu_parity import TOL_OUT, fcsa, record, rel_err  # noqa: F401
+from window_bounds import window_attention_bounds
 
 pytestmark = pytest.mark.gpu
 
@@ -28,8 +30,11 @@ def sm_count():
     return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
 
 
-def n_split_of(B, H, Hk, Nq, cap):
+def n_split_of(B, H, Hk, Nq, cap, window=None, causal=True):
+    """The split count of a decode call; with a window below Nq + cap, the keys the split rule sees are bounded by it."""
     G = H // Hk
+    if window is not None and window < Nq + cap:
+        cap = int(decode_window_keys(cap, window, causal)[0])
     return decode_split(B * Hk * math.ceil(G * Nq / 64), cap, sm_count())
 
 
@@ -47,8 +52,9 @@ def make_cache(B, Hk, cap, D, dtype, lens, g, l2norm_qk, groups, amp):
 
 
 def check_case(fcsa, dtype, D, H, Hk, Nq, lens, cap, n_new, causal=True, groups=1, l2norm_qk=True, scale=8,
-               seed=0, launches=None):
-    """One call; checks the append bitwise, the untouched rows, and o per batch element.  Returns o."""
+               seed=0, launches=None, window=None):
+    """One call; checks the append bitwise, the untouched rows, and o per batch element (against the windowed
+    reference of tests/window_bounds.py when `window` is set).  Returns o."""
     from flash_cosine_sim_attention_b200 import l2norm_tensors
     B = len(lens)
     g = torch.Generator().manual_seed(seed)
@@ -67,7 +73,7 @@ def check_case(fcsa, dtype, D, H, Hk, Nq, lens, cap, n_new, causal=True, groups=
     before = fcsa.debug()
     with torch.no_grad():
         o = fcsa.flash_cosine_sim_attention_with_kv_cache(q, kc, vc, seqlens, k, v, scale=scale, groups=groups,
-                                                          causal=causal, l2norm_qk=l2norm_qk)
+                                                          causal=causal, l2norm_qk=l2norm_qk, window=window)
     torch.cuda.synchronize()
     if launches is not None:
         assert fcsa.debug() - before == launches
@@ -92,8 +98,9 @@ def check_case(fcsa, dtype, D, H, Hk, Nq, lens, cap, n_new, causal=True, groups=
         if T == 0:
             assert int(o[b].count_nonzero()) == 0
             continue
-        ref, bound = attention_bounds(qh[b:b + 1], kc[b:b + 1, :, :T], vc[b:b + 1, :, :T], scale=scale, causal=causal,
-                                      l2norm_qk=False, fmt=fmt, shift=shift, device="cuda")
+        bounds = attention_bounds if window is None else functools.partial(window_attention_bounds, window=window)
+        ref, bound = bounds(qh[b:b + 1], kc[b:b + 1, :, :T], vc[b:b + 1, :, :T], scale=scale, causal=causal,
+                            l2norm_qk=False, fmt=fmt, shift=shift, device="cuda")
         r = ref["o"].cpu().numpy()
         e = rel_err(o[b:b + 1], r) if abs(r).max() > 0 else float(o[b].abs().max())
         record(dtype, "decode o", e, TOL_OUT[dtype])
@@ -104,13 +111,17 @@ def check_case(fcsa, dtype, D, H, Hk, Nq, lens, cap, n_new, causal=True, groups=
 
 
 # ---- the covering grid: every value of every axis with both dtypes and both head dims ---------------------------
-_BASE = dict(H=8, Hk=2, Nq=5, causal=True, groups=1, l2norm_qk=True, append=True)
+_BASE = dict(H=8, Hk=2, Nq=5, causal=True, groups=1, l2norm_qk=True, append=True, window=None)
 _VARIANTS = [dict()]
 _VARIANTS += [dict(H=h, Hk=hk) for h, hk in ((8, 8), (8, 1), (6, 3))]
 _VARIANTS += [dict(Nq=n) for n in (1, 2, 33, 130)]
 _VARIANTS += [dict(H=h, Hk=hk, Nq=64 // (h // hk) + d) for h, hk in ((8, 8), (8, 2), (8, 1), (6, 3)) for d in (-1, 1)]
 _VARIANTS += [dict(causal=False), dict(groups=8), dict(l2norm_qk=False), dict(append=False),
               dict(causal=False, append=False, Nq=1)]
+# sliding windows (640 = the capacity: the windowed kernel with a band that hides nothing), lengths around their edges
+_VARIANTS += [dict(window=w) for w in (1, 65, 200, 640)]
+_VARIANTS += [dict(window=65, causal=False), dict(window=200, Nq=33), dict(window=65, H=8, Hk=8),
+              dict(window=200, append=False), dict(window=200, causal=False, groups=8)]
 
 
 def _case_id(v):
@@ -125,9 +136,13 @@ def test_decode_grid(fcsa, variant, D, dtype):
     Nq = c["Nq"]
     n_new = Nq if c["append"] else 0
     cap = 640
+    W = c["window"]
     lens = [0, 131, 383, cap - n_new]
+    if W is not None:
+        # T_b = L_b + n_new at W - 1, W, W + 1 and 2 W: the band's first key at 0 and past it
+        lens += [min(max(t - n_new, 0), cap - n_new) for t in (W - 1, W, W + 1, 2 * W)]
     check_case(fcsa, dtype, D, c["H"], c["Hk"], Nq, lens, cap, n_new, causal=c["causal"], groups=c["groups"],
-               l2norm_qk=c["l2norm_qk"], seed=_VARIANTS.index(variant) + D)
+               l2norm_qk=c["l2norm_qk"], seed=_VARIANTS.index(variant) + D, window=W)
 
 
 # ---- lengths in one call ---------------------------------------------------------------------------------------
@@ -163,6 +178,19 @@ def test_split_rule_sides(fcsa, side, D):
     assert (s == 1) == (side == "one"), s
     lens = [(977 * b) % 1023 for b in range(B)]
     check_case(fcsa, torch.bfloat16, D, H, Hk, Nq, lens, 1024, 1, seed=B + D, launches=2 if s == 1 else 3)
+
+
+@pytest.mark.parametrize("side", ["split", "one"])
+@pytest.mark.parametrize("D", [64, 128])
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
+def test_window_split_rule_sides(fcsa, side, D, dtype):
+    """The windowed decode kernel with and without the combine kernel; the split rule bounds the keys by the window."""
+    H, Hk, Nq, cap, window = 8, 8, 1, 1024, 200
+    B = 2 if side == "split" else math.ceil(sm_count() / Hk)
+    s = n_split_of(B, H, Hk, Nq, cap, window)
+    assert (s == 1) == (side == "one"), s
+    lens = [(window - 2 + 37 * b) % (cap - 1) for b in range(B)]
+    check_case(fcsa, dtype, D, H, Hk, Nq, lens, cap, 1, seed=B + D, launches=2 if s == 1 else 3, window=window)
 
 
 @pytest.mark.parametrize("D", [64, 128])

@@ -152,16 +152,29 @@ def test_key_mask(fcsa, D):
     default_agrees(fcsa, got, q, k, v, do, mask=mask.cuda())
 
 
-@pytest.mark.parametrize("window", [1, 65, 200])
-@pytest.mark.parametrize("causal", [False, True], ids=["full", "causal"])
-@pytest.mark.parametrize("D", [64, 128])
-def test_window(fcsa, window, causal, D):
-    dtype = torch.bfloat16
-    q, k, v, do = make(1, 4, 2, 700, 300, D, dtype, seed=window + D)
+def window_case(fcsa, dtype, heads, kv_heads, window, causal, D):
+    q, k, v, do = make(1, heads, kv_heads, 700, 300, D, dtype, seed=window + D)
     got, launched = repeated(fcsa, q, k, v, do, causal=causal, window=window)
     assert launched == 3, launched
     bounded(dtype, got, q, k, v, do, window=window, causal=causal)
     default_agrees(fcsa, got, q, k, v, do, causal=causal, window=window)
+
+
+@pytest.mark.parametrize("window", [1, 65, 200])
+@pytest.mark.parametrize("causal", [False, True], ids=["full", "causal"])
+@pytest.mark.parametrize("D", [64, 128])
+def test_window(fcsa, window, causal, D):
+    window_case(fcsa, torch.bfloat16, 4, 2, window, causal, D)
+
+
+# the other dtype and MHA (one query head per CTA: no head loop in the dK / dV kernel)
+@pytest.mark.parametrize("window", [1, 65, 200])
+@pytest.mark.parametrize("causal", [False, True], ids=["full", "causal"])
+@pytest.mark.parametrize("D", [64, 128])
+@pytest.mark.parametrize("dtype,heads,kv_heads", [(torch.float16, 4, 4), (torch.float16, 4, 2),
+                                                  (torch.bfloat16, 4, 4)], ids=["f16-4:4", "f16-4:2", "bf16-4:4"])
+def test_window_dtypes_and_heads(fcsa, dtype, heads, kv_heads, window, causal, D):
+    window_case(fcsa, dtype, heads, kv_heads, window, causal, D)
 
 
 @pytest.mark.parametrize("opts", [dict(groups=1), dict(groups=8, scale=1), dict(l2norm_qk=False, scale=1)],
@@ -175,17 +188,20 @@ def test_l2norm_options(fcsa, opts, D):
 
 
 # ---- 5. float32 and zero-padded head dims -----------------------------------------------------------------------------
-@pytest.mark.parametrize("dtype,D", [(torch.float32, 32), (torch.float32, 64), (torch.float32, 96),
-                                     (torch.bfloat16, 32), (torch.bfloat16, 96)],
-                         ids=["f32-32", "f32-64", "f32-96", "bf16-32", "bf16-96"])
-def test_other_dtypes_and_head_dims(fcsa, dtype, D):
+@pytest.mark.parametrize("dtype,D,window", [(torch.float32, 32, None), (torch.float32, 64, None),
+                                            (torch.float32, 96, None), (torch.bfloat16, 32, None),
+                                            (torch.bfloat16, 96, None), (torch.float32, 64, 65)],
+                         ids=["f32-32", "f32-64", "f32-96", "bf16-32", "bf16-96", "f32-64-window65"])
+def test_other_dtypes_and_head_dims(fcsa, dtype, D, window):
     q, k, v, do = make(1, 4, 2, 300, 300, D, dtype, seed=29 + D)
-    got, _ = repeated(fcsa, q, k, v, do, causal=True)
+    kw = dict(causal=True) if window is None else dict(causal=True, window=window)
+    got, _ = repeated(fcsa, q, k, v, do, **kw)
     if dtype == torch.float32:
-        judge(dtype, {n: t.cuda() for n, t in got.items()}, *(t.cuda() for t in (q, k, v, do)), causal=True)
+        bounds = attention_bounds if window is None else window_attention_bounds
+        judge(dtype, {n: t.cuda() for n, t in got.items()}, *(t.cuda() for t in (q, k, v, do)), bounds=bounds, **kw)
     else:
-        bounded(dtype, got, q, k, v, do, causal=True)
-    default_agrees(fcsa, got, q, k, v, do, causal=True)
+        bounded(dtype, got, q, k, v, do, **kw)
+    default_agrees(fcsa, got, q, k, v, do, **kw)
 
 
 # ---- 6. packed sequences ------------------------------------------------------------------------------------------------
@@ -201,24 +217,21 @@ def varlen_repeated(fcsa, q, k, v, do, cu, m, **kw):
     return first
 
 
-@pytest.mark.parametrize("heads,kv_heads", [(4, 4), (4, 2)])
-@pytest.mark.parametrize("D", [64, 128])
-@pytest.mark.parametrize("causal", [False, True], ids=["full", "causal"])
-def test_varlen(fcsa, heads, kv_heads, D, causal):
-    dtype = torch.bfloat16
+def varlen_case(fcsa, dtype, heads, kv_heads, D, causal, window=None):
     ls = SKEWED
     q, k, v, do = make_packed(ls, ls, heads, kv_heads, D, dtype, seed=31 + D + kv_heads)
     cu = cu_of(ls)
-    *got, launched = varlen_repeated(fcsa, q, k, v, do, cu, max(ls), causal=causal)
+    kw = dict(causal=causal) if window is None else dict(causal=causal, window=window)
+    *got, launched = varlen_repeated(fcsa, q, k, v, do, cu, max(ls), **kw)
     assert launched == 4, launched            # preprocess, dK / dV, dQ, the rows outside every sequence
-    seq_check(dtype, got, q, k, v, do, ls, ls, causal=causal)
+    seq_check(dtype, got, q, k, v, do, ls, ls, **kw)
     # the same sequences in another order: each sequence's gradients bitwise unchanged
     order = [3, 5, 0, 2, 1, 4]
     starts = cu.tolist()
     pick = lambda t: torch.cat([t[starts[i]:starts[i + 1]] for i in order])
     ls2 = [ls[i] for i in order]
     cu2 = cu_of(ls2)
-    got2 = varlen_repeated(fcsa, *(pick(t) for t in (q, k, v, do)), cu2, max(ls), causal=causal)
+    got2 = varlen_repeated(fcsa, *(pick(t) for t in (q, k, v, do)), cu2, max(ls), **kw)
     starts2 = cu2.tolist()
     for j, i in enumerate(order):
         for n, a, b in zip(NAMES, got, got2[:4]):
@@ -229,9 +242,26 @@ def test_varlen(fcsa, heads, kv_heads, D, causal):
             if n == 0:
                 continue
             s = starts[i]
-            dense, _ = run(fcsa, *(per_seq(t, s, n) for t in (q, k, v, do)), causal=causal, deterministic=DET)
+            dense, _ = run(fcsa, *(per_seq(t, s, n) for t in (q, k, v, do)), deterministic=DET, **kw)
             for name, t in zip(NAMES, got):
                 assert torch.equal(per_seq(t, s, n), dense[name]), (i, name)
+
+
+@pytest.mark.parametrize("heads,kv_heads", [(4, 4), (4, 2)])
+@pytest.mark.parametrize("D", [64, 128])
+@pytest.mark.parametrize("causal", [False, True], ids=["full", "causal"])
+def test_varlen(fcsa, heads, kv_heads, D, causal):
+    varlen_case(fcsa, torch.bfloat16, heads, kv_heads, D, causal)
+
+
+# fp16, and a sliding window in both dtypes (the packed, windowed dK / dV and dQ kernels)
+@pytest.mark.parametrize("heads,kv_heads", [(4, 4), (4, 2)])
+@pytest.mark.parametrize("D", [64, 128])
+@pytest.mark.parametrize("causal", [False, True], ids=["full", "causal"])
+@pytest.mark.parametrize("dtype,window", [(torch.float16, None), (torch.float16, 65), (torch.bfloat16, 65)],
+                         ids=["f16", "f16-window65", "bf16-window65"])
+def test_varlen_dtypes_and_windows(fcsa, dtype, window, heads, kv_heads, D, causal):
+    varlen_case(fcsa, dtype, heads, kv_heads, D, causal, window)
 
 
 def test_varlen_rows_outside_sequences(fcsa):

@@ -5,6 +5,8 @@ sequence alone, with the relative tolerances of test_gpu_parity.py and the eleme
 dense op called on each sequence (o bitwise, and dk / dv bitwise where the backward keeps each group in one CTA);
 for isolation from the other sequences, slack in max_seqlen, the zeroed dq workspace after non-finite inputs, strided
 views, CUDA graph replay with new lengths, and the transformer's packed path."""
+import functools
+
 import pytest
 import torch
 
@@ -12,6 +14,7 @@ from elementwise_bounds import FMT, attention_bounds, check_bound, kernel_shift
 from test_gpu_gqa import sm_count
 from tile_ranges import group_split
 from test_gpu_parity import TOL_GRAD, TOL_OUT, fcsa, record, rel_err  # noqa: F401
+from window_bounds import window_attention_bounds
 
 pytestmark = pytest.mark.gpu
 
@@ -50,8 +53,9 @@ def per_seq(t, s, n):
     return t[s:s + n].transpose(0, 1).unsqueeze(0)
 
 
-def seq_check(dtype, got, q, k, v, do, lq, lk, only=None, **kw):
-    """Each sequence (or only sequence `only`) against the float64 reference on it alone."""
+def seq_check(dtype, got, q, k, v, do, lq, lk, only=None, window=None, **kw):
+    """Each sequence (or only sequence `only`) against the float64 reference on it alone (with a sliding window: the
+    windowed reference of tests/window_bounds.py)."""
     fmt = FMT[dtype]
     l2 = kw.get("l2norm_qk", True)
     shift = kernel_shift(fmt, kw.get("scale", 8), kw.get("groups", 1), l2)
@@ -64,9 +68,10 @@ def seq_check(dtype, got, q, k, v, do, lq, lk, only=None, **kw):
                 for t in (o[sq:sq + a], dq[sq:sq + a], dk[sk:sk + b], dv[sk:sk + b]):
                     assert (t == 0).all(), (i, a, b)
             else:
-                ref, bound = attention_bounds(per_seq(q, sq, a), per_seq(k, sk, b), per_seq(v, sk, b),
-                                              per_seq(do, sq, a), round_qk=fmt if l2 else None, fmt=fmt, shift=shift,
-                                              device="cuda", **kw)
+                bounds = attention_bounds if window is None else functools.partial(window_attention_bounds,
+                                                                                   window=window)
+                ref, bound = bounds(per_seq(q, sq, a), per_seq(k, sk, b), per_seq(v, sk, b), per_seq(do, sq, a),
+                                    round_qk=fmt if l2 else None, fmt=fmt, shift=shift, device="cuda", **kw)
                 for name, t, s0, n in (("o", o, sq, a), ("dq", dq, sq, a), ("dk", dk, sk, b), ("dv", dv, sk, b)):
                     got_t = per_seq(t, s0, n)
                     e = rel_err(got_t, ref[name].cpu().numpy())

@@ -5,7 +5,8 @@ Covering grid: windows {1, 63, 64, 65, 127, 128, 129, 200, 1000, >= Nq + Nk}, ca
 Nq > Nk, both dtypes and both head dims, MHA, GQA on both sides of the backward's split rule (the HEAD_LOOP path with
 2 and 3 query heads per CTA, checked by the launch count), MQA and merged 3-D layouts, a key-padding mask, the float32
 path, head dims 32 and 96, l2norm_qk=False and two (groups, scale) points.  Also: a window of Nq + Nk is bitwise the
-unwindowed op, varlen per sequence is bitwise the dense op, decode matches the dense forward on the valid prefix, the
+unwindowed op, each packed sequence's o, dq, dk, dv match the windowed reference and the dense op (o bitwise, dk, dv
+bitwise where the groups stay in one CTA), decode matches the dense forward on the valid prefix, the
 dq workspace stays zero, and the transformer's windowed CUDA path matches its plain path."""
 import numpy as np
 import pytest
@@ -16,6 +17,7 @@ from window_bounds import window_attention_bounds
 from test_gpu_gqa import loop_batch, sm_count
 from tile_ranges import group_split
 from test_gpu_parity import TOL_GRAD, TOL_OUT, fcsa, float32_ds_scale, float32_operands, make_inputs, record  # noqa: F401
+from test_gpu_varlen import seq_check
 
 pytestmark = pytest.mark.gpu
 
@@ -142,29 +144,54 @@ def test_window_of_nq_plus_nk_is_the_unwindowed_op(fcsa, causal, dim):
             assert torch.equal(a, b)
 
 
-@pytest.mark.parametrize("causal", [True, False])
-@pytest.mark.parametrize("dim", [64, 128])
-def test_window_varlen_per_sequence_is_the_dense_op(fcsa, causal, dim):
+def window_varlen_case(fcsa, dtype, heads, kv_heads, causal, dim):
+    """Packed sequences with rows outside every sequence at both ends: each sequence's o, dq, dk, dv against the
+    float64 windowed reference on it alone, o bitwise the dense op's, and dk, dv bitwise the dense op's where both
+    calls keep each kv group in one CTA."""
     g = torch.Generator().manual_seed(9)
     lq, lk = [130, 0, 257, 64, 1], ([130, 40, 300, 64, 1] if not causal else [130, 0, 257, 64, 1])
     cq = torch.tensor(np.cumsum([3] + lq), dtype=torch.int32)
     ck = torch.tensor(np.cumsum([0] + lk), dtype=torch.int32)
     Tq, Tk = int(cq[-1]) + 5, int(ck[-1])
-    q = torch.randn(Tq, 4, dim, generator=g).to(torch.bfloat16).cuda().requires_grad_()
-    k = torch.randn(Tk, 2, dim, generator=g).to(torch.bfloat16).cuda().requires_grad_()
-    v = torch.randn(Tk, 2, dim, generator=g).to(torch.bfloat16).cuda().requires_grad_()
+    q = torch.randn(Tq, heads, dim, generator=g).to(dtype).cuda().requires_grad_()
+    k = torch.randn(Tk, kv_heads, dim, generator=g).to(dtype).cuda().requires_grad_()
+    v = torch.randn(Tk, kv_heads, dim, generator=g).to(dtype).cuda().requires_grad_()
+    do = torch.randn(Tq, heads, dim, generator=g).to(dtype).cuda()
     window = 70
     o = fcsa.flash_cosine_sim_attention_varlen(q, k, v, cq.cuda(), ck.cuda(), max(lq), max(lk), causal=causal,
                                                window=window)
-    o.float().square().sum().backward()
+    o.backward(do)
     assert (o[:3] == 0).all() and (o[-5:] == 0).all() and (q.grad[:3] == 0).all() and (q.grad[-5:] == 0).all()
+    inside = slice(3, Tq - 5)
+    seq_check(dtype, (o.detach()[inside], q.grad[inside], k.grad, v.grad), q.detach()[inside], k.detach(), v.detach(),
+              do[inside], lq, lk, window=window, causal=causal)
+    packed_one_cta = group_split(len(lq), heads, kv_heads, max(lk), sm_count()) == 1
     for b in range(len(lq)):
         if lq[b] == 0 or lk[b] == 0:
             continue
         qs, ks = slice(int(cq[b]), int(cq[b + 1])), slice(int(ck[b]), int(ck[b + 1]))
         dense = lambda t, s: t.detach()[s].transpose(0, 1).unsqueeze(0)
-        od = fcsa.flash_cosine_sim_attention(dense(q, qs), dense(k, ks), dense(v, ks), causal=causal, window=window)
-        assert torch.equal(o[qs].detach(), od[0].transpose(0, 1))
+        qd, kd, vd = (dense(t, s).requires_grad_() for t, s in ((q, qs), (k, ks), (v, ks)))
+        od = fcsa.flash_cosine_sim_attention(qd, kd, vd, causal=causal, window=window)
+        od.backward(dense(do, qs))
+        assert torch.equal(o[qs].detach(), od.detach()[0].transpose(0, 1))
+        if packed_one_cta and group_split(1, heads, kv_heads, lk[b], sm_count()) == 1:
+            assert torch.equal(k.grad[ks], kd.grad[0].transpose(0, 1)), ("dk", b)
+            assert torch.equal(v.grad[ks], vd.grad[0].transpose(0, 1)), ("dv", b)
+
+
+@pytest.mark.parametrize("causal", [True, False])
+@pytest.mark.parametrize("dim", [64, 128])
+def test_window_varlen_per_sequence_is_the_dense_op(fcsa, causal, dim):
+    window_varlen_case(fcsa, torch.bfloat16, 4, 2, causal, dim)
+
+
+@pytest.mark.parametrize("causal", [True, False])
+@pytest.mark.parametrize("dim", [64, 128])
+@pytest.mark.parametrize("dtype,heads,kv_heads", [(torch.float16, 4, 2), (torch.float16, 4, 4), (torch.bfloat16, 4, 4)],
+                         ids=["f16-4:2", "f16-4:4", "bf16-4:4"])
+def test_window_varlen_dtypes_and_heads(fcsa, dtype, heads, kv_heads, causal, dim):
+    window_varlen_case(fcsa, dtype, heads, kv_heads, causal, dim)
 
 
 @pytest.mark.parametrize("causal", [True, False])
