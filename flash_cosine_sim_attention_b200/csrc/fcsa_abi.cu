@@ -160,7 +160,7 @@ int launch_forward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tenso
     return r;
 
   // (the window's arguments extend the kernel's)
-  fcsa::FwdArgsOf<VARLEN, true> a;
+  fcsa::ArgsOf<fcsa::FwdArgs, fcsa::FwdVarlenArgs, VARLEN, true> a;
   a.window = kernel_window(p);
   if constexpr (VARLEN) {
     a.cu_q = vl->cu_seqlens_q; a.cu_k = vl->cu_seqlens_k; a.total_q = vl->total_q; a.total_k = vl->total_k;
@@ -388,7 +388,7 @@ int launch_dq(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, const float* st
       (r = map_operand<T, D>(&tv, "v", h.v, tB, h.kv_heads, tNk, 128)) ||
       (r = map_operand<T, D>(&tdo, "d_o", h.d_o, tB, h.H, tNq, Cfg::kBlockM)))
     return r;
-  fcsa::DqArgsOf<VARLEN, true> a;
+  fcsa::ArgsOf<fcsa::DqArgs, fcsa::DqVarlenArgs, VARLEN, true> a;
   a.window = h.window;
   if constexpr (VARLEN) {
     a.cu_q = h.cu_q; a.cu_k = h.cu_k; a.total_q = h.total_q; a.total_k = h.total_k; a.ntile = w.nqt;
@@ -485,7 +485,7 @@ int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream
                                   D, h.H * acc_sh, acc_sh, D, Cfg::QT, 32)))
       return fail(FCSA_ERR_CUDA, "dq accumulator: cuTensorMapEncodeTiled failed (%d)", r);
     // (the window's arguments extend the kernel's)
-    BwdArgsOf<VARLEN, true> a;
+    ArgsOf<BwdArgs, BwdVarlenArgs, VARLEN, true> a;
     a.window = h.window;
     a.B = h.B; a.H = h.H; a.Nq = h.Nq; a.Nk = h.Nk; a.kv_heads = h.kv_heads; a.causal = h.causal;
     a.has_mask = h.mask ? 1 : 0; a.nqt = w.nqt;

@@ -76,28 +76,16 @@ struct FwdCfg {
   static_assert(kSmem <= 232448, "forward kernel shared memory");
 };
 
-// The exp stage's key padding mask (key_tile.cuh): key col is kept iff its byte in the batch's mask row is nonzero.
-struct PaddingMask {
-  const uint8_t* row;
-  bool has;
-  __device__ __forceinline__ bool on() const { return has; }
-  __device__ __forceinline__ bool operator()(int col) const { return row[col] != 0; }
-};
-
-template <bool VARLEN, bool WINDOW>
-using FwdArgsOf = std::conditional_t<WINDOW, Windowed<std::conditional_t<VARLEN, FwdVarlenArgs, FwdArgs>>,
-                                     std::conditional_t<VARLEN, FwdVarlenArgs, FwdArgs>>;
-
 // WINDOW: sliding-window attention (Windowed<>::window = W).  A block visits key tiles [j_lo, NT) instead of
 // [0, NT): j_lo is the tile of the smallest lower limit of its rows, and NT moves up by W - 1 when not causal.
 template <typename T, int D, bool BIAS = false, bool VARLEN = false, bool WINDOW = false>
 __global__ void __launch_bounds__(FwdCfg<D>::kThreads, 1)
 fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
-                const __grid_constant__ CUtensorMap tm_v, const FwdArgsOf<VARLEN, WINDOW> a) {
+                const __grid_constant__ CUtensorMap tm_v, const ArgsOf<FwdArgs, FwdVarlenArgs, VARLEN, WINDOW> a) {
   static_assert(!(BIAS && VARLEN), "packed sequences take no bias");
   static_assert(!(BIAS && WINDOW), "a window takes no bias");
   using Cfg = FwdCfg<D>;
-  constexpr int S = Cfg::kStages, TILE = Cfg::kTile, DCH = D / 64, BM = Cfg::kBlockM;
+  constexpr int S = Cfg::kStages, TILE = Cfg::kTile, BM = Cfg::kBlockM;
 
   uint8_t* smem = smem_1024();
   const uint32_t sQ = smem_u32(smem + Cfg::kOffQ);
@@ -114,21 +102,8 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int wg = warp >> 2;
   pdl_launch_dependents();
 
-  // ---- work item: BM query rows of one (batch, head) ------------------------------------
-  // (the heads of one (batch, query block) are consecutive CTAs: the `group` heads sharing a key/value head
-  // stream the same K / V tiles close together in time and meet in L2)
-  const int bh_count = a.B * a.H;
-  const int rank = blockIdx.x / bh_count;
-  const int bh = blockIdx.x - rank * bh_count;
-  const int qblk = a.causal ? (a.n_qblk - 1 - rank) : rank;   // heaviest causal blocks first
-  const int b = bh / a.H, h = bh - b * a.H;
-  const int hk = h / a.group;
-  const int m0 = qblk * BM;
-  // the (batch) coordinate of the tensor maps and the first query / key row of the sequence: packed sequences are
-  // row offsets into maps of batch extent 1; their lengths are read after pdl_wait (a previous kernel may write them)
-  const int tb = VARLEN ? 0 : b;
-  int Nq = a.Nq, Nk = a.Nk, q_row0 = 0, k_row0 = 0;
-
+  // ---- work item: BM query rows of one (batch, head) (key_tile.cuh) ----
+  QueryBlock q = query_block<BM, VARLEN>(a);
   if (threadIdx.x == 0) {
     mbar_init(BAR(Q_FULL), 1);
     kr.init(1, 128 * Cfg::kConsumers);
@@ -137,16 +112,8 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   }
   __syncthreads();
   pdl_wait();          // q, k (normalised by the previous kernel), v, mask are read from here on
-  if constexpr (VARLEN) {
-    const SeqSpan sq = seq_span(a.cu_q, b, a.Nq, a.total_q), sk = seq_span(a.cu_k, b, a.Nk, a.total_k);
-    Nq = sq.len; Nk = sk.len; q_row0 = sq.start; k_row0 = sk.start;
-    if (m0 >= Nq) return;                                     // a query block past the end of its sequence
-  }
-  const int off = diag_off(Nq, Nk);
-  int W = 0;                                                  // the window
-  if constexpr (WINDOW) W = a.window;
-  const TileRange blk = block_key_tiles<WINDOW>(m0, BM, Nq, Nk, off, a.causal, W);
-  const int j_lo = blk.lo, NT = blk.hi;                       // the key tiles [j_lo, NT) this block visits
+  if (!query_block_span<BM, VARLEN, WINDOW>(q, a)) return;
+  const int b = q.b, h = q.h, tb = q.tb, j_lo = q.j_lo, NT = q.NT;
 
   if (wg == 0) {
     // =============================== TMA producer ===============================
@@ -156,9 +123,8 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       tma_prefetch_desc(&tm_k);
       tma_prefetch_desc(&tm_v);
       mbar_expect_tx(BAR(Q_FULL), Cfg::kQ);
-#pragma unroll
-      for (int ch = 0; ch < DCH; ++ch) tma_load_4d(sQ + ch * BM * 128, &tm_q, BAR(Q_FULL), ch * 64, q_row0 + m0, h, tb);
-      load_kv_tiles<D>(&tm_k, &tm_v, kr, vr, sK, sV, j_lo, NT, k_row0, hk, tb);
+      load_query_rows<D>(&tm_q, BAR(Q_FULL), sQ, BM, q.q_row0 + q.m0, h, tb);
+      load_kv_tiles<D>(&tm_k, &tm_v, kr, vr, sK, sV, j_lo, NT, q.k_row0, q.hk, tb);
     }
     return;
   }
@@ -166,10 +132,7 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   // =============================== consumer warpgroups =========================
   reg_alloc<Cfg::kConsumerRegs>();
   const int w = wg - 1;                       // which 64 of the block's BM query rows
-  const int wl = warp & 3;
-  // this thread's two rows (accumulator layout, sm90_primitives.cuh): row_a and row_a + 8
-  const int row_a = m0 + 64 * w + 16 * wl + (lane >> 2);
-  const int cq = 2 * (lane & 3);              // first of the thread's two columns inside every 8-column block
+  const QueryRows r = query_rows<WINDOW>(q, w, a.causal);
   float nc2 = -a.c2;
   if constexpr (BIAS) {
     if (a.bias_amax != nullptr) nc2 -= fmaxf(__ldg(a.bias_amax), 0.f) * 1.4426950408889634f;
@@ -180,12 +143,8 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf)          // (clamped for the padding rows of the last block, never stored)
       brow[hf] = reinterpret_cast<const T*>(a.bias) + (long long)b * a.bias_sb + (long long)h * a.bias_sh +
-                 (long long)min(row_a + 8 * hf, a.Nq - 1) * a.bias_sn;
+                 (long long)min(r.row_a + 8 * hf, a.Nq - 1) * a.bias_sn;
   }
-  // the visible key columns of each of the thread's rows (the selects of a masked tile)
-  ColRange lim[2];
-#pragma unroll
-  for (int hf = 0; hf < 2; ++hf) lim[hf] = row_key_cols<WINDOW>(row_a + 8 * hf, off, Nk, a.causal, W);
   // the additive term (with BIAS: + bias * log2e) and the key padding mask of the exp stage
   auto add = [&](int hf, int col) {
     if constexpr (BIAS) {
@@ -198,9 +157,6 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     }
   };
   const PaddingMask keys = {a.mask + (long long)b * a.mask_sb, a.has_mask != 0};
-  // the key tiles [jw_lo, jw_hi) this warpgroup's own 64 rows see; it only passes the ring slots of the others on
-  const TileRange wgt = warpgroup_key_tiles<WINDOW>(m0 + 64 * w, j_lo, NT, Nq, off, a.causal, W);
-  const int jw_lo = wgt.lo, jw_hi = wgt.hi;
 
   float o[D / 2];
 #pragma unroll
@@ -211,7 +167,7 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
   for (int j = j_lo; j < NT; ++j) {
     const int n = j - j_lo;                   // the rings' use
-    if (j < jw_lo || j >= jw_hi) {
+    if (j < r.wgt.lo || j >= r.wgt.hi) {
       kr.pass(n);
       vr.pass(n);
       continue;
@@ -221,12 +177,9 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     qk_tile<T, D>(sacc, sQw, BM * 128, sK + s * TILE);
     kr.release(n);
 
-    // (the warpgroup's 64 rows unclipped: rows past Nq are never stored, and a later last row only masks more)
-    const int col0 = j * 128;
-    const bool need_mask =
-        a.has_mask || !tile_visible<WINDOW>(m0 + 64 * w, m0 + 64 * w + 63, col0, col0 + 127, off, Nk, a.causal, W);
     uint32_t pf[32];
-    exp_tile<T, WINDOW>(need_mask, sacc, pf, l, c1, col0, cq, lim, add, keys);
+    exp_tile<T, WINDOW>(tile_needs_mask<WINDOW>(q, w, j, a.causal, a.has_mask), sacc, pf, l, c1, j * 128, r.cq, r.lim,
+                        add, keys);
 
     vr.wait(n);
     pv_tile<T>(o, pf, sV + s * TILE);
@@ -242,13 +195,13 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   for (int hf = 0; hf < 2; ++hf) inv[hf] = 1.0f / fmaxf(quad_sum(l[hf]), 1e-37f);
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
-    const int row = row_a + 8 * hf;
-    if (row >= Nq) continue;
-    const long long o_off = (long long)tb * a.o_sb + (long long)h * a.o_sh + (long long)(q_row0 + row) * a.o_sn;
-    if (a.o_f32) store_row(reinterpret_cast<float*>(a.o) + o_off, o, hf, cq, inv[hf]);
-    else store_row(reinterpret_cast<T*>(a.o) + o_off, o, hf, cq, inv[hf]);
+    const int row = r.row_a + 8 * hf;
+    if (row >= q.Nq) continue;
+    const long long o_off = (long long)tb * a.o_sb + (long long)h * a.o_sh + (long long)(q.q_row0 + row) * a.o_sn;
+    if (a.o_f32) store_row(reinterpret_cast<float*>(a.o) + o_off, o, hf, r.cq, inv[hf]);
+    else store_row(reinterpret_cast<T*>(a.o) + o_off, o, hf, r.cq, inv[hf]);
     if ((lane & 3) == 0 && a.inv_l != nullptr) {
-      if constexpr (VARLEN) a.inv_l[(long long)h * a.total_q + q_row0 + row] = inv[hf];
+      if constexpr (VARLEN) a.inv_l[(long long)h * a.total_q + q.q_row0 + row] = inv[hf];
       else a.inv_l[((long long)b * a.H + h) * a.Nq + row] = inv[hf];
     }
   }

@@ -1,9 +1,10 @@
-// The pipeline the forward and decode kernels share, and the mbarrier ring all three attention kernels use.
+// The pipeline the forward, dQ and decode kernels share, and the mbarrier ring all the attention kernels use.
 //
 // Per 128-key tile a consumer warpgroup of 64 query rows computes S = Q K^T (64 x 128, fp32) -> P = exp2(S*c1 + add),
 // masked where the tile needs it, row sums in fp32, 16-bit P as wgmma A fragments -> O += P V.  The kernels keep what
 // differs: how Q gets into shared memory, the additive term and key mask (the forward's bias and padding mask), what
-// happens to V before P V (decode zeroes rows past its valid length) and what the epilogue writes.
+// happens to V before P V (decode zeroes rows past its valid length) and what the epilogue writes.  The forward and
+// dQ kernels also share their work item (QueryBlock): which query block a CTA takes and which key tiles it visits.
 #pragma once
 
 #include "sm90_primitives.cuh"
@@ -47,6 +48,88 @@ struct Ring {
     release(n);
   }
 };
+
+// ---- the work item of the forward and dQ kernels: BM query rows of one (batch, query head) -------------------------
+// CTAs are numbered heaviest causal blocks first (the last query blocks see the most keys, so the block scheduler
+// starts the long ones first), and the heads of one (batch, query block) are consecutive CTAs: the `group` heads
+// sharing a key/value head stream the same K / V tiles close together in time and meet in L2.  Packed sequences
+// (VARLEN) are row offsets into tensor maps of batch extent 1; their lengths are read after pdl_wait (a previous
+// kernel may write them), so the work item is set in two steps: query_block before pdl_wait, query_block_span after.
+struct QueryBlock {
+  int b, h, hk;                    // batch (VARLEN: sequence), query head, key/value head
+  int m0;                          // the block's first query row
+  int tb;                          // the tensor maps' batch coordinate
+  int Nq, Nk, q_row0, k_row0;      // the sequence's lengths and its first query / key row
+  int off, W;                      // diag_off, the window (0 without)
+  int j_lo, NT;                    // the key tiles [j_lo, NT) the block visits
+};
+
+template <int BM, bool VARLEN, class Args>
+__device__ __forceinline__ QueryBlock query_block(const Args& a) {
+  QueryBlock q;
+  const int bh_count = a.B * a.H;
+  const int rank = blockIdx.x / bh_count;
+  const int bh = blockIdx.x - rank * bh_count;
+  const int qblk = a.causal ? (a.n_qblk - 1 - rank) : rank;
+  q.b = bh / a.H;
+  q.h = bh - q.b * a.H;
+  q.hk = q.h / a.group;
+  q.m0 = qblk * BM;
+  q.tb = VARLEN ? 0 : q.b;
+  return q;
+}
+
+// The sequence's lengths and the block's key tiles; false for a query block past the end of its sequence.
+template <int BM, bool VARLEN, bool WINDOW, class Args>
+__device__ __forceinline__ bool query_block_span(QueryBlock& q, const Args& a) {
+  q.Nq = a.Nq, q.Nk = a.Nk, q.q_row0 = 0, q.k_row0 = 0;
+  if constexpr (VARLEN) {
+    const SeqSpan sq = seq_span(a.cu_q, q.b, a.Nq, a.total_q), sk = seq_span(a.cu_k, q.b, a.Nk, a.total_k);
+    q.Nq = sq.len, q.Nk = sk.len, q.q_row0 = sq.start, q.k_row0 = sk.start;
+    if (q.m0 >= q.Nq) return false;
+  }
+  q.off = diag_off(q.Nq, q.Nk);
+  q.W = 0;
+  if constexpr (WINDOW) q.W = a.window;
+  const TileRange blk = block_key_tiles<WINDOW>(q.m0, BM, q.Nq, q.Nk, q.off, a.causal, q.W);
+  q.j_lo = blk.lo, q.NT = blk.hi;
+  return true;
+}
+
+// A consumer thread of warpgroup w, which owns the block's rows m0 + 64 w .. + 63.
+struct QueryRows {
+  int row_a;                       // the thread's rows (accumulator layout, sm90_primitives.cuh): row_a and row_a + 8
+  int cq;                          // first of the thread's two columns inside every 8-column block
+  ColRange lim[2];                 // the visible key columns of each of its rows (the selects of a masked tile)
+  TileRange wgt;                   // the key tiles its warpgroup's rows see; it only passes the others' ring slots on
+};
+template <bool WINDOW>
+__device__ __forceinline__ QueryRows query_rows(const QueryBlock& q, int w, int causal) {
+  const int lane = threadIdx.x & 31, wl = (threadIdx.x >> 5) & 3;
+  QueryRows r;
+  r.row_a = q.m0 + 64 * w + 16 * wl + (lane >> 2);
+  r.cq = 2 * (lane & 3);
+#pragma unroll
+  for (int hf = 0; hf < 2; ++hf) r.lim[hf] = row_key_cols<WINDOW>(r.row_a + 8 * hf, q.off, q.Nk, causal, q.W);
+  r.wgt = warpgroup_key_tiles<WINDOW>(q.m0 + 64 * w, q.j_lo, q.NT, q.Nq, q.off, causal, q.W);
+  return r;
+}
+
+// Whether key tile j needs the per-element selects for warpgroup w's rows (the 64 rows unclipped: rows past Nq are
+// never stored, and a later last row only masks more).
+template <bool WINDOW>
+__device__ __forceinline__ bool tile_needs_mask(const QueryBlock& q, int w, int j, int causal, int has_mask) {
+  const int r0 = q.m0 + 64 * w, col0 = j * 128;
+  return has_mask || !tile_visible<WINDOW>(r0, r0 + 63, col0, col0 + 127, q.off, q.Nk, causal, q.W);
+}
+
+// ---- producer: a block's query rows [row, row + rows) of head h, one TMA box per 64-feature chunk -----------------
+template <int D>
+__device__ __forceinline__ void load_query_rows(const CUtensorMap* tm, uint32_t bar, uint32_t sdst, int rows, int row,
+                                                int h, int tb) {
+#pragma unroll
+  for (int ch = 0; ch < D / 64; ++ch) tma_load_4d(sdst + ch * rows * 128, tm, bar, ch * 64, row, h, tb);
+}
 
 // ---- producer: K and V tiles [j0, j1) through the two rings (tile j is use j - j0) --------------------------------
 // Tile j is rows row0 + 128 j of kv head hk at batch coordinate tb, D / 64 TMA boxes of 64 features each.
@@ -97,9 +180,17 @@ struct AllKeys {                     // no key padding mask
   __device__ __forceinline__ bool on() const { return false; }
   __device__ __forceinline__ bool operator()(int) const { return true; }
 };
-template <typename T, bool WINDOW, class Add, class Keys>
-__device__ __forceinline__ void exp_tile(bool need_mask, const float (&sacc)[64], uint32_t (&pf)[32], float (&l)[2],
-                                         float c1, int col0, int cq, const ColRange (&lim)[2], Add add, Keys keys) {
+struct PaddingMask {                 // key col is kept iff its byte in the batch's mask row is nonzero
+  const uint8_t* row;
+  bool has;
+  __device__ __forceinline__ bool on() const { return has; }
+  __device__ __forceinline__ bool operator()(int col) const { return row[col] != 0; }
+};
+// The loop of exp_tile, handing each pair (p0, p1) of element pair i to emit(i, hf, p0, p1): the dQ kernel's dS stage
+// runs it with c3 as the additive term.
+template <bool WINDOW, class Add, class Keys, class Emit>
+__device__ __forceinline__ void exp_pairs(bool need_mask, const float (&sacc)[64], float c1, int col0, int cq,
+                                          const ColRange (&lim)[2], Add add, Keys keys, Emit emit) {
   auto run = [&](auto masked_tag) {
     constexpr bool MASKED = decltype(masked_tag)::value;
 #pragma unroll
@@ -122,12 +213,19 @@ __device__ __forceinline__ void exp_tile(bool need_mask, const float (&sacc)[64]
         p0 = v0 ? p0 : 0.f;
         p1 = v1 ? p1 : 0.f;
       }
-      l[hf] += p0 + p1;
-      pf[i] = pack2<T>(p0, p1);
+      emit(i, hf, p0, p1);
     }
   };
   if (need_mask) run(std::true_type{});
   else run(std::false_type{});
+}
+template <typename T, bool WINDOW, class Add, class Keys>
+__device__ __forceinline__ void exp_tile(bool need_mask, const float (&sacc)[64], uint32_t (&pf)[32], float (&l)[2],
+                                         float c1, int col0, int cq, const ColRange (&lim)[2], Add add, Keys keys) {
+  exp_pairs<WINDOW>(need_mask, sacc, c1, col0, cq, lim, add, keys, [&](int i, int hf, float p0, float p1) {
+    l[hf] += p0 + p1;
+    pf[i] = pack2<T>(p0, p1);
+  });
 }
 
 // ---- consumer: O += P V ----------------------------------------------------------------------------------------

@@ -148,6 +148,67 @@ __device__ __forceinline__ void l2norm_bwd_group(float (&g)[F], const float (&y)
   }
 }
 
+// l2norm backward of one key row in the backward epilogue: dk = (dk_hat - k_hat <k_hat, dk_hat>_group) * rnorm_group.
+// The thread holds features 8 jb + cq + {0, 1} (g[2 jb], g[2 jb + 1]) of the row; the row's other features are in the
+// other three lanes of its quad.  k_hat comes from the resident K tile (row address sk_row, 128B swizzle, 64-feature
+// chunks 16 KB apart).  All lanes of the warp must call it (quad shuffles); `in` = the key exists.  k_rnorm has
+// `groups` floats per row; the key's row is krow0 + key.  (The dQ kernel applies it to a row of its resident Q tile.)
+template <typename T, int D>
+__device__ __forceinline__ void l2norm_bwd_key_row(float (&g)[D / 4], const float* k_rnorm, int groups, uint32_t sk_row,
+                                                   long long krow0, int key, bool in) {
+  const int lane = threadIdx.x & 31;
+  const int r8 = (lane >> 2) & 7, cq = 2 * (lane & 3);
+  const int gs = D / groups;                    // features per group (a power of two)
+  float y[D / 4], dot[D / 4];
+#pragma unroll
+  for (int jb = 0; jb < D / 8; ++jb) {
+    const float2 v = unpack2<T>(lds32(sk_row + (jb >> 3) * 16384 + ((((jb & 7) ^ r8)) << 4) + 2 * cq));
+    y[2 * jb] = v.x;
+    y[2 * jb + 1] = v.y;
+  }
+  if (gs == 1) {
+#pragma unroll
+    for (int e = 0; e < D / 4; ++e) dot[e] = y[e] * g[e];
+  } else {
+    float q[D / 8];                             // sums over the thread's feature pairs, then over the group
+#pragma unroll
+    for (int jb = 0; jb < D / 8; ++jb) q[jb] = y[2 * jb] * g[2 * jb] + y[2 * jb + 1] * g[2 * jb + 1];
+    // groups wider than 8 features: aligned blocks of gs / 8 pairs (compile-time register indices only)
+#pragma unroll
+    for (int m = 1; m < D / 8; m <<= 1) {
+      float t[D / 8];
+#pragma unroll
+      for (int jb = 0; jb < D / 8; ++jb) t[jb] = q[jb] + q[jb ^ m];
+      if (8 * m < gs) {
+#pragma unroll
+        for (int jb = 0; jb < D / 8; ++jb) q[jb] = t[jb];
+      }
+    }
+    // across the quad: gs = 4 spans lane pairs, gs >= 8 all four lanes
+    if (gs >= 4) {
+#pragma unroll
+      for (int jb = 0; jb < D / 8; ++jb) q[jb] += __shfl_xor_sync(0xFFFFFFFFu, q[jb], 1);
+    }
+    if (gs >= 8) {
+#pragma unroll
+      for (int jb = 0; jb < D / 8; ++jb) q[jb] += __shfl_xor_sync(0xFFFFFFFFu, q[jb], 2);
+    }
+#pragma unroll
+    for (int jb = 0; jb < D / 8; ++jb) dot[2 * jb] = dot[2 * jb + 1] = q[jb];
+  }
+  const int lg = __ffs(gs) - 1;
+  const float* rn = k_rnorm + (krow0 + (in ? key : 0)) * groups;         // k_rnorm row krow0 + key
+  // one load per feature pair (a pair shares its group unless gs = 1); the pairs of one group hit the same L1 line
+#pragma unroll
+  for (int jb = 0; jb < D / 8; ++jb) {
+    const int f = 8 * jb + cq;
+    const float r0 = in ? __ldg(rn + (f >> lg)) : 0.f;
+    const float r1 = gs == 1 && in ? __ldg(rn + f + 1) : r0;
+    g[2 * jb] = (g[2 * jb] - y[2 * jb] * dot[2 * jb]) * r0;
+    g[2 * jb + 1] = (g[2 * jb + 1] - y[2 * jb + 1] * dot[2 * jb + 1]) * r1;
+  }
+}
+
 // One 16-byte vector of X (16-bit: 8 elements, float: 4) to and from fp32.
 template <typename X>
 __device__ __forceinline__ void unpack16B(uint4 r, float* f) {

@@ -426,4 +426,9 @@ struct Windowed : Base {
   int window;
 };
 
+// A kernel's argument struct: Dense, or Varlen for packed sequences, with the window when WINDOW.
+template <class Dense, class Varlen, bool VARLEN, bool WINDOW>
+using ArgsOf = std::conditional_t<WINDOW, Windowed<std::conditional_t<VARLEN, Varlen, Dense>>,
+                                  std::conditional_t<VARLEN, Varlen, Dense>>;
+
 }  // namespace fcsa
