@@ -10,7 +10,8 @@
 // The machine mapping is new.  Three kernels:
 //   1. bwd_prep_kernel    : per query row {c3 = log2(inv_l) - shift*log2e, -delta} (fp32, never
 //                           rounded to 16 bit as the reference does at cu:1260/1820)
-//   2. fcsa_bwd_kernel    : one CTA = one 128-key tile of one (batch, kv head), K and V stationary in shared memory,
+//   2. fcsa_bwd_kernel    : one CTA = one 128-key tile of one (batch, kv head) (192 keys and three consumer
+//                           warpgroups for D = 64 without a bias or head loop: BwdCfg), K and V stationary in shared memory,
 //                           loop over the query tiles of QT = 64 rows that can see it, for each query head of the
 //                           CTA's slice of the kv head's group (grouped-query attention; one head for MHA): the
 //                           (head, query tile) pairs form one flat sequence of tiles.  Warpgroup 0 is the TMA
@@ -46,34 +47,43 @@
 
 namespace fcsa {
 
-// D = 64 computes one dQ tile per query tile and CTA (a contraction over all 128 keys, shared by the two
-// warpgroups through shared memory), stages it for TMA reduce-adds and pipelines the products of consecutive
-// query tiles; D = 128 has neither the shared memory (two 32 KB staging tiles on top of 194 KB) nor the
-// registers (a second S^T / dP^T pair next to 128 dV / dK accumulators) for that, and keeps the in-order loop
-// with a dQ partial per warpgroup and vector reductions from registers.
-template <int D>
+// D = 64 computes one dQ tile per query tile and CTA (a contraction over all the CTA's keys, shared by its
+// warpgroups through shared memory) and stages it for TMA reduce-adds.  Without a bias or a head loop it runs three
+// consumer warpgroups over 192 keys (kWide) on the in-order loop: at 160 registers a warpgroup has no room for the
+// next tile's S^T / dP^T, so the other two warpgroups' products fill the tensor cores instead (DESIGN.md 4.2).  The
+// BIAS and HEAD_LOOP kernels keep two warpgroups over 128 keys and pipeline the products of consecutive query tiles
+// (a head loop's grid is sized to about fill the device with 128-key CTAs).  D = 128 has
+// neither the shared memory (two 32 KB staging tiles on top of 194 KB) nor the registers (a second S^T / dP^T pair
+// next to 128 dV / dK accumulators) for either, and keeps the in-order loop with a dQ partial per warpgroup and vector
+// reductions from registers.  The dK / dV-only kernels (DQ = false) keep the two-warpgroup layout.
+template <int D, bool BIAS = false, bool DQ = true, bool HEAD_LOOP = false>
 struct BwdCfg {
+  static constexpr int kKeys = bwd_block_keys(D, BIAS, DQ, HEAD_LOOP);     // keys of one work item
+  static constexpr int kConsumers = kKeys / 64;                    // consumer warpgroups, 64 keys each
+  static constexpr bool kWide = kConsumers == 3;
   static constexpr bool kStaged = (D == 64);
   static constexpr int QT = 64;                           // query rows per tile
-  static constexpr int kKV = 128 * D * 2;                 // bytes of the K (or V) tile
+  static constexpr int kKV = kKeys * D * 2;               // bytes of the K (or V) tile
   static constexpr int kQ = QT * D * 2;                   // bytes of one Q (or dO) stage
   static constexpr int NST = kStaged ? 4 : 3;             // Q / dO / stats ring depth
   static constexpr int kDS = 64 * QT * 2;                 // one warpgroup's dS^T: 64 keys x QT queries, 16-bit
-  static constexpr int NDS = kStaged ? 3 : 2;             // dS^T slots (one buffer per warpgroup each)
+  static constexpr int NDS = kStaged && !kWide ? 3 : 2;   // dS^T slots (one buffer per warpgroup each)
   static constexpr int NDQ = kStaged ? 1 : 0;             // dQ staging buffers per warpgroup
   static constexpr int kDQ = kStaged ? QT * D * 4 : 0;    // one fp32 dQ staging tile: D / 32 boxes of 32 x QT
   static constexpr int kOffK = 0;
   static constexpr int kOffV = kOffK + kKV;
   static constexpr int kOffQ = kOffV + kKV;
   static constexpr int kOffDO = kOffQ + NST * kQ;
-  static constexpr int kOffDS = kOffDO + NST * kQ;        // NDS slots x 2 warpgroups (slot-major: 128 keys each)
-  static constexpr int kOffDQ = kOffDS + 2 * NDS * kDS;   // 2 warpgroups x NDQ buffers (1024-byte aligned)
-  static constexpr int kOffStats = kOffDQ + 2 * NDQ * kDQ;  // NST stages x {c3, -delta} x QT floats
+  static constexpr int kOffDS = kOffDO + NST * kQ;        // NDS slots x kConsumers warpgroups (slot-major)
+  static constexpr int kOffDQ = kOffDS + kConsumers * NDS * kDS;     // kConsumers x NDQ buffers (1024-byte aligned)
+  static constexpr int kOffStats = kOffDQ + kConsumers * NDQ * kDQ;  // NST stages x {c3, -delta} x QT floats
   static constexpr int kOffBar = kOffStats + NST * 8 * QT;
   static constexpr int kSmem = kOffBar + 256 + 1024;
   static_assert(kSmem <= 232448, "backward kernel shared memory");
   static_assert(kOffDQ % 1024 == 0, "128B-swizzled staging tiles");
-  static constexpr int kThreads = 384;                    // producer warpgroup + 2 consumer warpgroups
+  static constexpr int kThreads = 128 * (1 + kConsumers);  // + the producer warpgroup
+  static constexpr int kProducerRegs = kWide ? kProducerRegs3 : fcsa::kProducerRegs;
+  static constexpr int kConsumerRegs = kWide ? kConsumerRegs3 : fcsa::kConsumerRegs;
 };
 
 // ------------------------------------------------------------------------------------------
@@ -315,9 +325,12 @@ __device__ __forceinline__ float4 ldg_cg128f(const float* p) {
 // DQ = false: dK and dV only (the deterministic backward, whose dq comes from fcsa_dq_kernel).  No dS^T in shared
 // memory, no dQ product, no reducer warps, no dq accumulator; both head dims run the in-order loop, and the host
 // launches it with split = 1, so dk / dv always leave through the direct epilogue.
+// Work items of kKeys = 192 keys (BwdCfg::kWide: D = 64 with dQ, without a bias or a head loop) have three consumer
+// warpgroups and run the in-order loop with one staged dQ tile per query tile and CTA; each warpgroup computes only the
+// query tiles its own 64 keys see.
 template <typename T, int D, bool BIAS = false, bool HEAD_LOOP = false, bool VARLEN = false, bool WINDOW = false,
           bool DQ = true>
-__global__ void __launch_bounds__(384, 1)
+__global__ void __launch_bounds__(BwdCfg<D, BIAS, DQ, HEAD_LOOP>::kThreads, 1)
 fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                 const __grid_constant__ CUtensorMap tm_v, const __grid_constant__ CUtensorMap tm_do,
                 const __grid_constant__ CUtensorMap tm_dq, const ArgsOf<BwdArgs, BwdVarlenArgs, VARLEN, WINDOW> a) {
@@ -326,11 +339,14 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   static_assert(!(BIAS && VARLEN), "packed sequences take no bias");
   static_assert(!(BIAS && WINDOW), "a window takes no bias");
   static_assert(DQ || !BIAS, "the dK / dV-only kernel takes no bias");
-  using Cfg = BwdCfg<D>;
+  using Cfg = BwdCfg<D, BIAS, DQ, HEAD_LOOP>;
+  constexpr bool WIDE = Cfg::kWide;
+  constexpr int NC = Cfg::kConsumers;      // consumer warpgroups
   constexpr bool STAGED = Cfg::kStaged && DQ;
   constexpr int QT = Cfg::QT;              // query rows per tile
   constexpr int KCH = D / 64;              // 64-feature chunks of every operand tile
   constexpr int QCHUNK = QT * 128;         // bytes of one 64-feature chunk of a Q / dO stage
+  constexpr int KCHUNK = Cfg::kKeys * 128; // ... and of the K (or V) tile
   constexpr int NST = Cfg::NST;
 
   uint8_t* smem = smem_1024();
@@ -346,8 +362,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   // STAGED only: DQ_FULL / DQ_EMPTY + NDQ w + buffer: warpgroup w's dQ staging tiles; DS_FULL / DS_EMPTY + slot:
   // the dS^T slot holds both halves of the tile that uses it / the dQ product reading the slot has retired
   constexpr int NDQ = STAGED ? Cfg::NDQ : 1, NDS = Cfg::NDS;    // (a divisor even where the staging is compiled out)
-  constexpr int KV_FULL = 0, FULL = 1, EMPTY = FULL + NST, DQ_FULL = EMPTY + NST, DQ_EMPTY = DQ_FULL + 2 * NDQ,
-                DS_FULL = DQ_EMPTY + 2 * NDQ, DS_EMPTY = DS_FULL + NDS, NBARS = DS_EMPTY + NDS;
+  constexpr int KV_FULL = 0, FULL = 1, EMPTY = FULL + NST, DQ_FULL = EMPTY + NST, DQ_EMPTY = DQ_FULL + NC * NDQ,
+                DS_FULL = DQ_EMPTY + NC * NDQ, DS_EMPTY = DS_FULL + NDS, NBARS = DS_EMPTY + NDS;
   static_assert(NBARS * 8 <= 256, "barrier area");
   const Ring<NST> qring = {BAR(FULL), BAR(EMPTY)};            // Q, dO and the stats of a query tile
   const Ring<NDS> dsr = {BAR(DS_FULL), BAR(DS_EMPTY)};        // STAGED: the dS^T slots
@@ -368,7 +384,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int hk = (HEAD_LOOP || a.split > 1) ? sl / a.split : sl;
   const int hpc = HEAD_LOOP ? a.hpc : 1;
   const int h0 = sl * hpc;                    // = hk * G + (slice within the group) * hpc
-  const int key0 = jt * 128;
+  const int key0 = jt * Cfg::kKeys;
   // packed sequences: the tensor maps' batch coordinate is 0, the sequence starts at query row q_row0 and key row
   // k_row0, and its stats / dq accumulator at tile qbase of each head; the lengths are read after pdl_wait
   const int tb = VARLEN ? 0 : b;
@@ -376,10 +392,10 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
 
   if (threadIdx.x == 0) {
     mbar_init(BAR(KV_FULL), 1);
-    qring.init(1, 256);
-    dq_ring(0).init(128, 1);                  // filled by a consumer warpgroup, emptied by its reducer thread
-    dq_ring(1).init(128, 1);
-    dsr.init(128, 128);
+    qring.init(1, 128 * NC);
+#pragma unroll
+    for (int c = 0; c < NC; ++c) dq_ring(c).init(128, 1);    // filled by a consumer warpgroup, emptied by its reducer
+    dsr.init(128 * (NC - 1), 128);
     fence_mbar_init();
   }
   __syncthreads();
@@ -394,14 +410,16 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const int off = diag_off(Nq, Nk);
   int W = 0;                                  // the window
   if constexpr (WINDOW) W = a.window;
-  const TileRange qr = query_tiles<WINDOW>(key0, off, nqt, a.causal, W);
+  // (WIDE: a short last item's range ends with its last key's)
+  const TileRange qr = WIDE ? key_block_query_tiles<WINDOW>(key0, Cfg::kKeys, Nk, off, nqt, a.causal, W)
+                            : query_tiles<WINDOW>(key0, off, nqt, a.causal, W);
   const int i_lo = qr.lo, i_end = qr.hi;      // the query tiles [i_lo, i_end) visited per query head
   const int NI = tile_count(qr);              // number of query tiles to visit per query head
   const int NT = hpc * NI;                    // flat tile index i: head h0 + i / NI, query tile i_lo + i % NI
 
   if (wg == 0) {
     // =============================== TMA producer ===============================
-    reg_dealloc<kProducerRegs>();
+    reg_dealloc<Cfg::kProducerRegs>();
     if (warp == 0 && elect_one()) {
       tma_prefetch_desc(&tm_q);
       tma_prefetch_desc(&tm_k);
@@ -410,8 +428,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       mbar_expect_tx(BAR(KV_FULL), 2 * Cfg::kKV);
 #pragma unroll
       for (int ch = 0; ch < KCH; ++ch) {
-        tma_load_4d(sK + ch * 16384, &tm_k, BAR(KV_FULL), ch * 64, k_row0 + key0, hk, tb);
-        tma_load_4d(sV + ch * 16384, &tm_v, BAR(KV_FULL), ch * 64, k_row0 + key0, hk, tb);
+        tma_load_4d(sK + ch * KCHUNK, &tm_k, BAR(KV_FULL), ch * 64, k_row0 + key0, hk, tb);
+        tma_load_4d(sV + ch * KCHUNK, &tm_v, BAR(KV_FULL), ch * 64, k_row0 + key0, hk, tb);
       }
       for (int i = 0, h = h0; h < h0 + hpc; ++h) {
         long long tile0 = ((long long)b * a.H + h) * a.nqt;     // the stats tile of query tile 0
@@ -429,16 +447,16 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           bulk_load_1d(sStats + st * 8 * QT, stats_h + (long long)qt * 2 * QT, 8 * QT, full);
         }
       }
-    } else if (STAGED && (warp == 1 || warp == 2) && elect_one()) {
-      // dQ reducer of consumer warpgroup warp - 1, which owns the query tiles i = warp - 1 (mod 2): each staged
+    } else if (STAGED && warp >= 1 && warp <= NC && elect_one()) {
+      // dQ reducer of consumer warpgroup warp - 1, which owns the query tiles i = warp - 1 (mod NC): each staged
       // 64 x D fp32 tile is added into the accumulator by TMA (rows at or beyond Nq lie outside the tensor map
       // and are not written; with packed sequences the rows of a tail tile past the sequence's end are inside it,
       // and the dq finish kernel clears them)
       const int rw = warp - 1;
       const Ring<NDQ> dqr = dq_ring(rw);
       if (rw == 0) tma_prefetch_desc(&tm_dq);
-      for (int i = rw; i < NT; i += 2) {
-        const int n = i >> 1;                      // the warpgroup's n-th tile
+      for (int i = rw; i < NT; i += NC) {
+        const int n = i / NC;                      // the warpgroup's n-th tile
         const HeadTile ht = head_tile(i, i_lo, NI, HEAD_LOOP);
         const int hh = ht.head, qt = ht.qt;
         const uint32_t src = sDQ + (NDQ * rw + dqr.wait(n)) * Cfg::kDQ;
@@ -455,7 +473,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   }
 
   // =============================== consumer warpgroups =============================
-  reg_alloc<kConsumerRegs>();
+  reg_alloc<Cfg::kConsumerRegs>();
   const int w = wg - 1;                       // keys key0 + 64 w .. + 63
   const int wl = warp & 3;
   const int r8 = lane >> 2;                   // row inside every 8-row group of an accumulator
@@ -493,13 +511,13 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk) {
-      const uint32_t ka = (kk >> 2) * 16384 + (kk & 3) * 32, kb = (kk >> 2) * QCHUNK + (kk & 3) * 32;
+      const uint32_t ka = (kk >> 2) * KCHUNK + (kk & 3) * 32, kb = (kk >> 2) * QCHUNK + (kk & 3) * 32;
       wgmma_ss_n64<T, 0, 0>(s, gmma_desc_sw128(sKw + ka, 16, 1024), gmma_desc_sw128(sQs + kb, 16, 1024),
                             kk > 0 ? 1u : 0u);
     }
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk) {
-      const uint32_t ka = (kk >> 2) * 16384 + (kk & 3) * 32, kb = (kk >> 2) * QCHUNK + (kk & 3) * 32;
+      const uint32_t ka = (kk >> 2) * KCHUNK + (kk & 3) * 32, kb = (kk >> 2) * QCHUNK + (kk & 3) * 32;
       wgmma_ss_n64<T, 0, 0>(dp, gmma_desc_sw128(sVw + ka, 16, 1024), gmma_desc_sw128(sDOs + kb, 16, 1024),
                             kk > 0 ? 1u : 0u);
     }
@@ -578,7 +596,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
                  row0 + QT - 1 <= key0 + 64 * w + hi_off;
     if (!BIAS && interior) elementwise(false, s, dp, pf, dsf, row0, stc3, dsbuf);
     else elementwise(true, s, dp, pf, dsf, row0, stc3, dsbuf);
-    if constexpr (DQ) {
+    if constexpr (DQ && !WIDE) {
       fence_proxy_async_smem();
       named_bar_sync(1 + w, 128);             // the warpgroup's whole dS^T tile is in shared memory
     }
@@ -599,18 +617,39 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       wgmma_rs<T, 1>(dk, af, gmma_desc_sw128(sQs + kk * 2048, QCHUNK, 1024), 1u);
     }
   };
-  // dQ = dS K.  STAGED: contraction over all 128 keys of the CTA (dsbuf = a dS^T slot, whose two warpgroup halves
-  // are contiguous: 16 keys = 2048 bytes throughout); otherwise a partial over the warpgroup's 64 keys.
+  // dQ = dS K.  STAGED: contraction over all kKeys keys of the CTA (dsbuf = a dS^T slot, whose warpgroup parts are
+  // contiguous: 16 keys = 2048 bytes throughout); otherwise a partial over the warpgroup's 64 keys.
   auto issue_dq = [&](float (&dq)[D / 2], uint32_t dsbuf) {
-    constexpr int NKK = STAGED ? 8 : 4;
+    constexpr int NKK = STAGED ? Cfg::kKeys / 16 : 4;
     const uint32_t sKd = STAGED ? sK : sKw;
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < NKK; ++kk) {
       const uint64_t da = gmma_desc_sw128(dsbuf + kk * 2048, 8192, 1024);     // dS: queries contiguous (MN-major)
-      const uint64_t db = gmma_desc_sw128(sKd + kk * 2048, 16384, 1024);      // K: features contiguous (MN-major)
+      const uint64_t db = gmma_desc_sw128(sKd + kk * 2048, KCHUNK, 1024);      // K: features contiguous (MN-major)
       wgmma_ss<T, 1, 1>(dq, da, db, kk > 0 ? 1u : 0u);
     }
+  };
+
+  // STAGED: tile i's dS^T lives in slot i % NDS (the warpgroups' parts contiguous), and a finished dQ tile, the
+  // warpgroup's n-th, leaves through the warpgroup's staging buffer to its reducer warp.
+  // Staging word of accumulator pair (jb, hf): box jb / 4, row 16 wl + r8 + 8 hf, 16-byte chunk
+  // (2 (jb & 3) + (lane & 3) / 2) ^ r8, 8-byte half lane & 1.  Each warp store covers all 32 banks twice.
+  auto ds_slot = [&](int i) { return sDS + NC * (i % NDS) * Cfg::kDS; };
+  const uint32_t dq_thr = (16 * wl + r8) * 128 + (lane & 1) * 8;
+  const int dq_sx = ((lane & 3) >> 1) ^ r8;
+  const Ring<NDQ> dqr = dq_ring(w);
+  auto stage_dq = [&](const float (&dq)[D / 2], int n) {
+    const int sb = dqr.acquire(n);            // the reducer has read the buffer's last tile
+    const uint32_t dst = sDQ + (NDQ * w + sb) * Cfg::kDQ + dq_thr;
+#pragma unroll
+    for (int jb = 0; jb < D / 8; ++jb) {
+      const uint32_t o = dst + (jb >> 2) * (QT * 128) + (((2 * (jb & 3)) ^ dq_sx) << 4);
+      sts64f(o, dq[4 * jb], dq[4 * jb + 1]);
+      sts64f(o + 1024, dq[4 * jb + 2], dq[4 * jb + 3]);
+    }
+    fence_proxy_async_smem();
+    dqr.commit(n);
   };
 
   float dv[D / 2], dk[D / 2];
@@ -619,7 +658,84 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   // the producer loads K and V whatever NI; the epilogue reads K (l2norm backward) even when no query tile is visited
   mbar_wait(BAR(KV_FULL), 0);
 
-  if constexpr (STAGED) {
+  if constexpr (WIDE) {
+    // In order per tile: S^T, dP^T -> elementwise -> dV, dK -> (owner) dQ of the tile before, one wait per batch.  One
+    // dQ tile per query tile and CTA, dQ(i) = [dS_0(i) | dS_1(i) | dS_2(i)] K over all 192 keys, owned by warpgroup
+    // i % 3 and issued in its iteration i + 1 after the dV / dK wait, so that the 32 dQ accumulators are dead through
+    // the elementwise stage and the dV / dK products.
+    // A warpgroup computes only the query tiles its own keys see (wr); on the item's other tiles it writes zeros to
+    // its part of the slot, so dQ(i) is always the one 12-wgmma product, and passes the Q slot on.
+    //   DS_FULL  : the two non-owners fence their parts to the async proxy and arrive (256 threads) after writing
+    //              them; the owner waits before issuing dQ(i)
+    //   DS_EMPTY : the owner arrives (128 threads) after the wait that retires dQ(i); every warpgroup waits for it
+    //              before writing its part of the slot for tile i + NDS (the owner of i has retired dQ(i) itself)
+    // The owner then stages dQ(i) for its reducer warp.
+    const TileRange wr = key_block_query_tiles<WINDOW>(key0 + 64 * w, 64, Nk, off, nqt, a.causal, W);
+    for (int i = 0; i < NT; ++i) {
+      const HeadTile ht = head_tile(i, i_lo, NI, HEAD_LOOP);
+      const int st = qring.wait(i);
+      const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
+      const uint32_t dsbuf = ds_slot(i) + w * Cfg::kDS;
+      const bool mine = ht.qt >= wr.lo && ht.qt < wr.hi;
+      uint32_t pf[QT / 4], dsf[QT / 4];
+      if (mine) {
+        float s[QT / 2], dp[QT / 2];
+        issue_s_dp(s, dp, sQs, sDOs);
+        if (i >= NDS) dsr.acquire(i);
+        wgmma_wait<0>();
+        fence_regs(s);
+        fence_regs(dp);
+        elementwise_tile(s, dp, pf, dsf, ht.qt * QT, sStats + st * 8 * QT, dsbuf);
+      } else {
+        if (i >= NDS) dsr.acquire(i);
+#pragma unroll
+        for (int j = 0; j < QT / 8; ++j) {
+          sts32(dsbuf + ds_thr + ((j ^ r8) << 4), 0u);
+          sts32(dsbuf + ds_thr + ((j ^ r8) << 4) + 1024, 0u);
+        }
+      }
+      fence_proxy_async_smem();
+      named_bar_sync(1 + w, 128);               // the warpgroup's whole part of dS^T(i) is in shared memory
+      // what follows is redone from an opaque copy of i rather than kept live through the elementwise stage
+      int io = i;
+      asm volatile("" : "+r"(io));
+      const int own = io % NC;
+      if (own != w) dsr.commit(io);
+      if (mine) {
+        const int so = io % NST;
+        issue_dv_dk(pf, dsf, sQ + so * Cfg::kQ, sDO + so * Cfg::kQ, dv, dk);
+        wgmma_commit();
+        wgmma_wait<0>();                        // the dQ accumulator only fits once the A fragments are dead
+        fence_regs(pf);
+        fence_regs(dsf);
+        fence_regs(dv);
+        fence_regs(dk);
+      }
+      qring.release(io);                        // Q, dO and the stats of this stage are no longer read
+      if (io > 0 && (own == 0 ? NC - 1 : own - 1) == w) {
+        float dq[D / 2];
+        dsr.wait(io - 1);
+        issue_dq(dq, ds_slot(io - 1));
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(dv);
+        fence_regs(dk);
+        fence_regs(dq);
+        dsr.release(io - 1);
+        stage_dq(dq, (io - 1) / NC);
+      }
+    }
+    if (NT > 0 && (NT - 1) % NC == w) {
+      float dq[D / 2];
+      dsr.wait(NT - 1);
+      issue_dq(dq, ds_slot(NT - 1));
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(dq);
+      dsr.release(NT - 1);
+      stage_dq(dq, (NT - 1) / NC);
+    }
+  } else if constexpr (STAGED) {
     // One dQ tile per query tile and CTA, dQ(i) = [dS_0(i) | dS_1(i)] K over all 128 keys, owned by warpgroup i & 1
     // (i = loop index, so both warpgroups agree; the last tile has one owner whatever NI).  The owner issues it one
     // tile late, in the batch of tile i + 1 behind dV / dK(i + 1) and ahead of S^T / dP^T(i + 2) (20 wgmmas, one
@@ -633,34 +749,15 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     // dQ(i) is retired by the owner's wait at iteration i + 2 and leaves through shared memory: the warpgroup
     // stores the fp32 tile (128B swizzle, the layout of a 32-feature TMA box) and its reducer warp adds it into
     // the accumulator.  Each warpgroup stages every other tile.
-    // Staging word of accumulator pair (jb, hf): box jb / 4, row 16 wl + r8 + 8 hf, 16-byte chunk
-    // (2 (jb & 3) + (lane & 3) / 2) ^ r8, 8-byte half lane & 1.  Each warp store covers all 32 banks twice.
     static_assert(NDS % 2 == 1, "consecutive users of a dS^T slot must have different owners");
-    const uint32_t dq_thr = (16 * wl + r8) * 128 + (lane & 1) * 8;
-    const int dq_sx = ((lane & 3) >> 1) ^ r8;
     float s[QT / 2], dp[QT / 2], dq[D / 2];
     uint32_t pf[QT / 4], dsf[QT / 4];
 #pragma unroll
     for (int k = 0; k < D / 2; ++k) dq[k] = 0.f;
-    auto ds_slot = [&](int i) { return sDS + 2 * (i % NDS) * Cfg::kDS; };
-    const Ring<NDQ> dqr = dq_ring(w);
-    auto stage_dq = [&](int i) {              // i & 1 == w
-      const int n = i >> 1;
-      const int sb = dqr.acquire(n);          // the reducer has read the buffer's last tile
-      const uint32_t dst = sDQ + (NDQ * w + sb) * Cfg::kDQ + dq_thr;
-#pragma unroll
-      for (int jb = 0; jb < D / 8; ++jb) {
-        const uint32_t o = dst + (jb >> 2) * (QT * 128) + (((2 * (jb & 3)) ^ dq_sx) << 4);
-        sts64f(o, dq[4 * jb], dq[4 * jb + 1]);
-        sts64f(o + 1024, dq[4 * jb + 2], dq[4 * jb + 3]);
-      }
-      fence_proxy_async_smem();
-      dqr.commit(n);
-    };
     // dQ(i) retired: release its dS^T slot, stage the tile
     auto retire_dq = [&](int i) {
       dsr.release(i);
-      stage_dq(i);
+      stage_dq(dq, i >> 1);
     };
     auto issue_owned_dq = [&](int i) {        // i & 1 == w
       dsr.wait(i);

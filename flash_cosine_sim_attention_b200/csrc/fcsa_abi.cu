@@ -471,9 +471,13 @@ int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream
   // 2. main
   {
     CUtensorMap tq, tk, tv, tdo, tdq;
+    // keys of one work item (BwdCfg::kKeys of the kernel launched below): one K / V box each
+    const bool head_loop = !BIAS && h.H / h.kv_heads / split > 1;
+    const int keys = h.deterministic ? BwdCfg<D, BIAS, false>::kKeys
+                                     : head_loop ? BwdCfg<D, BIAS, true, true>::kKeys : BwdCfg<D, BIAS, true>::kKeys;
     if ((r = map_operand<T, D>(&tq, "q", h.q, tB, h.H, tNq, Cfg::QT)) ||
-        (r = map_operand<T, D>(&tk, "k", h.k, tB, h.kv_heads, tNk, 128)) ||
-        (r = map_operand<T, D>(&tv, "v", h.v, tB, h.kv_heads, tNk, 128)) ||
+        (r = map_operand<T, D>(&tk, "k", h.k, tB, h.kv_heads, tNk, keys)) ||
+        (r = map_operand<T, D>(&tv, "v", h.v, tB, h.kv_heads, tNk, keys)) ||
         (r = map_operand<T, D>(&tdo, "d_o", h.d_o, tB, h.H, tNq, Cfg::QT)))
       return r;
     // the dq accumulator as [B][H][Nq][D] fp32 over its padded rows: boxes of 32 features x QT rows (packed
@@ -503,24 +507,30 @@ int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream
     a.dbias = h.dbias; a.dbias_sb = h.dbias_sb; a.dbias_sh = h.dbias_sh;
     a.out_f32 = h.out_f32 ? 1 : 0;
     a.k_rnorm = h.k_rnorm; a.groups = h.groups;
-    // one CTA per (key tile, batch, kv head, slice of its group); packed sequences: key tiles of the longest one
-    const long long items = (long long)((h.Nk + 127) / 128) * h.B * h.kv_heads * split;
+    // one CTA per (block of `keys` keys, batch, kv head, slice of its group), heaviest blocks first; packed
+    // sequences: key blocks of the longest one
+    const long long items = (long long)((h.Nk + keys - 1) / keys) * h.B * h.kv_heads * split;
     if (items > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
-    const auto launch = [&](auto kern) {
-      return launch_attention<decltype(kern)::value>("backward", g_ev[1], items, Cfg::kThreads, Cfg::kSmem, stream,
+    // (kern, its config)
+    const auto launch = [&](auto kern, auto cfg) {
+      using KCfg = decltype(cfg);
+      return launch_attention<decltype(kern)::value>("backward", g_ev[1], items, KCfg::kThreads, KCfg::kSmem, stream,
                                                      tq, tk, tv, tdo, tdq, a);
     };
     // DQ = false: the dK / dV kernel of the deterministic route
     const auto launch_main = [&](auto dq) {
       constexpr bool DQ = decltype(dq)::value;
       if (a.hpc > 1)   // HEAD_LOOP
-        return a.window > 0 ? launch(kernel_c<fcsa_bwd_kernel<T, D, false, true, VARLEN, true, DQ>>{})
-                            : launch(kernel_c<fcsa_bwd_kernel<T, D, false, true, VARLEN, false, DQ>>{});
-      return a.window > 0 ? launch(kernel_c<fcsa_bwd_kernel<T, D, false, false, VARLEN, true, DQ>>{})
-                          : launch(kernel_c<fcsa_bwd_kernel<T, D, false, false, VARLEN, false, DQ>>{});
+        return a.window > 0 ? launch(kernel_c<fcsa_bwd_kernel<T, D, false, true, VARLEN, true, DQ>>{},
+                                     BwdCfg<D, false, DQ, true>{})
+                            : launch(kernel_c<fcsa_bwd_kernel<T, D, false, true, VARLEN, false, DQ>>{},
+                                     BwdCfg<D, false, DQ, true>{});
+      const BwdCfg<D, false, DQ> cfg;
+      return a.window > 0 ? launch(kernel_c<fcsa_bwd_kernel<T, D, false, false, VARLEN, true, DQ>>{}, cfg)
+                          : launch(kernel_c<fcsa_bwd_kernel<T, D, false, false, VARLEN, false, DQ>>{}, cfg);
     };
     if constexpr (BIAS)   // (one query head per CTA, no window)
-      r = launch(kernel_c<fcsa_bwd_kernel<T, D, true>>{});
+      r = launch(kernel_c<fcsa_bwd_kernel<T, D, true>>{}, BwdCfg<D, true>{});
     else
       r = h.deterministic ? launch_main(std::false_type{}) : launch_main(std::true_type{});
     if (r) return r;

@@ -118,21 +118,40 @@ FCSA_TILE_FN bool tile_visible(int q_first, int q_last, int k_first, int k_last,
 // this one offset for both of a thread's key rows.
 FCSA_TILE_FN int window_hi_off(int off, int W) { return W - 1 - off; }
 
-// The 64-row query tiles [lo, hi) that the 128 keys from key0 are visible to, nqt = ceil(Nq / 64) tiles in all: from
-// the first tile with a row that can see key0 (causal: 64 i + 63 + off >= key0; a non-causal window: whose band
-// reaches key0) to, with a window, the tile of the last query row whose lower limit is at most key0 + 127.
+// The 64-row query tiles [lo, hi) that the `keys` keys from key0 (128: a key tile) are visible to, nqt = ceil(Nq / 64)
+// tiles in all: from the first tile with a row that can see key0 (causal: 64 i + 63 + off >= key0; a non-causal
+// window: whose band reaches key0) to, with a window, the tile of the last query row whose lower limit is at most
+// key0 + keys - 1.
 template <bool WINDOW>
-FCSA_TILE_FN TileRange query_tiles(int key0, int off, int nqt, int causal, int W) {
+FCSA_TILE_FN TileRange query_tiles(int key0, int off, int nqt, int causal, int W, int keys = 128) {
   TileRange t = {0, nqt};
   if (causal || WINDOW) {
     const int x = key0 - off - 63 - (WINDOW && !causal ? W - 1 : 0);
     t.lo = x <= 0 ? 0 : (x + 63) / 64;
   }
   if constexpr (WINDOW) {
-    const int last_row = key0 + 127 - off + W - 1;
+    const int last_row = key0 + keys - 1 - off + W - 1;
     t.hi = last_row < 0 ? 0 : tile_min(nqt, last_row / 64 + 1);
   }
   return t;
+}
+
+// Keys of one backward work item: three consumer warpgroups of 64 keys for the D = 64 kernels that compute dQ without
+// a bias or a head loop (BwdCfg), two for the others.  A head loop runs where the split rule (bwd_group_split) sizes
+// the grid to about fill the device with 128-key CTAs: 192-key items would leave it at 1.33 waves.
+constexpr int bwd_block_keys(int D, bool bias, bool dq, bool head_loop = false) {
+  return D == 64 && !bias && dq && !head_loop ? 192 : 128;
+}
+
+// The query tiles that the existing keys among the `keys` from key0 see, Nk keys in all: a 192-key work item's
+// (keys = 192) or one of its warpgroups' (key0 + 64 w, keys = 64).  Empty when key0 >= Nk.  The warpgroups' ranges
+// tile the item's: a key's visible rows form one interval that moves up by one row per key, so the item's range is the
+// first warpgroup's lower end to the last existing warpgroup's upper end, and a tile between them is some warpgroup's.
+template <bool WINDOW>
+FCSA_TILE_FN TileRange key_block_query_tiles(int key0, int keys, int Nk, int off, int nqt, int causal, int W) {
+  const int n = tile_min(keys, Nk - key0);
+  if (n <= 0) return {0, 0};
+  return query_tiles<WINDOW>(key0, off, nqt, causal, W, n);
 }
 
 // A backward CTA with several query heads works through one flat sequence of hpc * NI tiles, NI = max(0, hi - lo) per
@@ -195,6 +214,8 @@ inline int decode_window_keys(int cap, int window, bool causal) {
 // (no accumulator, no finish pass, bitwise reproducible), but the grid then has B * kv_heads * key tiles CTAs; below
 // one CTA per SM the group is split into the fewest slices that fill the device.  Keys/values shared by all heads
 // (kv_heads == 1) and the BIAS kernels (no registers to spare for the head loop) take one query head per CTA.
+// The rule counts 128-key CTAs for every kernel, so which path a shape takes does not depend on the head dim; a grid of
+// 192-key items that stays unsplit between 2/3 of a wave and one wave still keeps dk / dv in registers.
 inline int bwd_group_split(int B, int H, int kv_heads, int Nk, bool bias, int sm_count) {
   const int G = H / kv_heads;
   if (G == 1) return 1;
