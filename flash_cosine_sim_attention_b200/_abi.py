@@ -42,6 +42,8 @@ EXPORTED_SYMBOLS = (
     "fcsa_f32_cast_backward",
     "fcsa_decode_workspace_bytes",
     "fcsa_decode",
+    "fcsa_decode_varlen_workspace_bytes",
+    "fcsa_decode_varlen",
     "fcsa_forward_fused_varlen",
     "fcsa_backward_fused_varlen_workspace_bytes",
     "fcsa_backward_fused_varlen_zeroed_bytes",
@@ -152,6 +154,11 @@ def load():
     lib.fcsa_decode_workspace_bytes.argtypes = [PP, c_int32]
     lib.fcsa_decode.restype = c_int32
     lib.fcsa_decode.argtypes = [PP, PT, PT, PT, c_void_p, PT, PT, c_int32, c_int32, PT, c_void_p, c_size_t, c_void_p]
+    lib.fcsa_decode_varlen_workspace_bytes.restype = c_size_t
+    lib.fcsa_decode_varlen_workspace_bytes.argtypes = [PP, c_int32]
+    lib.fcsa_decode_varlen.restype = c_int32
+    lib.fcsa_decode_varlen.argtypes = [PP, c_void_p, c_int32, PT, PT, PT, c_void_p, PT, PT, c_int32, PT, c_void_p,
+                                       c_size_t, c_void_p]
     PV = POINTER(FcsaVarlen)
     lib.fcsa_forward_fused_varlen.restype = c_int32
     lib.fcsa_forward_fused_varlen.argtypes = [PP, PV, PT, PT, PT, PN, PT, c_void_p, c_void_p]

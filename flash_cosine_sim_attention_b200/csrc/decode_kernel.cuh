@@ -15,6 +15,10 @@
 //     are cut into n_split contiguous chunks on the device, so a cache allocated at full length costs nothing.
 //   * n_split = 1: o is written directly.  Otherwise each split writes fp32 partials (O_s, l_s) and
 //     decode_combine_kernel forms o = sum_s O_s / max(sum_s l_s, 1e-37) in split order: o is bitwise reproducible.
+//   * packed new tokens (cu_q set): batch element b brings n_b = cu_q[b + 1] - cu_q[b] queries at packed rows
+//     [cu_q[b], cu_q[b + 1]) of q and o (q_sb = o_sb = 0), read on the device after pdl_wait (seq_span).  Nq and R of
+//     the rules above become n_b and R_b = G * n_b; the grid is sized by the maximum (a.Nq), and a row block at or past
+//     R_b has no work.
 #pragma once
 
 #include "key_tile.cuh"
@@ -24,8 +28,10 @@ namespace fcsa {
 struct DecodeArgs {
   int B, H, KVH, G;          // G = H / KVH query heads per kv head
   int Nq, cap, n_new;        // new queries, cache rows (capacity), rows the append pass added at cache_seqlens[b]
+                             // (packed: 1 = each sequence appended its own n_b rows, 0 = none); Nq: packed, the maximum
   int causal;
-  int R, n_rb, n_split;      // R = G * Nq rows per (batch, kv head), in n_rb blocks of 64; key splits
+  int R, n_rb, n_split;      // R = G * Nq rows per (batch, kv head) (packed: of the longest), in n_rb blocks of 64;
+                             // key splits
   float c1;                  // scale * log2(e)
   float c2;                  // shift * log2(e)
   const int32_t* seqlens;    // (B,) valid cache rows before the call
@@ -34,7 +40,20 @@ struct DecodeArgs {
   void* o;
   long long o_sb, o_sh, o_sn;
   float* part;               // n_split > 1: O_s [item][split][64][D], then l_s [item][split][64] (fp32)
+  const int32_t* cu_q;       // packed new tokens: (B + 1,) cumulative counts over q's and o's rows; nullptr = dense
+  int total_q;               // packed: rows of q and o
 };
+
+// The queries of batch element b: dense, the a.Nq rows of q's batch b; packed, the n_b rows of sequence b from packed
+// row `start` (clamped as seq_span does).  The rows of the (batch, kv head) are R = G * Nq.
+struct DecodeRows {
+  int Nq, start;
+};
+__device__ __forceinline__ DecodeRows decode_rows(const DecodeArgs& a, int b) {
+  if (a.cu_q == nullptr) return {a.Nq, 0};
+  const SeqSpan s = seq_span(a.cu_q, b, a.Nq, a.total_q);
+  return {s.len, s.start};
+}
 
 template <int D>
 struct DecodeCfg {
@@ -82,7 +101,6 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
   const int rb = item - bh * a.n_rb;
   const int b = bh / a.KVH, hk = bh - b * a.KVH;
   const int r0 = rb * 64;
-  const int r_last = min(r0 + 63, a.R - 1);
 
   if (threadIdx.x == 0) {
     kr.init(1, 128);
@@ -90,12 +108,18 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
     fence_mbar_init();
   }
   __syncthreads();
-  pdl_wait();          // q (normalised by the append pass), the caches and cache_seqlens are read from here on
+  pdl_wait();          // q (normalised by the append pass), the caches, cache_seqlens and cu_q are read from here on
+
+  // this element's queries: a block past its rows has no work (packed; the combine skips its rows)
+  const DecodeRows qs = decode_rows(a, b);
+  const int R = a.G * qs.Nq;
+  if (r0 >= R) return;
+  const int r_last = min(r0 + 63, R - 1);
 
   // visible keys and this split's key tiles (uniform over the CTA)
   const int L = min(max(a.seqlens[b], 0), a.cap);
-  const int Tb = min(L + a.n_new, a.cap);
-  const int off = diag_off(a.Nq, Tb);
+  const int Tb = min(L + (a.cu_q != nullptr ? (a.n_new ? qs.Nq : 0) : a.n_new), a.cap);
+  const int off = diag_off(qs.Nq, Tb);
   int W = 0;                                  // the window
   if constexpr (WINDOW) W = a.window;
   // the tiles the block's queries r0 / G .. r_last / G see (the forward's rule with Nk = T_b), and this split's chunk
@@ -122,18 +146,19 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
   const int cq = 2 * (lane & 3);
 
   if (j1 > j0) {
-    // Q: row r of the block is query i = r / G of head hk * G + r % G; rows past R are zero.  Every 64-feature
-    // chunk is a 64 x 128-byte SWIZZLE_128B tile (8 KB), the layout a TMA box would leave.
+    // Q: row r of the block is query i = r / G of head hk * G + r % G; rows past R are zero (and not read: packed,
+    // they belong to the next sequence).  Every 64-feature chunk is a 64 x 128-byte SWIZZLE_128B tile (8 KB), the
+    // layout a TMA box would leave.
     constexpr int CH = D / 8;                 // 16-byte pieces per row
+    const T* qb = static_cast<const T*>(a.q) + b * a.q_sb + (long long)qs.start * a.q_sn;
 #pragma unroll
     for (int k = 0; k < 64 * CH / 128; ++k) {
       const int idx = t + 128 * k, row = idx / CH, c = idx - (idx / CH) * CH;
       const int r = r0 + row;
       uint4 v = make_uint4(0, 0, 0, 0);
-      if (r < a.R) {
+      if (r < R) {
         const int i = r / a.G, h = hk * a.G + (r - i * a.G);
-        v = __ldg(reinterpret_cast<const uint4*>(static_cast<const T*>(a.q) + b * a.q_sb + h * a.q_sh +
-                                                 (long long)i * a.q_sn + c * 8));
+        v = __ldg(reinterpret_cast<const uint4*>(qb + h * a.q_sh + (long long)i * a.q_sn + c * 8));
       }
       *reinterpret_cast<uint4*>(smem + Cfg::kOffQ + (c >> 3) * 8192 + sw128_offset(row, c & 7)) = v;
     }
@@ -146,7 +171,7 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) {
     const int r = r0 + row_a + 8 * hf;
-    lim[hf] = r >= a.R ? ColRange{0, -1} : row_key_cols<WINDOW>(r / a.G, off, Tb, a.causal, W);
+    lim[hf] = r >= R ? ColRange{0, -1} : row_key_cols<WINDOW>(r / a.G, off, Tb, a.causal, W);
   }
   const float c1 = a.c1;
 
@@ -188,13 +213,15 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
 #pragma unroll
   for (int hf = 0; hf < 2; ++hf) l[hf] = quad_sum(l[hf]);
   if (a.n_split == 1) {
+    // (the span read again: volatile loads, not kept live through the key loop)
+    const DecodeRows qe = decode_rows(a, b);
+    T* ob = static_cast<T*>(a.o) + b * a.o_sb + (long long)qe.start * a.o_sn;
 #pragma unroll
     for (int hf = 0; hf < 2; ++hf) {
       const int r = r0 + row_a + 8 * hf;
-      if (r >= a.R) continue;
+      if (r >= a.G * qe.Nq) continue;
       const int i = r / a.G, h = hk * a.G + (r - i * a.G);
-      store_row(static_cast<T*>(a.o) + b * a.o_sb + h * a.o_sh + (long long)i * a.o_sn, o, hf, cq,
-                1.0f / fmaxf(l[hf], 1e-37f));
+      store_row(ob + h * a.o_sh + (long long)i * a.o_sn, o, hf, cq, 1.0f / fmaxf(l[hf], 1e-37f));
     }
     return;
   }
@@ -227,19 +254,38 @@ __global__ void __launch_bounds__(256) decode_combine_kernel(const DecodeArgs a)
   const int bh = (int)(item / a.n_rb);
   const int b = bh / a.KVH, hk = bh - b * a.KVH;
   const int r = rb * 64 + row;
-  if (r >= a.R) return;
+  const DecodeRows qs = decode_rows(a, b);
+  if (r >= a.G * qs.Nq) return;
   const float* po = a.part + (item * a.n_split * 64 + row) * D + 4 * qd;
   const float* pl = a.part + n_items * a.n_split * 64 * D + item * a.n_split * 64 + row;
   float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
   float l = 0.f;
-  for (int s = 0; s < a.n_split; ++s) {
+  // the loop is latency-bound (few rows, many splits): eight splits' loads are issued before they are summed, in
+  // split order as one at a time would
+  constexpr int SB = 8;
+  int s = 0;
+  for (; s + SB <= a.n_split; s += SB) {
+    float4 v[SB];
+    float lv[SB];
+#pragma unroll
+    for (int u = 0; u < SB; ++u) {
+      v[u] = *reinterpret_cast<const float4*>(po + (long long)(s + u) * 64 * D);
+      lv[u] = pl[(s + u) * 64];
+    }
+#pragma unroll
+    for (int u = 0; u < SB; ++u) {
+      acc.x += v[u].x; acc.y += v[u].y; acc.z += v[u].z; acc.w += v[u].w;
+      l += lv[u];
+    }
+  }
+  for (; s < a.n_split; ++s) {
     const float4 v = *reinterpret_cast<const float4*>(po + (long long)s * 64 * D);
     acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
     l += pl[s * 64];
   }
   const float inv = 1.0f / fmaxf(l, 1e-37f);
   const int i = r / a.G, h = hk * a.G + (r - i * a.G);
-  T* orow = static_cast<T*>(a.o) + b * a.o_sb + h * a.o_sh + (long long)i * a.o_sn + 4 * qd;
+  T* orow = static_cast<T*>(a.o) + b * a.o_sb + h * a.o_sh + (long long)(qs.start + i) * a.o_sn + 4 * qd;
   *reinterpret_cast<uint2*>(orow) = make_uint2(pack2<T>(acc.x * inv, acc.y * inv), pack2<T>(acc.z * inv, acc.w * inv));
 }
 

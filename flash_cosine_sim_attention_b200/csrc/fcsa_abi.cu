@@ -243,6 +243,15 @@ int check_decode_problem(const fcsa_problem* p, int32_t n_new) {
   return FCSA_OK;
 }
 
+// The problem of a packed decode call: check_decode_problem's with seq_q = max_seqlen_q, and total_q packed rows
+int check_decode_varlen(const fcsa_problem* p, int32_t total_q) {
+  if (p && p->seq_q < 0) return fail(FCSA_ERR_INVALID, "decode varlen: max_seqlen_q (seq_q) %d < 0", p->seq_q);
+  int r;
+  if ((r = check_decode_problem(p, 0))) return r;
+  if (total_q < 0) return fail(FCSA_ERR_INVALID, "decode varlen: total_q %d < 0", total_q);
+  return FCSA_OK;
+}
+
 struct DecodeShape {
   int R, n_rb, n_split;
   long long items;
@@ -263,14 +272,14 @@ int decode_shape(const fcsa_problem* p, DecodeShape* s) {
 
 size_t align16(size_t n) { return (n + 15) & ~size_t(15); }
 
-size_t decode_qhat_bytes(const fcsa_problem* p) {
-  return align16((size_t)p->batch * p->heads * p->seq_q * p->head_dim * 2);
-}
+// q^ of `rows` query rows (batch x seq_q, or the packed total_q)
+size_t decode_qhat_bytes(const fcsa_problem* p, size_t rows) { return align16(rows * p->heads * p->head_dim * 2); }
 
+// cu, total_q: packed new tokens (DecodeArgs::cu_q), nullptr = dense; n_new is then 1 (appended) or 0
 template <typename T, int D>
 int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tensor* q, const fcsa_tensor* kc,
                   const fcsa_tensor* vc, const int32_t* seqlens, int32_t n_new, const fcsa_tensor* o, float* part,
-                  cudaStream_t stream) {
+                  const int32_t* cu, int32_t total_q, cudaStream_t stream) {
   using Cfg = fcsa::DecodeCfg<D>;
   CUtensorMap tk, tv;
   int r;
@@ -290,6 +299,8 @@ int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tenso
   a.q = q->ptr; a.q_sb = q->sb; a.q_sh = q->sh; a.q_sn = q->sn;
   a.o = o->ptr; a.o_sb = o->sb; a.o_sh = o->sh; a.o_sn = o->sn;
   a.part = part;
+  a.cu_q = cu; a.total_q = total_q;
+  if (cu) a.q_sb = a.o_sb = 0;
   const long long grid = sh.items * sh.n_split;
   if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "decode: problem too large for one launch");
   const auto launch = [&](auto kern) {
@@ -841,26 +852,26 @@ int fcsa_l2norm_backward(int32_t dtype, int32_t batch, int32_t heads, int32_t ro
                   "l2norm backward launch");
 }
 
-size_t fcsa_decode_workspace_bytes(const fcsa_problem* p, int32_t n_new) {
-  DecodeShape sh;
-  if (check_decode_problem(p, n_new) || decode_shape(p, &sh)) return 0;
-  return decode_qhat_bytes(p) + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
-}
-
-int fcsa_decode(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k_cache, const fcsa_tensor* v_cache,
-                const int32_t* cache_seqlens, const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t n_new,
-                int32_t groups, const fcsa_tensor* o, void* workspace, size_t workspace_bytes, void* stream) {
+// fcsa_decode and fcsa_decode_varlen: dense, or packed new tokens (cu != nullptr: q, o, k_new, v_new are total_q rows,
+// sequence b owning [cu[b], cu[b + 1]); appending when k_new and v_new are set, n_new unused)
+static int decode_impl(const fcsa_problem* p, const int32_t* cu, int32_t total_q, const fcsa_tensor* q,
+                       const fcsa_tensor* k_cache, const fcsa_tensor* v_cache, const int32_t* cache_seqlens,
+                       const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t n_new, int32_t groups,
+                       const fcsa_tensor* o, void* workspace, size_t workspace_bytes, void* stream) {
   int r;
-  if ((r = check_decode_problem(p, n_new))) return r;
+  const bool append = cu ? (k_new != nullptr || v_new != nullptr) : n_new > 0;
   if ((r = check_tensor(q, "q")) || (r = check_tensor(k_cache, "k_cache")) || (r = check_tensor(v_cache, "v_cache")) ||
       (r = check_tensor(o, "o")))
     return r;
-  if (n_new > 0 && ((r = check_tensor(k_new, "k")) || (r = check_tensor(v_new, "v")))) return r;
-  if (groups != 0 && (r = check_rows(false, p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, groups))) return r;
+  if (append && ((r = check_tensor(k_new, "k")) || (r = check_tensor(v_new, "v")))) return r;
+  if (cu && total_q == 0) return FCSA_OK;
+  // the row pass's shape: the batch's rows, or the packed rows as one batch
+  const int32_t rB = cu ? 1 : p->batch, rN = cu ? total_q : p->seq_q;
+  if (groups != 0 && (r = check_rows(false, p->dtype, rB, p->heads, rN, p->head_dim, groups))) return r;
   if (!cache_seqlens) return fail(FCSA_ERR_INVALID, "cache_seqlens: null");
   DecodeShape sh;
   if ((r = decode_shape(p, &sh))) return r;
-  const size_t qbytes = decode_qhat_bytes(p);
+  const size_t qbytes = decode_qhat_bytes(p, (size_t)rB * rN);
   const size_t need = qbytes + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
   if (!workspace || workspace_bytes < need)
     return fail(FCSA_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need, workspace_bytes);
@@ -868,25 +879,68 @@ int fcsa_decode(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* 
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
 
   // append pass: q_hat to the workspace (groups > 0), then k (normalised when groups > 0) and v into the caches at
-  // row cache_seqlens[b]
-  const int64_t H = p->heads, N = p->seq_q, D = p->head_dim;
+  // row cache_seqlens[b] (packed: the row's sequence b, at cache_seqlens[b] + its row within the sequence)
+  const int64_t H = p->heads, N = rN, D = p->head_dim;
   const fcsa_tensor qhat = {workspace, H * N * D, N * D, D};
-  fcsa::RowArgs a = row_args(p->batch, p->head_dim, groups);
+  fcsa::RowArgs a = row_args(rB, p->head_dim, groups);
+  const int32_t n_app = cu ? total_q : n_new;
   int n = 0;
-  if (groups > 0) a.t[n++] = {p->heads, p->seq_q, *q, qhat, {}, nullptr, nullptr, p->seq_q, 0};
-  if (n_new > 0) {
-    a.t[n++] = {p->kv_heads, n_new, *k_new, *k_cache, {}, nullptr, cache_seqlens, p->seq_k, groups == 0 ? 1 : 0};
-    a.t[n++] = {p->kv_heads, n_new, *v_new, *v_cache, {}, nullptr, cache_seqlens, p->seq_k, 1};
+  if (groups > 0) a.t[n++] = {p->heads, rN, *q, qhat, {}, nullptr, nullptr, rN, 0};
+  if (append) {
+    a.t[n++] = {p->kv_heads, n_app, *k_new, *k_cache, {}, nullptr, cache_seqlens, p->seq_k, groups == 0 ? 1 : 0, cu,
+                p->batch, p->seq_q};
+    a.t[n++] = {p->kv_heads, n_app, *v_new, *v_cache, {}, nullptr, cache_seqlens, p->seq_k, 1, cu, p->batch, p->seq_q};
   }
   if (n > 0 && (r = launched(fcsa::launch_row_append(a, n, p->dtype == FCSA_BF16, s), "append pass launch")))
     return r;
 
   const fcsa_tensor* qa = groups > 0 ? &qhat : q;
   float* part = reinterpret_cast<float*>(static_cast<char*>(workspace) + qbytes);
-  return dispatch(p, [&](auto t, auto d) {
-    return launch_decode<typename decltype(t)::type, decltype(d)::value>(p, sh, qa, k_cache, v_cache, cache_seqlens,
-                                                                         n_new, o, part, s);
+  r = dispatch(p, [&](auto t, auto d) {
+    return launch_decode<typename decltype(t)::type, decltype(d)::value>(
+        p, sh, qa, k_cache, v_cache, cache_seqlens, cu ? (append ? 1 : 0) : n_new, o, part, cu, total_q, s);
   });
+  if (r || !cu) return r;
+  // o = 0 in the rows outside every sequence
+  fcsa::TailArgs ta = {};
+  ta.t[0] = {o->ptr, o->sh, o->sn, p->heads, total_q, cu};
+  return launch_varlen_tail(p, ta, 1, s);
+}
+
+size_t fcsa_decode_workspace_bytes(const fcsa_problem* p, int32_t n_new) {
+  DecodeShape sh;
+  if (check_decode_problem(p, n_new) || decode_shape(p, &sh)) return 0;
+  return decode_qhat_bytes(p, (size_t)p->batch * p->seq_q) + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
+}
+
+int fcsa_decode(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k_cache, const fcsa_tensor* v_cache,
+                const int32_t* cache_seqlens, const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t n_new,
+                int32_t groups, const fcsa_tensor* o, void* workspace, size_t workspace_bytes, void* stream) {
+  int r;
+  if ((r = check_decode_problem(p, n_new))) return r;
+  return decode_impl(p, nullptr, 0, q, k_cache, v_cache, cache_seqlens, k_new, v_new, n_new, groups, o, workspace,
+                     workspace_bytes, stream);
+}
+
+size_t fcsa_decode_varlen_workspace_bytes(const fcsa_problem* p, int32_t total_q) {
+  DecodeShape sh;
+  if (check_decode_varlen(p, total_q) || decode_shape(p, &sh)) return 0;
+  return decode_qhat_bytes(p, (size_t)total_q) + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
+}
+
+int fcsa_decode_varlen(const fcsa_problem* p, const int32_t* cu_seqlens_q, int32_t total_q, const fcsa_tensor* q,
+                       const fcsa_tensor* k_cache, const fcsa_tensor* v_cache, const int32_t* cache_seqlens,
+                       const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t groups, const fcsa_tensor* o,
+                       void* workspace, size_t workspace_bytes, void* stream) {
+  int r;
+  if ((r = check_decode_varlen(p, total_q))) return r;
+  if (!cu_seqlens_q) return fail(FCSA_ERR_INVALID, "decode varlen: null cu_seqlens_q");
+  if (reinterpret_cast<uintptr_t>(cu_seqlens_q) & 3)
+    return fail(FCSA_ERR_INVALID, "decode varlen: cu_seqlens_q must be a 4-byte aligned int32 array");
+  if ((k_new == nullptr) != (v_new == nullptr))
+    return fail(FCSA_ERR_INVALID, "decode varlen: pass both k_new and v_new, or neither");
+  return decode_impl(p, cu_seqlens_q, total_q, q, k_cache, v_cache, cache_seqlens, k_new, v_new, 0, groups, o,
+                     workspace, workspace_bytes, stream);
 }
 
 int fcsa_forward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_tensor* q, const fcsa_tensor* k,

@@ -33,6 +33,11 @@ struct RowTensor {
   const int32_t* row0;            // device (B,): row n of x goes to row row0[b] + n of y; nullptr = row n
   int rows_y;                     // rows of y: a destination row outside [0, rows_y) is not written
   int raw;                        // 1: y = x, no l2norm whatever G (the values)
+  // packed sequences (with row0): x is one batch of N packed rows, sequence s owns rows [cu[s], cu[s + 1]) (clamped as
+  // seq_span does, at most max_n rows) and its row n goes to row row0[s] + n - cu[s] of y's batch s; rows outside
+  // every sequence are not written.  nullptr = row n of batch b goes to row row0[b] + n of y's batch b.
+  const int32_t* cu;
+  int n_seq, max_n;               // sequences (cu has n_seq + 1 entries), the longest
 };
 
 struct RowArgs {
@@ -41,6 +46,23 @@ struct RowArgs {
   int mul_reciprocal;             // 1: use 1 / *mul
   RowTensor t[3];                 // forward: one to three tensors (t[i].H = 0 ends the list); backward: t[0]
 };
+
+// The sequence s of packed row n (cu[s] <= n < cu[s + 1], with seq_span's clamp to max_n rows and [0, total)) and
+// its first row, or s = -1 for a row outside every sequence: a binary search over the n_seq + 1 entries.
+__device__ __forceinline__ int row_sequence(const int32_t* cu, int n_seq, int max_n, int total, int n, int* start) {
+  int lo = 0, hi = n_seq;                             // the last s in [0, n_seq] with cu[s] <= n
+  if (ld_cu(cu) > n) return -1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (ld_cu(cu + mid) <= n) lo = mid;
+    else hi = mid - 1;
+  }
+  if (lo == n_seq) return -1;
+  const SeqSpan sp = seq_span(cu, lo, max_n, total);
+  if (n < sp.start || n - sp.start >= sp.len) return -1;
+  *start = sp.start;
+  return lo;
+}
 
 // 1 / max(sqrt(ss), 1e-12)  (py:38-55: F.normalize's eps) = min(rsqrt(ss), 1e12): one MUFU.RSQ instead of an
 // IEEE sqrt + divide (~60 instructions per row and thread in a pass that must stay HBM-bound); the
@@ -242,7 +264,8 @@ __device__ __forceinline__ float row_mul(const RowArgs& a) {
 // issues its loads of all U rows before the first reduction; TPR = threads per row (D / 16) when known at compile
 // time (4 or 8), 0 = read it from the arguments.  x is read with coherent loads: it may alias y.  The 16-bit passes
 // keep four blocks per SM (at most 64 registers).  APPEND (16-bit only): grid.y runs over up to three tensors, each
-// row lands at the per-batch offset row0[b] (rows falling outside y are skipped) and `raw` tensors are copied.
+// row lands at the per-batch offset row0[b] (rows falling outside y are skipped) and `raw` tensors are copied; with
+// packed sequences (RowTensor::cu) at the offset of the row's sequence.
 template <typename T, typename X, int TPR, int U, bool APPEND = false>
 __global__ void __launch_bounds__(256, 8 / sizeof(X)) row_fwd_kernel(const RowArgs a) {
   // SIXTEEN features per thread: the pass is issue-bound before it is memory-bound (ncu: 84 % issue-slot
@@ -267,15 +290,29 @@ __global__ void __launch_bounds__(256, 8 / sizeof(X)) row_fwd_kernel(const RowAr
     const int row = row0 + u * rpp;
     const int bh = row / t.N, n = row - bh * t.N, b = bh / t.H, h = bh - b * t.H;
     const X* xp = static_cast<const X*>(t.x.ptr) + b * t.x.sb + h * t.x.sh + (long long)n * t.x.sn + tr * 16;
-    if constexpr (APPEND) {
-      long long ny = n;
-      if (t.row0 != nullptr && row < rows) ny += t.row0[b];
-      yoff[u] = (ny >= 0 && ny < t.rows_y) ? b * t.y.sb + h * t.y.sh + ny * t.y.sn + tr * 16 : -1;
-    } else {
-      yoff[u] = b * t.y.sb + h * t.y.sh + (long long)n * t.y.sn + tr * 16;
-    }
+    if constexpr (!APPEND) yoff[u] = b * t.y.sb + h * t.y.sh + (long long)n * t.y.sn + tr * 16;
 #pragma unroll
     for (int v = 0; v < 16 / E; ++v) raw[u][v] = row < rows ? ld_stream128(xp + v * E) : make_uint4(0, 0, 0, 0);
+  }
+  if constexpr (APPEND) {
+    // the destinations, while the loads are in flight (the sequence search of packed rows is a loop of its own)
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int row = row0 + u * rpp;
+      const int bh = row / t.N, n = row - bh * t.N, b = bh / t.H, h = bh - b * t.H;
+      long long ny = n;
+      int yb = b;
+      if (t.row0 != nullptr && row < rows) {
+        if (t.cu != nullptr) {
+          int start = 0;
+          yb = row_sequence(t.cu, t.n_seq, t.max_n, t.N, n, &start);
+          ny = yb < 0 ? -1 : (long long)t.row0[yb] + n - start;
+        } else {
+          ny += t.row0[b];
+        }
+      }
+      yoff[u] = (ny >= 0 && ny < t.rows_y) ? yb * t.y.sb + h * t.y.sh + ny * t.y.sn + tr * 16 : -1;
+    }
   }
 #pragma unroll
   for (int u = 0; u < U; ++u) {

@@ -64,6 +64,14 @@ fcsa_tensor view4(const Tensor& t) {
   return v;
 }
 
+// (total, heads, feature) -> the (batch, head, row) addressing of the ABI: one batch, rows = the packed rows
+fcsa_tensor view_packed(const Tensor& t) {
+  fcsa_tensor v;
+  v.ptr = t.data_ptr();
+  v.sb = 0; v.sh = t.stride(1); v.sn = t.stride(0);
+  return v;
+}
+
 // shape canonicalisation of the reference's host op (cu:1647-1660, cu:1679)
 struct Shapes {
   bool merged;
@@ -445,20 +453,26 @@ std::tuple<Tensor, Tensor, Tensor, optional<Tensor>> backward(
 //   are (no copy); cache_seqlens int32 on q's device; k, v (B, kv_heads, n_new, D) or both None; groups > 0:
 //   l2-normalise q and k over that many groups.  Returns o (B, H, Nq, D).  Scratch comes from the per-(device,
 //   stream) workspace of the backward, whose contents are irrelevant on entry.
+// decode_varlen: the same with packed new tokens (fcsa_decode_varlen): q (total_q, H, D), k, v (total_q, kv_heads, D)
+//   or both None, cu_seqlens_q int32 (B + 1,) on q's device, max_q >= every length.  Returns o (total_q, H, D).
 // ------------------------------------------------------------------------------------------------
-Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
-              const optional<Tensor>& k_in, const optional<Tensor>& v_in, double scale, double shift, bool causal,
-              int64_t groups, int64_t window) {
-  TORCH_CHECK(q_in.dim() == 4 && k_cache.dim() == 4 && v_cache.dim() == 4,
-              "decode: q, k_cache, v_cache must be (batch, heads, seq, head_dim)");
+// The checks both share: q's rank (3 packed, 4 dense) and dtype, the caches, cache_seqlens, and k / v, whose leading
+// `rows` dimensions must match q's (B for dense, total_q packed).  Returns k, v made TMA-ready (undefined when absent).
+std::tuple<Tensor, Tensor> decode_checks(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache,
+                                         const Tensor& cache_seqlens, const optional<Tensor>& k_in,
+                                         const optional<Tensor>& v_in, bool packed) {
+  const int64_t qdim = packed ? 3 : 4;
+  TORCH_CHECK(q_in.dim() == qdim && k_cache.dim() == 4 && v_cache.dim() == 4,
+              packed ? "decode_varlen: q must be (total_q, heads, head_dim) and k_cache, v_cache (batch, kv_heads, "
+                       "capacity, head_dim)"
+                     : "decode: q, k_cache, v_cache must be (batch, heads, seq, head_dim)");
   TORCH_CHECK(q_in.is_cuda() && k_cache.is_cuda() && v_cache.is_cuda(), "decode: CUDA tensors required");
   TORCH_CHECK(k_cache.scalar_type() == q_in.scalar_type() && v_cache.scalar_type() == q_in.scalar_type(),
               "decode: q and the caches must share one dtype");
   TORCH_CHECK(k_cache.sizes() == v_cache.sizes(), "decode: k_cache and v_cache must have the same shape");
-  const int64_t B = q_in.size(0), H = q_in.size(1), Nq = q_in.size(2), D = q_in.size(3);
-  const int64_t Hk = k_cache.size(1), cap = k_cache.size(2);
-  TORCH_CHECK(k_cache.size(0) == B && k_cache.size(3) == D, "decode: caches must be (", B, ", kv_heads, capacity, ", D,
-              ")");
+  const int64_t B = k_cache.size(0), H = q_in.size(1), D = q_in.size(qdim - 1), Hk = k_cache.size(1);
+  TORCH_CHECK((packed || q_in.size(0) == B) && k_cache.size(3) == D, "decode: caches must be (",
+              packed ? B : q_in.size(0), ", kv_heads, capacity, ", D, ")");
   TORCH_CHECK(Hk > 0 && H % Hk == 0, "decode: kv_heads (", Hk, ") must divide the query heads (", H, ")");
   TORCH_CHECK(cache_seqlens.is_cuda() && cache_seqlens.get_device() == q_in.get_device() &&
                   cache_seqlens.scalar_type() == at::kInt && cache_seqlens.dim() == 1 && cache_seqlens.size(0) == B,
@@ -471,19 +485,30 @@ Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, 
               "16-byte aligned base and strides, no expanded dimension");
   const bool has_new = k_in.has_value() && k_in->defined();
   TORCH_CHECK(has_new == (v_in.has_value() && v_in->defined()), "decode: pass both k and v, or neither");
-  int64_t n_new = 0;
   Tensor k, v;
   if (has_new) {
-    TORCH_CHECK(k_in->dim() == 4 && k_in->sizes() == v_in->sizes() && k_in->size(0) == B && k_in->size(1) == Hk &&
-                    k_in->size(3) == D,
-                "decode: k and v must be (", B, ", ", Hk, ", n_new, ", D, ")");
+    const int64_t rows = q_in.size(0);
+    TORCH_CHECK(k_in->dim() == qdim && k_in->sizes() == v_in->sizes() && k_in->size(0) == rows &&
+                    k_in->size(1) == Hk && k_in->size(qdim - 1) == D,
+                packed ? "decode_varlen: k and v must be (total_q, kv_heads, head_dim) = (" : "decode: k and v must be (",
+                rows, ", ", Hk, packed ? "" : ", n_new", ", ", D, ")");
     TORCH_CHECK(k_in->scalar_type() == q_in.scalar_type() && v_in->scalar_type() == q_in.scalar_type() &&
                     k_in->is_cuda() && v_in->is_cuda(),
                 "decode: k and v must be CUDA tensors of q's dtype");
     k = tma_ready(*k_in);
     v = tma_ready(*v_in);
-    n_new = k.size(2);
   }
+  return {k, v};
+}
+
+Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
+              const optional<Tensor>& k_in, const optional<Tensor>& v_in, double scale, double shift, bool causal,
+              int64_t groups, int64_t window) {
+  Tensor k, v;
+  std::tie(k, v) = decode_checks(q_in, k_cache, v_cache, cache_seqlens, k_in, v_in, false);
+  const int64_t B = q_in.size(0), H = q_in.size(1), Nq = q_in.size(2), D = q_in.size(3);
+  const int64_t Hk = k_cache.size(1), cap = k_cache.size(2);
+  const int64_t n_new = k.defined() ? k.size(2) : 0;
   const c10::cuda::CUDAGuard guard(q_in.device());
   const Tensor q = tma_ready(q_in);
   const fcsa_problem p =
@@ -494,9 +519,41 @@ Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, 
       workspaces_of_size(fcsa_decode_workspace_bytes(&p, (int32_t)n_new), 0, q, stream, false).scratch;
   const fcsa_tensor tq = view4(q), tkc = view4(k_cache), tvc = view4(v_cache), to = view4(o);
   fcsa_tensor tk = {nullptr, 0, 0, 0}, tv = {nullptr, 0, 0, 0};
-  if (has_new) { tk = view4(k); tv = view4(v); }
+  if (k.defined()) { tk = view4(k); tv = view4(v); }
   FCSA_CHECK(fcsa_decode(&p, &tq, &tkc, &tvc, cache_seqlens.data_ptr<int32_t>(), &tk, &tv, (int32_t)n_new,
                          (int32_t)groups, &to, scratch.data_ptr(), (size_t)scratch.numel(), stream));
+  return o;
+}
+
+Tensor decode_varlen(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
+                     const Tensor& cu_q, int64_t max_q, const optional<Tensor>& k_in, const optional<Tensor>& v_in,
+                     double scale, double shift, bool causal, int64_t groups, int64_t window) {
+  Tensor k, v;
+  std::tie(k, v) = decode_checks(q_in, k_cache, v_cache, cache_seqlens, k_in, v_in, true);
+  const int64_t B = k_cache.size(0), H = q_in.size(1), Tq = q_in.size(0), D = q_in.size(2);
+  const int64_t Hk = k_cache.size(1), cap = k_cache.size(2);
+  TORCH_CHECK(cu_q.is_cuda() && cu_q.get_device() == q_in.get_device() && cu_q.scalar_type() == at::kInt &&
+                  cu_q.dim() == 1 && cu_q.size(0) == B + 1,
+              "decode_varlen: cu_seqlens_q must be an int32 tensor of shape (", B + 1, ",) on q's device");
+  TORCH_CHECK(cu_q.is_contiguous(), "decode_varlen: cu_seqlens_q must be contiguous (not a strided or expanded view)");
+  TORCH_CHECK(max_q >= 1 && max_q <= 0x7FFFFFFF, "decode_varlen: max_seqlen_q must be a positive int32 value");
+  TORCH_CHECK(Tq <= 0x7FFFFFFF, "decode_varlen: too many packed rows");
+  const c10::cuda::CUDAGuard guard(q_in.device());
+  const Tensor q = tma_ready(q_in);
+  const fcsa_problem p =
+      build_problem("decode: ", q, B, H, Hk, max_q, cap, D, scale, shift, causal, c10::nullopt, false, window);
+  Tensor o = at::empty({Tq, H, D}, q.options());
+  if (Tq == 0) return o;
+  cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
+  const Tensor scratch =
+      workspaces_of_size(fcsa_decode_varlen_workspace_bytes(&p, (int32_t)Tq), 0, q, stream, false).scratch;
+  const fcsa_tensor tq = view_packed(q), tkc = view4(k_cache), tvc = view4(v_cache), to = view_packed(o);
+  fcsa_tensor tk, tv;
+  if (k.defined()) { tk = view_packed(k); tv = view_packed(v); }
+  FCSA_CHECK(fcsa_decode_varlen(&p, cu_q.data_ptr<int32_t>(), (int32_t)Tq, &tq, &tkc, &tvc,
+                                cache_seqlens.data_ptr<int32_t>(), k.defined() ? &tk : nullptr,
+                                k.defined() ? &tv : nullptr, (int32_t)groups, &to, scratch.data_ptr(),
+                                (size_t)scratch.numel(), stream));
   return o;
 }
 
@@ -505,14 +562,6 @@ Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, 
 //   q (total_q, H, D), k, v (total_k, kv_heads, D); cu_q, cu_k int32 (B + 1) on q's device, read by the kernels
 //   only (never copied: a CUDA graph replay must read the caller's buffers); max_q, max_k >= every length.
 // ------------------------------------------------------------------------------------------------
-// (total, heads, feature) -> the (batch, head, row) addressing of the ABI: one batch, rows = the packed rows
-fcsa_tensor view_packed(const Tensor& t) {
-  fcsa_tensor v;
-  v.ptr = t.data_ptr();
-  v.sb = 0; v.sh = t.stride(1); v.sn = t.stride(0);
-  return v;
-}
-
 struct Varlen {
   fcsa_problem p;
   fcsa_varlen vl;
@@ -683,6 +732,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("decode", &decode, "new queries against a key/value cache, appending k / v at cache_seqlens", py::arg("q"),
         py::arg("k_cache"), py::arg("v_cache"), py::arg("cache_seqlens"), py::arg("k"), py::arg("v"), py::arg("scale"),
         py::arg("shift"), py::arg("causal"), py::arg("groups"), py::arg("window") = 0);
+  m.def("decode_varlen", &decode_varlen, "decode with a different number of new tokens per sequence (packed q, k, v)",
+        py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cache_seqlens"), py::arg("cu_q"),
+        py::arg("max_q"), py::arg("k"), py::arg("v"), py::arg("scale"), py::arg("shift"), py::arg("causal"),
+        py::arg("groups"), py::arg("window") = 0);
   m.def("release_workspaces", &release_workspaces, "free the cached backward workspaces; returns the bytes released");
   m.def("abi_version", []() { return fcsa_version(); });
   m.def("_error_path_selftest", []() { FCSA_CHECK(fcsa_forward(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr)); },

@@ -650,14 +650,20 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
                                           window, deterministic)
 
 
-def _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias):
-    """Everything flash_cosine_sim_attention_with_kv_cache rejects before touching a device."""
+def _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias, cu_seqlens_q=None,
+                         max_seqlen_q=None):
+    """Everything flash_cosine_sim_attention_with_kv_cache rejects before touching a device.  With cu_seqlens_q, q, k
+    and v are packed: (total_q, heads, head_dim) and (total_q, kv_heads, head_dim)."""
+    packed = cu_seqlens_q is not None
     if exists(attn_bias):
         raise NotImplementedError("flash_cosine_sim_attention_with_kv_cache: attn_bias is not supported")
     if exists(mask):
         raise NotImplementedError("flash_cosine_sim_attention_with_kv_cache: no key-padding mask - cache_seqlens "
                                   "gives each batch element's valid cache rows")
-    if q.ndim != 4 or k_cache.ndim != 4 or v_cache.ndim != 4:
+    if packed and (q.ndim != 3 or k_cache.ndim != 4 or v_cache.ndim != 4):
+        raise ValueError("flash_cosine_sim_attention_with_kv_cache: with cu_seqlens_q, q must be packed as (total_q, "
+                         "heads, head_dim) and the caches (batch, kv_heads, capacity, head_dim)")
+    if q.ndim != (3 if packed else 4) or k_cache.ndim != 4 or v_cache.ndim != 4:
         raise ValueError("flash_cosine_sim_attention_with_kv_cache: q must be (batch, heads, seq, head_dim) and the "
                          "caches (batch, kv_heads, capacity, head_dim); merged batch-heads are not supported")
     if exists(k) != exists(v):
@@ -675,34 +681,64 @@ def _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask,
     D = q.shape[-1]
     if D not in _KERNEL_HEAD_DIMS:
         raise NotImplementedError(f"flash_cosine_sim_attention_with_kv_cache: head_dim {D} (64 and 128 only)")
-    if k_cache.shape != v_cache.shape or k_cache.shape[0] != q.shape[0] or k_cache.shape[-1] != D:
+    if k_cache.shape != v_cache.shape or (not packed and k_cache.shape[0] != q.shape[0]) or k_cache.shape[-1] != D:
         raise ValueError(f"flash_cosine_sim_attention_with_kv_cache: caches of shape {tuple(k_cache.shape)} and "
                          f"{tuple(v_cache.shape)} do not match q {tuple(q.shape)}")
     hk = k_cache.shape[1]
     if hk <= 0 or q.shape[1] % hk != 0:
         raise ValueError(f"flash_cosine_sim_attention_with_kv_cache: kv_heads ({hk}) must divide the query heads "
                          f"({q.shape[1]})")
-    if exists(k) and (k.shape != v.shape or k.ndim != 4 or k.shape[:2] != k_cache.shape[:2] or k.shape[-1] != D):
+    if packed and exists(k) and (k.shape != v.shape or k.shape != (q.shape[0], hk, D)):
+        raise ValueError(f"flash_cosine_sim_attention_with_kv_cache: k and v must be packed like q, (total_q, kv_heads, "
+                         f"head_dim) = {(q.shape[0], hk, D)} (got {tuple(k.shape)} and {tuple(v.shape)})")
+    if not packed and exists(k) and (k.shape != v.shape or k.ndim != 4 or k.shape[:2] != k_cache.shape[:2]
+                                     or k.shape[-1] != D):
         raise ValueError(f"flash_cosine_sim_attention_with_kv_cache: k and v must be (batch, kv_heads, n_new, {D}) "
                          f"like the caches (got {tuple(k.shape)} and {tuple(v.shape)})")
-    if not torch.is_tensor(cache_seqlens) or cache_seqlens.dtype != torch.int32 or cache_seqlens.shape != (q.shape[0],):
+    B = k_cache.shape[0]
+    if not torch.is_tensor(cache_seqlens) or cache_seqlens.dtype != torch.int32 or cache_seqlens.shape != (B,):
         raise TypeError("flash_cosine_sim_attention_with_kv_cache: cache_seqlens must be an int32 tensor of shape "
-                        f"({q.shape[0]},)")
+                        f"({B},)")
     if not cache_seqlens.is_contiguous():
         raise ValueError("flash_cosine_sim_attention_with_kv_cache: cache_seqlens must be contiguous (the kernels read "
                          "it as a dense array and a CUDA graph replay reads the caller's buffer; not a strided or "
                          "expanded view)")
+    if packed:
+        _check_cu_seqlens_q(q, B, cu_seqlens_q, max_seqlen_q)
+    elif max_seqlen_q is not None:
+        raise ValueError("flash_cosine_sim_attention_with_kv_cache: max_seqlen_q is for packed new tokens - pass "
+                         "cu_seqlens_q with it")
     gs = D // groups if groups > 0 and D % groups == 0 else 0
     if gs == 0 or (gs & (gs - 1)) != 0:
         raise ValueError(f"flash_cosine_sim_attention_with_kv_cache: groups {groups} must divide head_dim {D} into "
                          "power-of-two chunks")
-    if not (q.is_cuda and cache_seqlens.is_cuda):
-        raise RuntimeError("flash_cosine_sim_attention_with_kv_cache: CUDA tensors required (cache_seqlens included: "
-                           "the host never reads it) - this build has no CPU path")
+    if not (q.is_cuda and cache_seqlens.is_cuda and (not packed or cu_seqlens_q.is_cuda)):
+        raise RuntimeError("flash_cosine_sim_attention_with_kv_cache: CUDA tensors required (cache_seqlens and "
+                           "cu_seqlens_q included: the host never reads them) - this build has no CPU path")
+
+
+def _check_cu_seqlens_q(q, B, cu_seqlens_q, max_seqlen_q):
+    """The packed new tokens of flash_cosine_sim_attention_with_kv_cache: cu_seqlens_q (B + 1,) and max_seqlen_q."""
+    name = "flash_cosine_sim_attention_with_kv_cache"
+    if not torch.is_tensor(cu_seqlens_q) or cu_seqlens_q.dtype != torch.int32 or cu_seqlens_q.ndim != 1:
+        raise TypeError(f"{name}: cu_seqlens_q must be an int32 tensor of shape (batch + 1,) = ({B + 1},)")
+    if cu_seqlens_q.shape[0] != B + 1:
+        raise ValueError(f"{name}: cu_seqlens_q has {cu_seqlens_q.shape[0]} entries; the caches' batch {B} needs "
+                         f"{B + 1}")
+    if not cu_seqlens_q.is_contiguous():
+        raise ValueError(f"{name}: cu_seqlens_q must be contiguous (the kernels read it as a dense array and a CUDA "
+                         "graph replay reads the caller's buffer; not a strided or expanded view)")
+    if cu_seqlens_q.device != q.device:
+        raise RuntimeError(f"{name}: cu_seqlens_q must be on q's device ({q.device}, got {cu_seqlens_q.device}); the "
+                           "host never reads it")
+    if isinstance(max_seqlen_q, bool) or not isinstance(max_seqlen_q, int) or max_seqlen_q < 0:
+        raise TypeError(f"{name}: max_seqlen_q must be a non-negative Python int with cu_seqlens_q (got "
+                        f"{max_seqlen_q!r})")
 
 
 def flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens, k=None, v=None, scale=8, groups=1,
-                                             causal=True, l2norm_qk=True, mask=None, attn_bias=None, window=None):
+                                             causal=True, l2norm_qk=True, mask=None, attn_bias=None, window=None,
+                                             cu_seqlens_q=None, max_seqlen_q=None):
     """Cosine-sim attention of new queries against a key/value cache, for inference (generation).
 
     q: (batch, heads, n_q, head_dim) new queries.  k_cache, v_cache: (batch, kv_heads, capacity, head_dim), kv_heads
@@ -721,13 +757,30 @@ def flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens,
     capacity.  float16 / bfloat16 and head dims 64 and 128 only; no autograd, attn_bias, mask, float32 or merged
     batch-heads.  window: sliding-window attention as in flash_cosine_sim_attention with n_k = T_b; a step then reads
     the tiles of its window, not the whole valid cache (the cache itself stays full-length).
-    Returns o (batch, heads, n_q, head_dim)."""
+    Returns o (batch, heads, n_q, head_dim).
+
+    A different number of new tokens per batch element (speculative verification, chunked prefill, ragged prompts):
+    cu_seqlens_q, a contiguous int32 CUDA tensor (batch + 1,), non-decreasing, and max_seqlen_q, a Python int at least
+    every length (it sizes the grid; longer sequences are clamped to it).  q is then packed as (total_q, heads,
+    head_dim) and k, v (optional) as (total_q, kv_heads, head_dim) with the same boundaries: batch element b brings
+    n_b = cu_seqlens_q[b + 1] - cu_seqlens_q[b] new tokens at rows [cu_seqlens_q[b], cu_seqlens_q[b + 1]) and appends
+    its k, v rows at cache rows [L_b, L_b + n_b).  Without k, v nothing is appended and n_b counts queries only.  The
+    rules above hold per element with n_q = n_b and T_b = min(L_b + (n_b if appending, else 0), capacity).  Rows
+    outside every sequence ([0, cu_seqlens_q[0]) and [cu_seqlens_q[-1], total_q)) give 0.  cu_seqlens_q is never read
+    on the host either, and cache_seqlens is not advanced: add cu_seqlens_q[1:] - cu_seqlens_q[:-1] afterwards.
+    Returns o (total_q, heads, head_dim)."""
     window = _check_window(window, attn_bias, "flash_cosine_sim_attention_with_kv_cache")
-    _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias)
+    _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias, cu_seqlens_q, max_seqlen_q)
     _warn_fp16_overflow(q.dtype, scale, groups, l2norm_qk)
     shift = _choose_shift(q.dtype, scale, groups, l2norm_qk)
-    return _ext().decode(q, k_cache, v_cache, cache_seqlens, k, v, float(scale), float(shift), bool(causal),
-                         int(groups) if l2norm_qk else 0, window)
+    g = int(groups) if l2norm_qk else 0
+    if cu_seqlens_q is None:
+        return _ext().decode(q, k_cache, v_cache, cache_seqlens, k, v, float(scale), float(shift), bool(causal), g,
+                             window)
+    if q.shape[0] == 0:
+        return q.new_empty(q.shape)
+    return _ext().decode_varlen(q, k_cache, v_cache, cache_seqlens, cu_seqlens_q, max(int(max_seqlen_q), 1), k, v,
+                                float(scale), float(shift), bool(causal), g, window)
 
 
 class _FusedVarlenAttention(Function):

@@ -300,6 +300,31 @@ int fcsa_decode(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* 
                 const int32_t* cache_seqlens, const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t n_new,
                 int32_t groups, const fcsa_tensor* o, void* workspace, size_t workspace_bytes, void* stream);
 
+/* Packed decode: a different number of new tokens per batch element (speculative verification, chunked prefill,
+ * ragged prompts), in one call of the same kernels.  Arguments as fcsa_decode's, except:
+ *   p              : seq_q = max_seqlen_q, at least every n_b (it sizes the grid and the key splits; larger lengths are
+ *                    clamped to it).  batch = B, the cache's batch.
+ *   cu_seqlens_q   : DEVICE int32 (B + 1,), non-decreasing, never read by the host.  Batch element b brings the
+ *                    n_b = cu[b + 1] - cu[b] new tokens at packed rows [cu[b], cu[b + 1]).
+ *   total_q        : rows of the packed tensors (0: nothing is launched)
+ *   q, o           : (total_q, heads, head_dim) as fcsa_tensor with sh, sn set (sb unused)
+ *   k_new, v_new   : (total_q, kv_heads, head_dim), packed with the same boundaries, or both NULL (nothing appended).
+ *                    Row cu[b] + n goes to cache row L_b + n of batch element b; rows at or past the capacity and
+ *                    rows outside every sequence are not written.
+ * T_b = min(L_b + (n_b if appending, else 0), capacity); query i of element b sees key j iff j < T_b and, causal,
+ * j <= i + T_b - n_b (fcsa_decode's rule per element; the window likewise).  Rows with no visible key give o = 0, and
+ * so do the rows outside every sequence ([0, cu[0]) and [cu[B], total_q)).  Launches: the append pass, the decode
+ * kernel, the combine kernel when the keys are split, and the pass that zeroes the rows outside every sequence.  With
+ * cu = (0, n, 2n, ...) and seq_q = n, o and the caches are bitwise fcsa_decode's on the same data.  `workspace`:
+ * fcsa_decode_varlen_workspace_bytes(p, total_q) bytes of scratch (0 for a problem it rejects).  Rejected: a null
+ * cu_seqlens_q, total_q < 0, seq_q < 0, a key mask or out_f32.
+ */
+size_t fcsa_decode_varlen_workspace_bytes(const fcsa_problem* p, int32_t total_q);
+int fcsa_decode_varlen(const fcsa_problem* p, const int32_t* cu_seqlens_q, int32_t total_q, const fcsa_tensor* q,
+                       const fcsa_tensor* k_cache, const fcsa_tensor* v_cache, const int32_t* cache_seqlens,
+                       const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t groups, const fcsa_tensor* o,
+                       void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- packed variable-length sequences (no reference counterpart) ------------------------------------------------------
  * Training attention over B sequences of different lengths packed along the row dimension, without padding:
  *   p              : batch = B (sequences), seq_q / seq_k = maximum lengths (they size the grids and clamp the device
