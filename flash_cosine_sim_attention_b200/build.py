@@ -20,6 +20,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 ROOT = os.path.dirname(HERE)
 LIB = os.path.join(HERE, "libfcsa_b200.so")
+# the command line and the compiler output of the last library build: -Xptxas -v gives every kernel's registers and
+# spills, and ptxas notes there when it serialises a kernel's wgmmas (tests/test_ptxas_log.py reads it)
+LOG = os.path.join(HERE, "build.log")
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -123,7 +126,7 @@ def build_library(force=False, verbose=False):
     cmd = [_nvcc()] + NVCC_FLAGS + ["-o", LIB] + _sources()
     proc = subprocess.run(cmd, capture_output=True, text=True)
     log = proc.stdout + proc.stderr
-    with open(os.path.join(HERE, "build.log"), "w") as f:
+    with open(LOG, "w") as f:
         f.write(" ".join(cmd) + "\n" + log)
     if proc.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + log[-8000:])

@@ -317,6 +317,9 @@ __device__ __forceinline__ float4 ldg_cg128f(const float* p) {
   return v;
 }
 
+// What one elementwise pass of fcsa_bwd_kernel computes: P^T, dS^T (from the P^T of a kPassP pass), or both
+enum BwdPass : int { kPassP = 1, kPassDS = 2, kPassBoth = kPassP | kPassDS };
+
 // HEAD_LOOP: the CTA works through several query heads (hpc > 1, grouped-query launches); otherwise hpc = 1 is a
 // compile-time constant and the loops below are those of one query head (MHA, MQA, BIAS and split groups of one head).
 // VARLEN: packed sequences (BwdVarlenArgs); `b` is then the sequence, and its lengths replace Nq / Nk.
@@ -506,8 +509,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   const uint32_t ds_thr = kr * 128 + cq * 2;  // the thread's dS^T words: + 1024 hf + 16 (column block ^ r8)
   const float c1 = a.c1;
 
-  // S^T = K Q^T and dP^T = V dO^T (64 keys x QT queries each), one commit group
-  auto issue_s_dp = [&](float (&s)[QT / 2], float (&dp)[QT / 2], uint32_t sQs, uint32_t sDOs) {
+  // S^T = K Q^T and dP^T = V dO^T (64 keys x QT queries each), one commit group, or two (split: S^T, then dP^T)
+  auto issue_s_dp = [&](float (&s)[QT / 2], float (&dp)[QT / 2], uint32_t sQs, uint32_t sDOs, const bool split) {
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk) {
@@ -515,6 +518,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       wgmma_ss_n64<T, 0, 0>(s, gmma_desc_sw128(sKw + ka, 16, 1024), gmma_desc_sw128(sQs + kb, 16, 1024),
                             kk > 0 ? 1u : 0u);
     }
+    if (split) wgmma_commit();
 #pragma unroll
     for (int kk = 0; kk < D / 16; ++kk) {
       const uint32_t ka = (kk >> 2) * KCHUNK + (kk & 3) * 32, kb = (kk >> 2) * QCHUNK + (kk & 3) * 32;
@@ -527,7 +531,10 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   // P^T = exp2(S^T*c1 + c3 [+ bias*log2e]) (masked), dS^T = P^T * (dP^T - delta): 16-bit A fragments in
   // pf / dsf, dS^T also to shared memory (row = key, 128-byte rows of QT = 64 queries, 128B swizzle).
   // Element pair e = 2 j + hf: key row kr + 8 hf, query columns 8 j + cq + {0, 1}.
-  auto elementwise = [&](const bool MASKED, const float (&s)[QT / 2], const float (&dp)[QT / 2],
+  // PASS = kPassBoth computes both in one pass.  Split in two, kPassP needs only S^T: it writes the fp32 P^T back
+  // into s; kPassDS then packs pf from it and computes dS^T from it and dP^T (the masks are already in P^T).  The two
+  // passes perform the same operations as the one, so pf and dsf are bitwise the same.
+  auto elementwise = [&](const bool MASKED, const int PASS, float (&s)[QT / 2], const float (&dp)[QT / 2],
                          uint32_t (&pf)[QT / 4], uint32_t (&dsf)[QT / 4], int row0, uint32_t stc3, uint32_t dsbuf) {
     int hi = QT - 1, lo[2] = {0, 0}, hi_k[2];
     if (MASKED) {
@@ -545,8 +552,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       // bias loads leave no registers to hold them)
       float2 c3, ndl;
       if constexpr (!BIAS) {
-        c3 = lds64f(stc3 + 4 * cc);
-        ndl = lds64f(stc3 + 4 * QT + 4 * cc);
+        if (PASS & kPassP) c3 = lds64f(stc3 + 4 * cc);
+        if (PASS & kPassDS) ndl = lds64f(stc3 + 4 * QT + 4 * cc);
       }
       const uint32_t ds_addr = dsbuf + ds_thr + ((j ^ r8) << 4);
 #pragma unroll
@@ -556,21 +563,31 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           c3 = lds64f(stc3 + 4 * cc);
           ndl = lds64f(stc3 + 4 * QT + 4 * cc);
         }
-        float x0 = fmaf(s[2 * e], c1, c3.x), x1 = fmaf(s[2 * e + 1], c1, c3.y);
-        if constexpr (BIAS) {
-          // (BIAS launches have one query head per CTA: h0)
-          const uint8_t* bcol = reinterpret_cast<const uint8_t*>(a.bias) +
-                                2 * ((long long)b * a.bias_sb + (long long)h0 * a.bias_sh + min(key_g[hf], a.Nk - 1));
-          const int q0 = min(row0 + cc, a.Nq - 1), q1 = min(row0 + cc + 1, a.Nq - 1);
-          const float2 bv = unpack2<T>(ldg_u16(bcol + 2 * (long long)q0 * a.bias_sn) |
-                                       (ldg_u16(bcol + 2 * (long long)q1 * a.bias_sn) << 16));
-          x0 = fmaf(bv.x, 1.4426950408889634f, x0);
-          x1 = fmaf(bv.y, 1.4426950408889634f, x1);
+        float p0 = s[2 * e], p1 = s[2 * e + 1];     // kPassDS: P^T from a kPassP pass
+        bool v0 = true, v1 = true;
+        if (PASS & kPassP) {
+          float x0 = fmaf(s[2 * e], c1, c3.x), x1 = fmaf(s[2 * e + 1], c1, c3.y);
+          if constexpr (BIAS) {
+            // (BIAS launches have one query head per CTA: h0)
+            const uint8_t* bcol = reinterpret_cast<const uint8_t*>(a.bias) +
+                                  2 * ((long long)b * a.bias_sb + (long long)h0 * a.bias_sh + min(key_g[hf], a.Nk - 1));
+            const int q0 = min(row0 + cc, a.Nq - 1), q1 = min(row0 + cc + 1, a.Nq - 1);
+            const float2 bv = unpack2<T>(ldg_u16(bcol + 2 * (long long)q0 * a.bias_sn) |
+                                         (ldg_u16(bcol + 2 * (long long)q1 * a.bias_sn) << 16));
+            x0 = fmaf(bv.x, 1.4426950408889634f, x0);
+            x1 = fmaf(bv.y, 1.4426950408889634f, x1);
+          }
+          const int hk_ = WINDOW ? hi_k[hf] : hi;
+          v0 = !MASKED || (cc >= lo[hf] && cc <= hk_);
+          v1 = !MASKED || (cc + 1 >= lo[hf] && cc + 1 <= hk_);
+          p0 = v0 ? ex2_approx(x0) : 0.f;
+          p1 = v1 ? ex2_approx(x1) : 0.f;
         }
-        const int hk_ = WINDOW ? hi_k[hf] : hi;
-        const bool v0 = !MASKED || (cc >= lo[hf] && cc <= hk_), v1 = !MASKED || (cc + 1 >= lo[hf] && cc + 1 <= hk_);
-        const float p0 = v0 ? ex2_approx(x0) : 0.f;
-        const float p1 = v1 ? ex2_approx(x1) : 0.f;
+        if (PASS == kPassP) {
+          s[2 * e] = p0;
+          s[2 * e + 1] = p1;
+          continue;
+        }
         const float ds0 = p0 * (dp[2 * e] + ndl.x), ds1 = p1 * (dp[2 * e + 1] + ndl.y);
         pf[e] = pack2<T>(p0, p1);
         dsf[e] = pack2<T>(ds0, ds1);
@@ -586,7 +603,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       }
     }
   };
-  auto elementwise_tile = [&](const float (&s)[QT / 2], const float (&dp)[QT / 2], uint32_t (&pf)[QT / 4],
+  auto elementwise_tile = [&](const int PASS, float (&s)[QT / 2], const float (&dp)[QT / 2], uint32_t (&pf)[QT / 4],
                               uint32_t (&dsf)[QT / 4], int row0, uint32_t stc3, uint32_t dsbuf) {
     // interior tile: every key of the warpgroup sees every query row (no causal diagonal, no ragged end)
     bool interior = keys_full && row0 + QT <= Nq && (!a.causal || key0 + 64 * w + 63 - off <= row0);
@@ -594,8 +611,8 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     if constexpr (WINDOW)
       interior = keys_full && row0 + QT <= Nq && key0 + 64 * w + 63 + lo_off <= row0 &&
                  row0 + QT - 1 <= key0 + 64 * w + hi_off;
-    if (!BIAS && interior) elementwise(false, s, dp, pf, dsf, row0, stc3, dsbuf);
-    else elementwise(true, s, dp, pf, dsf, row0, stc3, dsbuf);
+    if (PASS == kPassDS || (!BIAS && interior)) elementwise(false, PASS, s, dp, pf, dsf, row0, stc3, dsbuf);
+    else elementwise(true, PASS, s, dp, pf, dsf, row0, stc3, dsbuf);
     if constexpr (DQ && !WIDE) {
       fence_proxy_async_smem();
       named_bar_sync(1 + w, 128);             // the warpgroup's whole dS^T tile is in shared memory
@@ -615,6 +632,25 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     for (int kk = 0; kk < QT / 16; ++kk) {
       const uint32_t af[4] = {dsf[4 * kk], dsf[4 * kk + 1], dsf[4 * kk + 2], dsf[4 * kk + 3]};
       wgmma_rs<T, 1>(dk, af, gmma_desc_sw128(sQs + kk * 2048, QCHUNK, 1024), 1u);
+    }
+  };
+  // The elementwise stage once S^T, dP^T are issued (split: as two commit groups).  Split, the P pass (the
+  // exponentials) runs once S^T has retired, under dP^T, and the dS pass once dP^T has retired; otherwise one pass
+  // after both.
+  auto elementwise_after = [&](const bool split, float (&s)[QT / 2], float (&dp)[QT / 2], uint32_t (&pf)[QT / 4],
+                               uint32_t (&dsf)[QT / 4], int row0, uint32_t stc3, uint32_t dsbuf) {
+    if (split) {
+      wgmma_wait<1>();                        // S^T has retired; dP^T may still run
+      fence_regs(s);
+      elementwise_tile(kPassP, s, dp, pf, dsf, row0, stc3, dsbuf);
+      wgmma_wait<0>();
+      fence_regs(dp);
+      elementwise_tile(kPassDS, s, dp, pf, dsf, row0, stc3, dsbuf);
+    } else {
+      wgmma_wait<0>();
+      fence_regs(s);
+      fence_regs(dp);
+      elementwise_tile(kPassBoth, s, dp, pf, dsf, row0, stc3, dsbuf);
     }
   };
   // dQ = dS K.  STAGED: contraction over all kKeys keys of the CTA (dsbuf = a dS^T slot, whose warpgroup parts are
@@ -659,10 +695,13 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
   mbar_wait(BAR(KV_FULL), 0);
 
   if constexpr (WIDE) {
-    // In order per tile: S^T, dP^T -> elementwise -> dV, dK -> (owner) dQ of the tile before, one wait per batch.  One
-    // dQ tile per query tile and CTA, dQ(i) = [dS_0(i) | dS_1(i) | dS_2(i)] K over all 192 keys, owned by warpgroup
-    // i % 3 and issued in its iteration i + 1 after the dV / dK wait, so that the 32 dQ accumulators are dead through
-    // the elementwise stage and the dV / dK products.
+    // In order per tile: S^T, dP^T -> P pass (under dP^T) -> dS pass -> dV, dK -> (owner) dQ of the tile before (the
+    // WINDOW kernels: one elementwise pass after S^T, dP^T).  The warpgroup publishes its part of dS^T under its dV / dK
+    // products, and every product it issued has retired at the end of its `mine` branch: with a product still in
+    // flight after the branch, ptxas serialised every wgmma (notes C7518, C7520).  One dQ tile per query tile and CTA,
+    // dQ(i) = [dS_0(i) | dS_1(i) | dS_2(i)] K over all 192 keys, owned by warpgroup i % 3 and issued in its iteration
+    // i + 1 after the dV / dK wait, so that the 32 dQ accumulators are dead through the elementwise stage and the
+    // dV / dK products.
     // A warpgroup computes only the query tiles its own keys see (wr); on the item's other tiles it writes zeros to
     // its part of the slot, so dQ(i) is always the one 12-wgmma product, and passes the Q slot on.
     //   DS_FULL  : the two non-owners fence their parts to the async proxy and arrive (256 threads) after writing
@@ -671,21 +710,35 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     //              before writing its part of the slot for tile i + NDS (the owner of i has retired dQ(i) itself)
     // The owner then stages dQ(i) for its reducer warp.
     const TileRange wr = key_block_query_tiles<WINDOW>(key0 + 64 * w, 64, Nk, off, nqt, a.causal, W);
+    // the warpgroup's part of dS^T(i) is in shared memory: fence it to the async proxy, sync the warpgroup, arrive
+    // (non-owners)
+    auto publish_ds = [&](int i) {
+      fence_proxy_async_smem();
+      named_bar_sync(1 + w, 128);
+      int io = i;                               // (an opaque copy, as below)
+      asm volatile("" : "+r"(io));
+      if (io % NC != w) dsr.commit(io);
+    };
     for (int i = 0; i < NT; ++i) {
       const HeadTile ht = head_tile(i, i_lo, NI, HEAD_LOOP);
       const int st = qring.wait(i);
       const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
       const uint32_t dsbuf = ds_slot(i) + w * Cfg::kDS;
       const bool mine = ht.qt >= wr.lo && ht.qt < wr.hi;
-      uint32_t pf[QT / 4], dsf[QT / 4];
       if (mine) {
         float s[QT / 2], dp[QT / 2];
-        issue_s_dp(s, dp, sQs, sDOs);
+        uint32_t pf[QT / 4], dsf[QT / 4];
+        issue_s_dp(s, dp, sQs, sDOs, !WINDOW);
         if (i >= NDS) dsr.acquire(i);
-        wgmma_wait<0>();
-        fence_regs(s);
-        fence_regs(dp);
-        elementwise_tile(s, dp, pf, dsf, ht.qt * QT, sStats + st * 8 * QT, dsbuf);
+        elementwise_after(!WINDOW, s, dp, pf, dsf, ht.qt * QT, sStats + st * 8 * QT, dsbuf);
+        issue_dv_dk(pf, dsf, sQs, sDOs, dv, dk);
+        wgmma_commit();
+        publish_ds(i);                          // under dV and dK
+        wgmma_wait<0>();                        // the dQ accumulator only fits once the A fragments are dead
+        fence_regs(pf);
+        fence_regs(dsf);
+        fence_regs(dv);
+        fence_regs(dk);
       } else {
         if (i >= NDS) dsr.acquire(i);
 #pragma unroll
@@ -693,24 +746,12 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
           sts32(dsbuf + ds_thr + ((j ^ r8) << 4), 0u);
           sts32(dsbuf + ds_thr + ((j ^ r8) << 4) + 1024, 0u);
         }
+        publish_ds(i);
       }
-      fence_proxy_async_smem();
-      named_bar_sync(1 + w, 128);               // the warpgroup's whole part of dS^T(i) is in shared memory
       // what follows is redone from an opaque copy of i rather than kept live through the elementwise stage
       int io = i;
       asm volatile("" : "+r"(io));
       const int own = io % NC;
-      if (own != w) dsr.commit(io);
-      if (mine) {
-        const int so = io % NST;
-        issue_dv_dk(pf, dsf, sQ + so * Cfg::kQ, sDO + so * Cfg::kQ, dv, dk);
-        wgmma_commit();
-        wgmma_wait<0>();                        // the dQ accumulator only fits once the A fragments are dead
-        fence_regs(pf);
-        fence_regs(dsf);
-        fence_regs(dv);
-        fence_regs(dk);
-      }
       qring.release(io);                        // Q, dO and the stats of this stage are no longer read
       if (io > 0 && (own == 0 ? NC - 1 : own - 1) == w) {
         float dq[D / 2];
@@ -771,7 +812,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
     fence_regs(dq);
     if (NT > 0) {
       qring.wait(0);
-      issue_s_dp(s, dp, sQ, sDO);
+      issue_s_dp(s, dp, sQ, sDO, false);
       // i runs over the flat (head, query tile) sequence; row0 restarts at i_lo * QT with every head (next_row0)
       for (int i = 0, row0 = i_lo * QT; i < NT; ++i,
                row0 = HEAD_LOOP ? next_row0<WINDOW>(row0, i_lo, VARLEN ? Nq : a.nqt * QT, key0, hi_off) : row0 + QT) {
@@ -789,7 +830,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         if (i > 0) qring.release(i - 1);        // Q, dO and the stats of tile i - 1 are no longer read
         const bool own = (i & 1) == w;
         if (own && i >= NDS) dsr.acquire(i);
-        elementwise_tile(s, dp, pf, dsf, row0, sStats + st * 8 * QT, ds_slot(i) + w * Cfg::kDS);
+        elementwise_tile(kPassBoth, s, dp, pf, dsf, row0, sStats + st * 8 * QT, ds_slot(i) + w * Cfg::kDS);
         // the slot arithmetic below is redone from an opaque copy of i rather than kept live through the elementwise
         // stage (the BIAS kernels have no register to spare there)
         int io = i;
@@ -800,7 +841,7 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
         wgmma_commit();
         if (i + 1 < NT) {
           const int sn = qring.wait(i + 1);
-          issue_s_dp(s, dp, sQ + sn * Cfg::kQ, sDO + sn * Cfg::kQ);
+          issue_s_dp(s, dp, sQ + sn * Cfg::kQ, sDO + sn * Cfg::kQ, false);
         }
       }
       // drain: dQ(NT - 2) is in flight if this warpgroup owns it, dQ(NT - 1) is not issued yet
@@ -825,14 +866,14 @@ fcsa_bwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       const int st = qring.wait(i);
       const uint32_t sQs = sQ + st * Cfg::kQ, sDOs = sDO + st * Cfg::kQ;
       float s[QT / 2], dp[QT / 2];
-      issue_s_dp(s, dp, sQs, sDOs);
+      issue_s_dp(s, dp, sQs, sDOs, false);
       wgmma_wait<0>();
       fence_regs(s);
       fence_regs(dp);
 
       const uint32_t dsbuf = sDS + (2 * (i & 1) + w) * Cfg::kDS;
       uint32_t pf[QT / 4], dsf[QT / 4];
-      elementwise_tile(s, dp, pf, dsf, row0, sStats + st * 8 * QT, dsbuf);
+      elementwise_tile(kPassBoth, s, dp, pf, dsf, row0, sStats + st * 8 * QT, dsbuf);
       issue_dv_dk(pf, dsf, sQs, sDOs, dv, dk);
       wgmma_commit();
       wgmma_wait<0>();                          // the dQ accumulator only fits once the A fragments are dead
