@@ -173,8 +173,8 @@ fcsa_bias bias_struct(const Tensor& t, bool batch_dim, const optional<Tensor>& a
   return b;
 }
 
-// Backward workspaces, one pair per (device, stream): `scratch` (contents irrelevant) and `zeroed`
-// (fp32 dq accumulator + tile counters; zero-filled once, left zero by every backward).  Only grow.
+// Backward and decode workspaces: `scratch` (contents irrelevant) and `zeroed` (the fp32 dq accumulator; zero-filled
+// once, left zero by every backward).  Eager calls keep one pair per (device, stream) that only grows.
 struct Workspaces {
   Tensor scratch, zeroed;
 };
@@ -183,12 +183,28 @@ std::map<std::pair<int, void*>, Workspaces> g_ws;
 
 // The workspaces of (like's device, stream), grown to need_s scratch and need_z zeroed bytes.  A size of 0 is the
 // library's refusal of the problem.  with_zeroed = false (decode) needs the scratch only.
+// A call captured into a CUDA graph gets workspaces of its own instead, outside the cache: allocated during the capture
+// they come from the graph's private pool, which keeps them for the graph's lifetime, and the zero fill of `zeroed`
+// becomes a memset node that runs before the backward at every replay.  A cached pair would be freed by a later growth
+// or release_workspaces() while the graph still points at it, and would be shared by every graph captured on the
+// stream.
 Workspaces workspaces_of_size(size_t need_s, size_t need_z, const Tensor& like, cudaStream_t stream,
                               bool with_zeroed = true) {
   TORCH_CHECK(need_s > 0 && (need_z > 0 || !with_zeroed), "libfcsa_b200: ", fcsa_last_error());
+  const auto opts = like.options().dtype(at::kByte);
+  cudaStreamCaptureStatus capture = cudaStreamCaptureStatusNone;
+  C10_CUDA_CHECK(cudaStreamIsCapturing(stream, &capture));
+  if (capture != cudaStreamCaptureStatusNone) {
+    Workspaces own;
+    own.scratch = at::empty({(int64_t)need_s}, opts);
+    if (with_zeroed) {
+      own.zeroed = at::empty({(int64_t)need_z}, opts);
+      FCSA_CHECK(fcsa_zeroed_init(own.zeroed.data_ptr(), need_z, stream));
+    }
+    return own;
+  }
   std::lock_guard<std::mutex> lock(g_ws_mutex);
   Workspaces& w = g_ws[{(int)like.get_device(), (void*)stream}];
-  const auto opts = like.options().dtype(at::kByte);
   if (!w.scratch.defined() || (size_t)w.scratch.numel() < need_s) w.scratch = at::empty({(int64_t)need_s}, opts);
   if (with_zeroed && (!w.zeroed.defined() || (size_t)w.zeroed.numel() < need_z)) {
     w.zeroed = at::empty({(int64_t)need_z}, opts);
@@ -452,7 +468,8 @@ std::tuple<Tensor, Tensor, Tensor, optional<Tensor>> backward(
 //   q (B, H, Nq, D); k_cache, v_cache (B, kv_heads, capacity, D), written in place, so they must be usable as they
 //   are (no copy); cache_seqlens int32 on q's device; k, v (B, kv_heads, n_new, D) or both None; groups > 0:
 //   l2-normalise q and k over that many groups.  Returns o (B, H, Nq, D).  Scratch comes from the per-(device,
-//   stream) workspace of the backward, whose contents are irrelevant on entry.
+//   stream) workspace of the backward (a captured call's own, see workspaces_of_size), whose contents are irrelevant
+//   on entry.
 // decode_varlen: the same with packed new tokens (fcsa_decode_varlen): q (total_q, H, D), k, v (total_q, kv_heads, D)
 //   or both None, cu_seqlens_q int32 (B + 1,) on q's device, max_q >= every length.  Returns o (total_q, H, D).
 // ------------------------------------------------------------------------------------------------
@@ -675,9 +692,10 @@ std::tuple<Tensor, Tensor, Tensor> backward_varlen(
   return {dq, dk, dv};
 }
 
-// Drops the cached backward workspaces of every (device, stream) (they only ever grow: a long-context call leaves a
-// 1 GB accumulator behind).  Returns the number of bytes released to the caching allocator.  Safe at any time between
-// calls: buffers still referenced by enqueued kernels stay alive through the allocator's stream semantics.
+// Drops the cached workspaces of every (device, stream) (they only ever grow: a long-context call leaves a 1 GB
+// accumulator behind).  Returns the number of bytes released to the caching allocator.  Safe at any time between
+// calls: buffers still referenced by enqueued kernels stay alive through the allocator's stream semantics, and CUDA
+// graphs never hold cached workspaces (a captured call allocates its own, see workspaces_of_size).
 int64_t release_workspaces() {
   std::lock_guard<std::mutex> lock(g_ws_mutex);
   int64_t bytes = 0;

@@ -203,8 +203,10 @@ def debug():
 
 
 def release_workspaces():
-    """Free the backward workspaces cached per (device, stream) - the fp32 dq accumulator and the scratch area
-    only ever grow with the largest problem seen.  Returns the number of bytes handed back to the allocator."""
+    """Free the workspaces cached per (device, stream) for eager backward and decode calls - the fp32 dq accumulator
+    and the scratch area only ever grow with the largest problem seen.  Returns the number of bytes handed back to the
+    allocator.  Safe at any time, also while CUDA graphs are alive: a call captured into a graph allocates workspaces
+    of its own from the graph's memory pool, kept until the graph is destroyed, so a replay never uses the cache."""
     return int(_ext().release_workspaces())
 
 

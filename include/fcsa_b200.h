@@ -118,7 +118,11 @@ size_t fcsa_backward_workspace_bytes(const fcsa_problem* p);
  * finished - the pass that converts an accumulator tile to dq also clears it - so one buffer,
  * zero-filled ONCE (fcsa_zeroed_init), serves any number of calls of any shape enqueued on the same
  * stream.  This is what replaces the reference's per-call 33.5 MB memset of its fp32 dq (cu:1818).
- * Do not share one buffer between streams that may run concurrently. */
+ * Do not share one buffer between streams that may run concurrently.
+ * CUDA graphs: a workspace (scratch or zeroed, of any entry point) passed to a call that is being captured belongs to
+ * the graph until the graph is destroyed, since every replay uses it; do not free it, reuse it for other calls, or
+ * share it with a graph that may replay concurrently.  Capture the zero fill too (fcsa_zeroed_init on the capturing
+ * stream), so that the replay does not depend on what ran before it. */
 size_t fcsa_backward_zeroed_bytes(const fcsa_problem* p);
 
 /* Zero-fill a freshly allocated (or grown) zeroed workspace: cudaMemsetAsync on `stream`. */
