@@ -44,6 +44,8 @@ EXPORTED_SYMBOLS = (
     "fcsa_decode",
     "fcsa_decode_varlen_workspace_bytes",
     "fcsa_decode_varlen",
+    "fcsa_decode_rolling_workspace_bytes",
+    "fcsa_decode_rolling",
     "fcsa_forward_fused_varlen",
     "fcsa_backward_fused_varlen_workspace_bytes",
     "fcsa_backward_fused_varlen_zeroed_bytes",
@@ -159,6 +161,11 @@ def load():
     lib.fcsa_decode_varlen.restype = c_int32
     lib.fcsa_decode_varlen.argtypes = [PP, c_void_p, c_int32, PT, PT, PT, c_void_p, PT, PT, c_int32, PT, c_void_p,
                                        c_size_t, c_void_p]
+    lib.fcsa_decode_rolling_workspace_bytes.restype = c_size_t
+    lib.fcsa_decode_rolling_workspace_bytes.argtypes = [PP, c_void_p, c_int32]
+    lib.fcsa_decode_rolling.restype = c_int32
+    lib.fcsa_decode_rolling.argtypes = [PP, c_void_p, c_int32, PT, PT, PT, c_void_p, PT, PT, c_int32, PT, c_void_p,
+                                        c_size_t, c_void_p]
     PV = POINTER(FcsaVarlen)
     lib.fcsa_forward_fused_varlen.restype = c_int32
     lib.fcsa_forward_fused_varlen.argtypes = [PP, PV, PT, PT, PT, PN, PT, c_void_p, c_void_p]

@@ -19,6 +19,13 @@
 //     [cu_q[b], cu_q[b + 1]) of q and o (q_sb = o_sb = 0), read on the device after pdl_wait (seq_span).  Nq and R of
 //     the rules above become n_b and R_b = G * n_b; the grid is sized by the maximum (a.Nq), and a row block at or past
 //     R_b has no work.
+//   * rolling cache (ring = C > 0, WINDOW kernels only): the cache is a ring of C rows, absolute position p at row
+//     p mod C.  cache_seqlens[b] counts every token the element has seen and may exceed C; L_b and T_b are not clamped,
+//     and the tile ranges, split chunks and masks stay in absolute positions.  Absolute tile t is read from ring row
+//     (128 t) mod C (C is a multiple of 128, so a tile never straddles the wrap).  The host checks C >= W + Nq - 1: the
+//     keys a call sees, [T_b - Nq - W + 1, T_b), then still hold their own positions after its append.  A ring row
+//     past T_b in a tile holds an older position or was never written: the select gives P = 0 there, and V's rows
+//     past T_b are zeroed as before.
 #pragma once
 
 #include "key_tile.cuh"
@@ -34,6 +41,7 @@ struct DecodeArgs {
                              // key splits
   float c1;                  // scale * log2(e)
   float c2;                  // shift * log2(e)
+  int ring;                  // rolling cache (WINDOW kernels only): C = cap ring rows, position p at row p mod C; 0 = none
   const int32_t* seqlens;    // (B,) valid cache rows before the call
   const void* q;             // (B, H, Nq, D), element strides, feature dim contiguous
   long long q_sb, q_sh, q_sn;
@@ -116,9 +124,12 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
   if (r0 >= R) return;
   const int r_last = min(r0 + 63, R - 1);
 
-  // visible keys and this split's key tiles (uniform over the CTA)
-  const int L = min(max(a.seqlens[b], 0), a.cap);
-  const int Tb = min(L + (a.cu_q != nullptr ? (a.n_new ? qs.Nq : 0) : a.n_new), a.cap);
+  // visible keys and this split's key tiles (uniform over the CTA); a ring's lengths are absolute and not clamped
+  int ring = 0;
+  if constexpr (WINDOW) ring = a.ring;
+  const int L0 = max(a.seqlens[b], 0), L = ring ? L0 : min(L0, a.cap);
+  const int Tn = L + (a.cu_q != nullptr ? (a.n_new ? qs.Nq : 0) : a.n_new);
+  const int Tb = ring ? Tn : min(Tn, a.cap);
   const int off = diag_off(qs.Nq, Tb);
   int W = 0;                                  // the window
   if constexpr (WINDOW) W = a.window;
@@ -133,7 +144,8 @@ fcsa_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
     if (warp == 0 && elect_one() && j1 > j0) {
       tma_prefetch_desc(&tm_k);
       tma_prefetch_desc(&tm_v);
-      load_kv_tiles<D>(&tm_k, &tm_v, kr, vr, sK, sV, j0, j1, 0, hk, b);
+      if (ring) load_kv_tiles<D>(&tm_k, &tm_v, kr, vr, sK, sV, j0, j1, [=](int j) { return (j * 128) % ring; }, hk, b);
+      else load_kv_tiles<D>(&tm_k, &tm_v, kr, vr, sK, sV, j0, j1, TileRows{0}, hk, b);
     }
     return;
   }

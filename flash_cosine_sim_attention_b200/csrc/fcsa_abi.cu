@@ -252,6 +252,19 @@ int check_decode_varlen(const fcsa_problem* p, int32_t total_q) {
   return FCSA_OK;
 }
 
+// A rolling cache (fcsa_decode_rolling) of C = seq_k rows for seq_q new queries (packed: the longest): it needs a
+// window, whole 128-row tiles (a tile never straddles the wrap), and C >= W + seq_q - 1, so that the keys a call sees,
+// [T_b - seq_q - W + 1, T_b), are not overwritten by its own append.
+int check_decode_ring(const fcsa_problem* p) {
+  if (p->window <= 0) return fail(FCSA_ERR_INVALID, "decode rolling: a rolling cache needs a window");
+  if (p->seq_k % 128 != 0)
+    return fail(FCSA_ERR_INVALID, "decode rolling: cache rows %d must be a multiple of 128", p->seq_k);
+  if ((long long)p->seq_k < (long long)p->window + p->seq_q - 1)
+    return fail(FCSA_ERR_INVALID, "decode rolling: cache rows %d < window %d + new queries %d - 1", p->seq_k,
+                p->window, p->seq_q);
+  return FCSA_OK;
+}
+
 struct DecodeShape {
   int R, n_rb, n_split;
   long long items;
@@ -275,11 +288,12 @@ size_t align16(size_t n) { return (n + 15) & ~size_t(15); }
 // q^ of `rows` query rows (batch x seq_q, or the packed total_q)
 size_t decode_qhat_bytes(const fcsa_problem* p, size_t rows) { return align16(rows * p->heads * p->head_dim * 2); }
 
-// cu, total_q: packed new tokens (DecodeArgs::cu_q), nullptr = dense; n_new is then 1 (appended) or 0
+// cu, total_q: packed new tokens (DecodeArgs::cu_q), nullptr = dense; n_new is then 1 (appended) or 0.  ring: the
+// caches are rolling caches of seq_k rows (checked by check_decode_ring)
 template <typename T, int D>
 int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tensor* q, const fcsa_tensor* kc,
                   const fcsa_tensor* vc, const int32_t* seqlens, int32_t n_new, const fcsa_tensor* o, float* part,
-                  const int32_t* cu, int32_t total_q, cudaStream_t stream) {
+                  const int32_t* cu, int32_t total_q, bool ring, cudaStream_t stream) {
   using Cfg = fcsa::DecodeCfg<D>;
   CUtensorMap tk, tv;
   int r;
@@ -295,6 +309,7 @@ int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tenso
   const float log2e = 1.4426950408889634f;
   a.c1 = p->scale * log2e;
   a.c2 = p->shift * log2e;
+  a.ring = ring ? p->seq_k : 0;
   a.seqlens = seqlens;
   a.q = q->ptr; a.q_sb = q->sb; a.q_sh = q->sh; a.q_sn = q->sn;
   a.o = o->ptr; a.o_sb = o->sb; a.o_sh = o->sh; a.o_sn = o->sn;
@@ -852,12 +867,13 @@ int fcsa_l2norm_backward(int32_t dtype, int32_t batch, int32_t heads, int32_t ro
                   "l2norm backward launch");
 }
 
-// fcsa_decode and fcsa_decode_varlen: dense, or packed new tokens (cu != nullptr: q, o, k_new, v_new are total_q rows,
-// sequence b owning [cu[b], cu[b + 1]); appending when k_new and v_new are set, n_new unused)
+// fcsa_decode, fcsa_decode_varlen and fcsa_decode_rolling: dense, or packed new tokens (cu != nullptr: q, o, k_new,
+// v_new are total_q rows, sequence b owning [cu[b], cu[b + 1]); appending when k_new and v_new are set, n_new unused),
+// into full-length or (ring) rolling caches
 static int decode_impl(const fcsa_problem* p, const int32_t* cu, int32_t total_q, const fcsa_tensor* q,
                        const fcsa_tensor* k_cache, const fcsa_tensor* v_cache, const int32_t* cache_seqlens,
                        const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t n_new, int32_t groups,
-                       const fcsa_tensor* o, void* workspace, size_t workspace_bytes, void* stream) {
+                       const fcsa_tensor* o, void* workspace, size_t workspace_bytes, void* stream, bool ring = false) {
   int r;
   const bool append = cu ? (k_new != nullptr || v_new != nullptr) : n_new > 0;
   if ((r = check_tensor(q, "q")) || (r = check_tensor(k_cache, "k_cache")) || (r = check_tensor(v_cache, "v_cache")) ||
@@ -879,7 +895,8 @@ static int decode_impl(const fcsa_problem* p, const int32_t* cu, int32_t total_q
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
 
   // append pass: q_hat to the workspace (groups > 0), then k (normalised when groups > 0) and v into the caches at
-  // row cache_seqlens[b] (packed: the row's sequence b, at cache_seqlens[b] + its row within the sequence)
+  // row cache_seqlens[b] (packed: the row's sequence b, at cache_seqlens[b] + its row within the sequence), modulo
+  // the rows of a rolling cache
   const int64_t H = p->heads, N = rN, D = p->head_dim;
   const fcsa_tensor qhat = {workspace, H * N * D, N * D, D};
   fcsa::RowArgs a = row_args(rB, p->head_dim, groups);
@@ -887,9 +904,11 @@ static int decode_impl(const fcsa_problem* p, const int32_t* cu, int32_t total_q
   int n = 0;
   if (groups > 0) a.t[n++] = {p->heads, rN, *q, qhat, {}, nullptr, nullptr, rN, 0};
   if (append) {
-    a.t[n++] = {p->kv_heads, n_app, *k_new, *k_cache, {}, nullptr, cache_seqlens, p->seq_k, groups == 0 ? 1 : 0, cu,
+    const uint8_t k_raw = groups == 0 ? 1 : 0, rolling = ring ? 1 : 0;
+    a.t[n++] = {p->kv_heads, n_app, *k_new, *k_cache, {}, nullptr, cache_seqlens, p->seq_k, k_raw, rolling, cu,
                 p->batch, p->seq_q};
-    a.t[n++] = {p->kv_heads, n_app, *v_new, *v_cache, {}, nullptr, cache_seqlens, p->seq_k, 1, cu, p->batch, p->seq_q};
+    a.t[n++] = {p->kv_heads, n_app, *v_new, *v_cache, {}, nullptr, cache_seqlens, p->seq_k, 1, rolling, cu, p->batch,
+                p->seq_q};
   }
   if (n > 0 && (r = launched(fcsa::launch_row_append(a, n, p->dtype == FCSA_BF16, s), "append pass launch")))
     return r;
@@ -898,7 +917,7 @@ static int decode_impl(const fcsa_problem* p, const int32_t* cu, int32_t total_q
   float* part = reinterpret_cast<float*>(static_cast<char*>(workspace) + qbytes);
   r = dispatch(p, [&](auto t, auto d) {
     return launch_decode<typename decltype(t)::type, decltype(d)::value>(
-        p, sh, qa, k_cache, v_cache, cache_seqlens, cu ? (append ? 1 : 0) : n_new, o, part, cu, total_q, s);
+        p, sh, qa, k_cache, v_cache, cache_seqlens, cu ? (append ? 1 : 0) : n_new, o, part, cu, total_q, ring, s);
   });
   if (r || !cu) return r;
   // o = 0 in the rows outside every sequence
@@ -941,6 +960,35 @@ int fcsa_decode_varlen(const fcsa_problem* p, const int32_t* cu_seqlens_q, int32
     return fail(FCSA_ERR_INVALID, "decode varlen: pass both k_new and v_new, or neither");
   return decode_impl(p, cu_seqlens_q, total_q, q, k_cache, v_cache, cache_seqlens, k_new, v_new, 0, groups, o,
                      workspace, workspace_bytes, stream);
+}
+
+// The problem of a rolling-cache call: check_decode_problem's (dense) or check_decode_varlen's (packed), then the ring's
+static int check_decode_rolling(const fcsa_problem* p, const int32_t* cu, int32_t total_q) {
+  int r;
+  if ((r = cu ? check_decode_varlen(p, total_q) : check_decode_problem(p, 0))) return r;
+  return check_decode_ring(p);
+}
+
+size_t fcsa_decode_rolling_workspace_bytes(const fcsa_problem* p, const int32_t* cu_seqlens_q, int32_t total_q) {
+  DecodeShape sh;
+  if (check_decode_rolling(p, cu_seqlens_q, total_q) || decode_shape(p, &sh)) return 0;
+  const size_t rows = cu_seqlens_q ? (size_t)total_q : (size_t)p->batch * p->seq_q;
+  return decode_qhat_bytes(p, rows) + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
+}
+
+int fcsa_decode_rolling(const fcsa_problem* p, const int32_t* cu_seqlens_q, int32_t total_q, const fcsa_tensor* q,
+                        const fcsa_tensor* k_cache, const fcsa_tensor* v_cache, const int32_t* cache_seqlens,
+                        const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t groups, const fcsa_tensor* o,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  int r;
+  if ((r = check_decode_rolling(p, cu_seqlens_q, total_q))) return r;
+  if (reinterpret_cast<uintptr_t>(cu_seqlens_q) & 3)
+    return fail(FCSA_ERR_INVALID, "decode rolling: cu_seqlens_q must be a 4-byte aligned int32 array");
+  if ((k_new == nullptr) != (v_new == nullptr))
+    return fail(FCSA_ERR_INVALID, "decode rolling: pass both k_new and v_new, or neither");
+  const int32_t n_new = !cu_seqlens_q && k_new ? p->seq_q : 0;
+  return decode_impl(p, cu_seqlens_q, total_q, q, k_cache, v_cache, cache_seqlens, k_new, v_new, n_new, groups, o,
+                     workspace, workspace_bytes, stream, true);
 }
 
 int fcsa_forward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_tensor* q, const fcsa_tensor* k,

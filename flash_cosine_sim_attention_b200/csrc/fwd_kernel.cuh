@@ -124,7 +124,7 @@ fcsa_fwd_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant_
       tma_prefetch_desc(&tm_v);
       mbar_expect_tx(BAR(Q_FULL), Cfg::kQ);
       load_query_rows<D>(&tm_q, BAR(Q_FULL), sQ, BM, q.q_row0 + q.m0, h, tb);
-      load_kv_tiles<D>(&tm_k, &tm_v, kr, vr, sK, sV, j_lo, NT, q.k_row0, q.hk, tb);
+      load_kv_tiles<D>(&tm_k, &tm_v, kr, vr, sK, sV, j_lo, NT, TileRows{q.k_row0}, q.hk, tb);
     }
     return;
   }

@@ -132,24 +132,32 @@ __device__ __forceinline__ void load_query_rows(const CUtensorMap* tm, uint32_t 
 }
 
 // ---- producer: K and V tiles [j0, j1) through the two rings (tile j is use j - j0) --------------------------------
-// Tile j is rows row0 + 128 j of kv head hk at batch coordinate tb, D / 64 TMA boxes of 64 features each.
-template <int D, int S>
+// Tile j is rows row_of(j) .. + 127 of kv head hk at batch coordinate tb, D / 64 TMA boxes of 64 features each.
+// row_of is the kernel's row mapping: row0 + 128 j for the forward and dQ kernels, the ring row of a rolling cache for
+// the decode kernel.
+template <int D, int S, class RowOf>
 __device__ __forceinline__ void load_kv_tiles(const CUtensorMap* tm_k, const CUtensorMap* tm_v, Ring<S> kr, Ring<S> vr,
-                                              uint32_t sK, uint32_t sV, int j0, int j1, int row0, int hk, int tb) {
+                                              uint32_t sK, uint32_t sV, int j0, int j1, RowOf row_of, int hk, int tb) {
   constexpr int TILE = 128 * D * 2;
   for (int j = j0; j < j1; ++j) {
     const int s = kr.acquire(j - j0);
     mbar_expect_tx(kr.full_bar(s), TILE);
 #pragma unroll
     for (int ch = 0; ch < D / 64; ++ch)
-      tma_load_4d(sK + s * TILE + ch * 16384, tm_k, kr.full_bar(s), ch * 64, row0 + j * 128, hk, tb);
+      tma_load_4d(sK + s * TILE + ch * 16384, tm_k, kr.full_bar(s), ch * 64, row_of(j), hk, tb);
     vr.acquire(j - j0);
     mbar_expect_tx(vr.full_bar(s), TILE);
 #pragma unroll
     for (int ch = 0; ch < D / 64; ++ch)
-      tma_load_4d(sV + s * TILE + ch * 16384, tm_v, vr.full_bar(s), ch * 64, row0 + j * 128, hk, tb);
+      tma_load_4d(sV + s * TILE + ch * 16384, tm_v, vr.full_bar(s), ch * 64, row_of(j), hk, tb);
   }
 }
+
+// The identity mapping of load_kv_tiles: tile j is rows row0 + 128 j.
+struct TileRows {
+  int row0;
+  __device__ __forceinline__ int operator()(int j) const { return row0 + j * 128; }
+};
 
 // ---- consumer: S = Q K^T (64 x 128, fp32) ----------------------------------------------------------------------
 // sQ: the warpgroup's 64 rows of the first 64-feature chunk of Q, q_chunk bytes to the next; sKs: the K tile's slot.

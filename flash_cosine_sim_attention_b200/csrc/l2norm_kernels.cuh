@@ -32,7 +32,9 @@ struct RowTensor {
   // read by the append pass only (row_fwd_kernel<..., APPEND = true>, the key/value-cache decode):
   const int32_t* row0;            // device (B,): row n of x goes to row row0[b] + n of y; nullptr = row n
   int rows_y;                     // rows of y: a destination row outside [0, rows_y) is not written
-  int raw;                        // 1: y = x, no l2norm whatever G (the values)
+  // (raw and ring share the four bytes raw once had alone: every row pass keeps its parameter block)
+  uint8_t raw;                    // 1: y = x, no l2norm whatever G (the values)
+  uint8_t ring;                   // 1: y is a rolling cache of rows_y rows, row r goes to row r mod rows_y
   // packed sequences (with row0): x is one batch of N packed rows, sequence s owns rows [cu[s], cu[s + 1]) (clamped as
   // seq_span does, at most max_n rows) and its row n goes to row row0[s] + n - cu[s] of y's batch s; rows outside
   // every sequence are not written.  nullptr = row n of batch b goes to row row0[b] + n of y's batch b.
@@ -265,7 +267,8 @@ __device__ __forceinline__ float row_mul(const RowArgs& a) {
 // time (4 or 8), 0 = read it from the arguments.  x is read with coherent loads: it may alias y.  The 16-bit passes
 // keep four blocks per SM (at most 64 registers).  APPEND (16-bit only): grid.y runs over up to three tensors, each
 // row lands at the per-batch offset row0[b] (rows falling outside y are skipped) and `raw` tensors are copied; with
-// packed sequences (RowTensor::cu) at the offset of the row's sequence.
+// packed sequences (RowTensor::cu) at the offset of the row's sequence; in a rolling cache (`ring`) at that row modulo
+// rows_y.
 template <typename T, typename X, int TPR, int U, bool APPEND = false>
 __global__ void __launch_bounds__(256, 8 / sizeof(X)) row_fwd_kernel(const RowArgs a) {
   // SIXTEEN features per thread: the pass is issue-bound before it is memory-bound (ncu: 84 % issue-slot
@@ -310,6 +313,7 @@ __global__ void __launch_bounds__(256, 8 / sizeof(X)) row_fwd_kernel(const RowAr
         } else {
           ny += t.row0[b];
         }
+        if (t.ring && ny >= 0) ny %= t.rows_y;
       }
       yoff[u] = (ny >= 0 && ny < t.rows_y) ? yb * t.y.sb + h * t.y.sh + ny * t.y.sn + tr * 16 : -1;
     }

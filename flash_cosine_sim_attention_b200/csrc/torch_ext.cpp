@@ -472,6 +472,8 @@ std::tuple<Tensor, Tensor, Tensor, optional<Tensor>> backward(
 //   on entry.
 // decode_varlen: the same with packed new tokens (fcsa_decode_varlen): q (total_q, H, D), k, v (total_q, kv_heads, D)
 //   or both None, cu_seqlens_q int32 (B + 1,) on q's device, max_q >= every length.  Returns o (total_q, H, D).
+// rolling (both): the caches are rolling caches of `capacity` rows (fcsa_decode_rolling); dense k, v then bring Nq
+//   rows, one per query.
 // ------------------------------------------------------------------------------------------------
 // The checks both share: q's rank (3 packed, 4 dense) and dtype, the caches, cache_seqlens, and k / v, whose leading
 // `rows` dimensions must match q's (B for dense, total_q packed).  Returns k, v made TMA-ready (undefined when absent).
@@ -520,12 +522,14 @@ std::tuple<Tensor, Tensor> decode_checks(const Tensor& q_in, const Tensor& k_cac
 
 Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
               const optional<Tensor>& k_in, const optional<Tensor>& v_in, double scale, double shift, bool causal,
-              int64_t groups, int64_t window) {
+              int64_t groups, int64_t window, bool rolling) {
   Tensor k, v;
   std::tie(k, v) = decode_checks(q_in, k_cache, v_cache, cache_seqlens, k_in, v_in, false);
   const int64_t B = q_in.size(0), H = q_in.size(1), Nq = q_in.size(2), D = q_in.size(3);
   const int64_t Hk = k_cache.size(1), cap = k_cache.size(2);
   const int64_t n_new = k.defined() ? k.size(2) : 0;
+  TORCH_CHECK(!rolling || !k.defined() || n_new == Nq, "decode: a rolling cache appends one k, v row per query (",
+              Nq, "), got ", n_new);
   const c10::cuda::CUDAGuard guard(q_in.device());
   const Tensor q = tma_ready(q_in);
   const fcsa_problem p =
@@ -533,18 +537,25 @@ Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, 
   Tensor o = at::empty({B, H, Nq, D}, q.options());
   cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
   const Tensor scratch =
-      workspaces_of_size(fcsa_decode_workspace_bytes(&p, (int32_t)n_new), 0, q, stream, false).scratch;
+      workspaces_of_size(rolling ? fcsa_decode_rolling_workspace_bytes(&p, nullptr, 0)
+                                 : fcsa_decode_workspace_bytes(&p, (int32_t)n_new),
+                         0, q, stream, false).scratch;
   const fcsa_tensor tq = view4(q), tkc = view4(k_cache), tvc = view4(v_cache), to = view4(o);
   fcsa_tensor tk = {nullptr, 0, 0, 0}, tv = {nullptr, 0, 0, 0};
   if (k.defined()) { tk = view4(k); tv = view4(v); }
-  FCSA_CHECK(fcsa_decode(&p, &tq, &tkc, &tvc, cache_seqlens.data_ptr<int32_t>(), &tk, &tv, (int32_t)n_new,
-                         (int32_t)groups, &to, scratch.data_ptr(), (size_t)scratch.numel(), stream));
+  if (rolling)
+    FCSA_CHECK(fcsa_decode_rolling(&p, nullptr, 0, &tq, &tkc, &tvc, cache_seqlens.data_ptr<int32_t>(),
+                                   k.defined() ? &tk : nullptr, k.defined() ? &tv : nullptr, (int32_t)groups, &to,
+                                   scratch.data_ptr(), (size_t)scratch.numel(), stream));
+  else
+    FCSA_CHECK(fcsa_decode(&p, &tq, &tkc, &tvc, cache_seqlens.data_ptr<int32_t>(), &tk, &tv, (int32_t)n_new,
+                           (int32_t)groups, &to, scratch.data_ptr(), (size_t)scratch.numel(), stream));
   return o;
 }
 
 Tensor decode_varlen(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
                      const Tensor& cu_q, int64_t max_q, const optional<Tensor>& k_in, const optional<Tensor>& v_in,
-                     double scale, double shift, bool causal, int64_t groups, int64_t window) {
+                     double scale, double shift, bool causal, int64_t groups, int64_t window, bool rolling) {
   Tensor k, v;
   std::tie(k, v) = decode_checks(q_in, k_cache, v_cache, cache_seqlens, k_in, v_in, true);
   const int64_t B = k_cache.size(0), H = q_in.size(1), Tq = q_in.size(0), D = q_in.size(2);
@@ -562,15 +573,17 @@ Tensor decode_varlen(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_
   Tensor o = at::empty({Tq, H, D}, q.options());
   if (Tq == 0) return o;
   cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
+  const int32_t* cu = cu_q.data_ptr<int32_t>();
   const Tensor scratch =
-      workspaces_of_size(fcsa_decode_varlen_workspace_bytes(&p, (int32_t)Tq), 0, q, stream, false).scratch;
+      workspaces_of_size(rolling ? fcsa_decode_rolling_workspace_bytes(&p, cu, (int32_t)Tq)
+                                 : fcsa_decode_varlen_workspace_bytes(&p, (int32_t)Tq),
+                         0, q, stream, false).scratch;
   const fcsa_tensor tq = view_packed(q), tkc = view4(k_cache), tvc = view4(v_cache), to = view_packed(o);
   fcsa_tensor tk, tv;
   if (k.defined()) { tk = view_packed(k); tv = view_packed(v); }
-  FCSA_CHECK(fcsa_decode_varlen(&p, cu_q.data_ptr<int32_t>(), (int32_t)Tq, &tq, &tkc, &tvc,
-                                cache_seqlens.data_ptr<int32_t>(), k.defined() ? &tk : nullptr,
-                                k.defined() ? &tv : nullptr, (int32_t)groups, &to, scratch.data_ptr(),
-                                (size_t)scratch.numel(), stream));
+  const auto run = rolling ? fcsa_decode_rolling : fcsa_decode_varlen;
+  FCSA_CHECK(run(&p, cu, (int32_t)Tq, &tq, &tkc, &tvc, cache_seqlens.data_ptr<int32_t>(), k.defined() ? &tk : nullptr,
+                 k.defined() ? &tv : nullptr, (int32_t)groups, &to, scratch.data_ptr(), (size_t)scratch.numel(), stream));
   return o;
 }
 
@@ -749,11 +762,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("causal"), py::arg("groups"), py::arg("window") = 0, py::arg("deterministic") = false);
   m.def("decode", &decode, "new queries against a key/value cache, appending k / v at cache_seqlens", py::arg("q"),
         py::arg("k_cache"), py::arg("v_cache"), py::arg("cache_seqlens"), py::arg("k"), py::arg("v"), py::arg("scale"),
-        py::arg("shift"), py::arg("causal"), py::arg("groups"), py::arg("window") = 0);
+        py::arg("shift"), py::arg("causal"), py::arg("groups"), py::arg("window") = 0, py::arg("rolling") = false);
   m.def("decode_varlen", &decode_varlen, "decode with a different number of new tokens per sequence (packed q, k, v)",
         py::arg("q"), py::arg("k_cache"), py::arg("v_cache"), py::arg("cache_seqlens"), py::arg("cu_q"),
         py::arg("max_q"), py::arg("k"), py::arg("v"), py::arg("scale"), py::arg("shift"), py::arg("causal"),
-        py::arg("groups"), py::arg("window") = 0);
+        py::arg("groups"), py::arg("window") = 0, py::arg("rolling") = false);
   m.def("release_workspaces", &release_workspaces, "free the cached backward workspaces; returns the bytes released");
   m.def("abi_version", []() { return fcsa_version(); });
   m.def("_error_path_selftest", []() { FCSA_CHECK(fcsa_forward(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr)); },

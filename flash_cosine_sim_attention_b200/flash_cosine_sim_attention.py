@@ -653,9 +653,9 @@ def flash_cosine_sim_attention(q, k, v, mask=None, attn_bias=None, scale=8, grou
 
 
 def _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias, cu_seqlens_q=None,
-                         max_seqlen_q=None):
+                         max_seqlen_q=None, window=0, rolling=False):
     """Everything flash_cosine_sim_attention_with_kv_cache rejects before touching a device.  With cu_seqlens_q, q, k
-    and v are packed: (total_q, heads, head_dim) and (total_q, kv_heads, head_dim)."""
+    and v are packed: (total_q, heads, head_dim) and (total_q, kv_heads, head_dim).  window: _check_window's."""
     packed = cu_seqlens_q is not None
     if exists(attn_bias):
         raise NotImplementedError("flash_cosine_sim_attention_with_kv_cache: attn_bias is not supported")
@@ -714,9 +714,30 @@ def _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask,
     if gs == 0 or (gs & (gs - 1)) != 0:
         raise ValueError(f"flash_cosine_sim_attention_with_kv_cache: groups {groups} must divide head_dim {D} into "
                          "power-of-two chunks")
+    if not isinstance(rolling, bool):
+        raise TypeError(f"flash_cosine_sim_attention_with_kv_cache: rolling must be a bool, got {rolling!r}")
+    if rolling:
+        _check_rolling(q, k_cache, k, window, max(max_seqlen_q, 1) if packed else q.shape[2], packed)
     if not (q.is_cuda and cache_seqlens.is_cuda and (not packed or cu_seqlens_q.is_cuda)):
         raise RuntimeError("flash_cosine_sim_attention_with_kv_cache: CUDA tensors required (cache_seqlens and "
                            "cu_seqlens_q included: the host never reads them) - this build has no CPU path")
+
+
+def _check_rolling(q, k_cache, k, window, n, packed):
+    """A rolling cache of C = k_cache.shape[2] rows for calls of at most n new tokens: it needs a window W, whole
+    128-row tiles and C >= W + n - 1 (the keys a call sees, [T_b - n - W + 1, T_b), must survive its own append)."""
+    name = "flash_cosine_sim_attention_with_kv_cache"
+    C = k_cache.shape[2]
+    if window == 0:
+        raise ValueError(f"{name}: a rolling cache needs a window (it keeps the window's keys only)")
+    if C % 128 != 0:
+        raise ValueError(f"{name}: a rolling cache's capacity must be a multiple of 128 rows, got {C}")
+    if C < window + n - 1:
+        raise ValueError(f"{name}: a rolling cache of {C} rows is too small for window {window} and {n} new tokens "
+                         f"per call: it needs at least window + n - 1 = {window + n - 1} rows")
+    if not packed and k is not None and k.shape[2] != q.shape[2]:
+        raise ValueError(f"{name}: with a rolling cache, k and v bring one row per query ({q.shape[2]}), got "
+                         f"{k.shape[2]}")
 
 
 def _check_cu_seqlens_q(q, B, cu_seqlens_q, max_seqlen_q):
@@ -740,7 +761,7 @@ def _check_cu_seqlens_q(q, B, cu_seqlens_q, max_seqlen_q):
 
 def flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens, k=None, v=None, scale=8, groups=1,
                                              causal=True, l2norm_qk=True, mask=None, attn_bias=None, window=None,
-                                             cu_seqlens_q=None, max_seqlen_q=None):
+                                             cu_seqlens_q=None, max_seqlen_q=None, rolling=False):
     """Cosine-sim attention of new queries against a key/value cache, for inference (generation).
 
     q: (batch, heads, n_q, head_dim) new queries.  k_cache, v_cache: (batch, kv_heads, capacity, head_dim), kv_heads
@@ -758,7 +779,7 @@ def flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens,
     L_b + n_new must not exceed the capacity: rows that do not fit are not written, and T_b is clamped to the
     capacity.  float16 / bfloat16 and head dims 64 and 128 only; no autograd, attn_bias, mask, float32 or merged
     batch-heads.  window: sliding-window attention as in flash_cosine_sim_attention with n_k = T_b; a step then reads
-    the tiles of its window, not the whole valid cache (the cache itself stays full-length).
+    the tiles of its window, not the whole valid cache (the cache itself stays full-length unless rolling=True).
     Returns o (batch, heads, n_q, head_dim).
 
     A different number of new tokens per batch element (speculative verification, chunked prefill, ragged prompts):
@@ -770,19 +791,36 @@ def flash_cosine_sim_attention_with_kv_cache(q, k_cache, v_cache, cache_seqlens,
     rules above hold per element with n_q = n_b and T_b = min(L_b + (n_b if appending, else 0), capacity).  Rows
     outside every sequence ([0, cu_seqlens_q[0]) and [cu_seqlens_q[-1], total_q)) give 0.  cu_seqlens_q is never read
     on the host either, and cache_seqlens is not advanced: add cu_seqlens_q[1:] - cu_seqlens_q[:-1] afterwards.
-    Returns o (total_q, heads, head_dim)."""
+    Returns o (total_q, heads, head_dim).
+
+    rolling=True: the caches are rolling caches for sliding-window decoding, rings of C = capacity rows that keep the
+    window's keys only, so their memory is bounded by the window instead of the sequence (as Mistral-style rolling
+    caches).  The rules above then read:
+      - absolute position p lives at ring row p mod C;
+      - cache_seqlens[b] = L_b counts every token element b has seen, and may be far larger than C; the caller still
+        advances it after the call;
+      - T_b = L_b + n_b (n_b = n_q dense, or the packed length when appending) with no clamp to C, and the window rule
+        holds over absolute positions: query i sees key j iff 0 <= i + T_b - n_b - j < window (causal) or
+        |i + T_b - n_b - j| < window;
+      - new row n of element b is written to ring row (L_b + n) mod C.
+    A window is required, C must be a multiple of 128, and C >= window + n - 1 with n = n_q (dense) or max_seqlen_q
+    (packed): below that, a call's append would overwrite a key that one of its own queries still sees.  Dense k, v
+    bring one row per query.  L_b + n_b must
+    stay below 2^31 - 128; cache_seqlens is never read on the host, so this is not checked.  With the same number of
+    key splits, o is bitwise what a full-length cache holding the same keys gives."""
     window = _check_window(window, attn_bias, "flash_cosine_sim_attention_with_kv_cache")
-    _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias, cu_seqlens_q, max_seqlen_q)
+    _check_kv_cache_args(q, k_cache, v_cache, cache_seqlens, k, v, groups, mask, attn_bias, cu_seqlens_q, max_seqlen_q,
+                         window, rolling)
     _warn_fp16_overflow(q.dtype, scale, groups, l2norm_qk)
     shift = _choose_shift(q.dtype, scale, groups, l2norm_qk)
     g = int(groups) if l2norm_qk else 0
     if cu_seqlens_q is None:
         return _ext().decode(q, k_cache, v_cache, cache_seqlens, k, v, float(scale), float(shift), bool(causal), g,
-                             window)
+                             window, rolling)
     if q.shape[0] == 0:
         return q.new_empty(q.shape)
     return _ext().decode_varlen(q, k_cache, v_cache, cache_seqlens, cu_seqlens_q, max(int(max_seqlen_q), 1), k, v,
-                                float(scale), float(shift), bool(causal), g, window)
+                                float(scale), float(shift), bool(causal), g, window, rolling)
 
 
 class _FusedVarlenAttention(Function):

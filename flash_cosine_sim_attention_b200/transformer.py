@@ -47,16 +47,34 @@ def FeedForward(dim, mult=4, pre_norm=False):
     )
 
 
+# the fewest tokens one call can append to a rolling cache: a rolling cache for window W has
+# round_up(W - 1 + ROLLING_CHUNK, 128) rows, and longer inputs (prompts) are prefilled in chunks
+ROLLING_CHUNK = 128
+
+
+def rolling_capacity(window):
+    """The rows of a rolling cache for a layer with this window: round_up(window - 1 + ROLLING_CHUNK, 128)."""
+    return -(-(window - 1 + ROLLING_CHUNK) // 128) * 128
+
+
 class KVCache:
     """Keys and values of one attention layer, for decoding token after token (`forward(x, cache=...)`).
 
     `k`, `v`: (batch, kv_heads, capacity, dim_head), allocated at the first call in the dtype of the keys.  With the
     CUDA kernel they hold what flash_cosine_sim_attention_with_kv_cache stores (l2-normalised keys); with the plain
-    attention the raw keys.  `seqlens`: the valid rows per batch element on the device (int32), `length`: the same
-    count on the host (the batch elements advance together here)."""
+    attention the raw keys.  `seqlens`: the tokens seen per batch element on the device (int32), `length`: the same
+    count on the host (the batch elements advance together here).
 
-    def __init__(self, capacity):
+    rolling=True: a rolling cache for a windowed layer, a ring of `capacity` rows (a multiple of 128) where position p
+    lives at row p mod capacity.  It takes any number of tokens; its memory is bounded by the window, not the sequence.
+    A call brings at most capacity - window + 1 tokens at a time, and longer inputs are split into chunks of that
+    size."""
+
+    def __init__(self, capacity, rolling=False):
+        if rolling and capacity % 128 != 0:
+            raise ValueError(f"a rolling cache has a multiple of 128 rows, got {capacity}")
         self.capacity = capacity
+        self.rolling = rolling
         self.k = self.v = self.seqlens = None
         self.length = 0
 
@@ -66,7 +84,7 @@ class Attention(nn.Module):
                  use_cuda_kernel=False, non_cosine_sim_attn=False, groups=None, kv_heads=None, window=None, **kwargs):
         super().__init__()
         # window: sliding-window attention - each token attends to itself and the window - 1 tokens before it, on
-        # every path (dense, packed documents, the key/value cache; the cache itself stays full-length)
+        # every path (dense, packed documents, the key/value cache, which may then be a rolling cache of the window)
         if window is not None and non_cosine_sim_attn:
             raise NotImplementedError("window is implemented for cosine-sim attention only (not non_cosine_sim_attn)")
         self.window = window
@@ -157,7 +175,17 @@ class Attention(nn.Module):
             raise NotImplementedError("the key/value cache is implemented for cosine-sim attention only")
         b, _, n, d = k.shape
         L = cache.length
-        if L + n > cache.capacity:
+        if cache.rolling:
+            if self.window is None:
+                raise ValueError("a rolling key/value cache needs a windowed layer (window=...)")
+            step = cache.capacity - self.window + 1
+            if step < 1:
+                raise ValueError(f"a rolling cache of {cache.capacity} rows is too small for window {self.window}")
+            if n > step:
+                # chunked prefill: each chunk's append leaves every key its own queries see in the ring
+                return torch.cat([self._attend_cached(q[:, :, s:s + step], k[:, :, s:s + step], v[:, :, s:s + step],
+                                                      cache) for s in range(0, n, step)], dim=2)
+        elif L + n > cache.capacity:
             raise ValueError(f"key/value cache full: {L} + {n} tokens exceed its capacity {cache.capacity}")
         # the uncached CUDA path hands these keywords to flash_cosine_sim_attention; with a cache only l2norm_qk has a
         # meaning, and a silently dropped one would make cached and uncached outputs differ.  `deterministic` only
@@ -176,7 +204,16 @@ class Attention(nn.Module):
             o = flash_cosine_sim_attention_with_kv_cache(q, cache.k, cache.v, cache.seqlens, k, v, scale=self.scale,
                                                          groups=self.l2norm_groups, causal=True,
                                                          l2norm_qk=self.kernel_kwargs.get("l2norm_qk", True),
-                                                         window=self.window)
+                                                         window=self.window, rolling=cache.rolling)
+        elif cache.rolling:
+            # the ring holds positions [max(0, L + n - C), L + n) after the append; the window rule is relative
+            C = cache.capacity
+            rows = torch.arange(L, L + n, device=k.device) % C
+            cache.k[:, :, rows] = k
+            cache.v[:, :, rows] = v
+            held = torch.arange(max(0, L + n - C), L + n, device=k.device) % C
+            o = plain_cosine_sim_attention(q, cache.k[:, :, held], cache.v[:, :, held], causal=True, scale=self.scale,
+                                           groups=self.l2norm_groups, window=self.window)
         else:
             cache.k[:, :, L:L + n] = k
             cache.v[:, :, L:L + n] = v
@@ -225,15 +262,24 @@ class CosineSimCausalTransformer(nn.Module):
                 nn.init.xavier_normal_(lin.weight.data, gain=g)
         nn.init.xavier_normal_(self.to_logits[-1].weight.data, gain=1.0)
 
-    def new_cache(self):
-        """One empty KVCache per layer, holding up to max_seq_len tokens, for forward(x, cache=...)."""
-        return [KVCache(self.max_seq_len) for _ in self.layers]
+    def new_cache(self, rolling=False):
+        """One empty KVCache per layer, holding up to max_seq_len tokens, for forward(x, cache=...).  rolling=True (a
+        windowed model only): rolling caches of rolling_capacity(window) rows each, which keep the window's keys
+        only; a prompt longer than one chunk is prefilled in chunks."""
+        if not rolling:
+            return [KVCache(self.max_seq_len) for _ in self.layers]
+        window = self.layers[0][0].window
+        if window is None:
+            raise ValueError("a rolling key/value cache needs a windowed model (window=...)")
+        return [KVCache(rolling_capacity(window), rolling=True) for _ in self.layers]
 
     @torch.no_grad()
-    def generate(self, start_tokens, seq_len, temperature=1.0, filter_thres=0.9, kv_cache=False, **kwargs):
+    def generate(self, start_tokens, seq_len, temperature=1.0, filter_thres=0.9, kv_cache=False, rolling_cache=False,
+                 **kwargs):
         """kv_cache=True: one forward over the prompt, then one token per step against the cached keys / values.
         Once the sequence is longer than max_seq_len, the window slides and its positions are re-encoded from 0, so
-        from then on each step re-fills a fresh cache with the window - the same computation as without the cache."""
+        from then on each step re-fills a fresh cache with the window - the same computation as without the cache.
+        rolling_cache=True (with kv_cache, a windowed model): the caches are rolling caches (new_cache(rolling=True))."""
         was_training = self.training
         self.eval()
         n0 = start_tokens.shape[1]
@@ -243,7 +289,7 @@ class CosineSimCausalTransformer(nn.Module):
             if not kv_cache:
                 logits = self.forward(out[:, -self.max_seq_len:], **kwargs)[:, -1, :]
             elif cache is None or out.shape[1] > self.max_seq_len:
-                cache = self.new_cache()
+                cache = self.new_cache(rolling=rolling_cache)
                 logits = self.forward(out[:, -self.max_seq_len:], cache=cache, **kwargs)[:, -1, :]
             else:
                 logits = self.forward(out[:, -1:], cache=cache, **kwargs)[:, -1, :]

@@ -329,6 +329,29 @@ int fcsa_decode_varlen(const fcsa_problem* p, const int32_t* cu_seqlens_q, int32
                        const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t groups, const fcsa_tensor* o,
                        void* workspace, size_t workspace_bytes, void* stream);
 
+/* Rolling caches for sliding-window decoding: k_cache and v_cache are rings of C = seq_k rows that keep the window's
+ * keys only, so their memory is bounded by the window instead of the sequence.  Arguments as fcsa_decode_varlen's,
+ * except that cu_seqlens_q may be NULL: the dense form, with q, o (batch, heads, seq_q, head_dim) and k_new, v_new
+ * (batch, kv_heads, seq_q, head_dim) or both NULL; total_q is then unused.
+ *   - Absolute position p lives at ring row p mod C.
+ *   - cache_seqlens[b] = L_b counts every token element b has seen, and may be far larger than C.
+ *   - The visible length is T_b = L_b + n_b with no clamp (n_b = seq_q dense, the packed length otherwise, 0 when
+ *     nothing is appended in the packed form).  The windowed rule of fcsa_decode holds over absolute positions: query i
+ *     sees key j iff 0 <= i + T_b - n_b - j < window (causal) or |i + T_b - n_b - j| < window.
+ *   - New row n of element b is written to ring row (L_b + n) mod C.
+ * Rejected with FCSA_ERR_INVALID, besides fcsa_decode_varlen's rejections: no window, C not a multiple of 128, and
+ * C < window + seq_q - 1 (seq_q = max_seqlen_q in the packed form), below which a call's append would overwrite a key
+ * that one of its own queries still sees.  L_b + n_b must stay below 2^31 - 128; the host never reads the lengths and
+ * cannot check it.  With the same number of key splits, o is bitwise what fcsa_decode or fcsa_decode_varlen give on a
+ * full-length cache holding the same keys.  `workspace`: fcsa_decode_rolling_workspace_bytes(p, cu_seqlens_q, total_q)
+ * bytes of scratch (0 for a problem it rejects).
+ */
+size_t fcsa_decode_rolling_workspace_bytes(const fcsa_problem* p, const int32_t* cu_seqlens_q, int32_t total_q);
+int fcsa_decode_rolling(const fcsa_problem* p, const int32_t* cu_seqlens_q, int32_t total_q, const fcsa_tensor* q,
+                        const fcsa_tensor* k_cache, const fcsa_tensor* v_cache, const int32_t* cache_seqlens,
+                        const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t groups, const fcsa_tensor* o,
+                        void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- packed variable-length sequences (no reference counterpart) ------------------------------------------------------
  * Training attention over B sequences of different lengths packed along the row dimension, without padding:
  *   p              : batch = B (sequences), seq_q / seq_k = maximum lengths (they size the grids and clamp the device
