@@ -125,21 +125,28 @@ int launched(cudaError_t e, const char* what) {
   return FCSA_OK;
 }
 
+// launch() between the events ev[0] / ev[1] of fcsa_set_kernel_events when they are set (ev = nullptr: untimed)
+template <typename L>
+cudaError_t timed(const cudaEvent_t* ev, cudaStream_t stream, L&& launch) {
+  if (ev && ev[0]) cudaEventRecord(ev[0], stream);
+  const cudaError_t e = launch();
+  if (ev && ev[1]) cudaEventRecord(ev[1], stream);
+  return e;
+}
+
 // A kernel as a type, so that a site can pick one of several variants and pass it to a single launch
 template <auto Kern>
 using kernel_c = std::integral_constant<decltype(Kern), Kern>;
 
-// Launch of an attention kernel: its dynamic shared memory set once per (kernel, device), then a PDL launch between
-// the events ev[0] / ev[1] when they are set.  A kernel whose parameter is the base of `args`' window arguments
-// (the unwindowed variants) receives that base.
+// Launch of an attention kernel: its dynamic shared memory set once per (kernel, device), then a timed PDL launch.
+// A kernel whose parameter is the base of `args`' window arguments (the unwindowed variants) receives that base.
 template <auto Kern, typename... Args>
 int launch_attention(const char* what, const cudaEvent_t* ev, long long grid, int threads, int smem,
                      cudaStream_t stream, const Args&... args) {
   cudaError_t e = fcsa::ensure_dynamic_smem<Kern>(smem);
   if (e != cudaSuccess) return fail(FCSA_ERR_CUDA, "cudaFuncSetAttribute(%s): %s", what, cudaGetErrorString(e));
-  if (ev && ev[0]) cudaEventRecord(ev[0], stream);
-  e = fcsa::launch_pdl(Kern, dim3((unsigned)grid), dim3(threads), smem, stream, args...);
-  if (ev && ev[1]) cudaEventRecord(ev[1], stream);
+  e = timed(ev, stream,
+            [&] { return fcsa::launch_pdl(Kern, dim3((unsigned)grid), dim3(threads), smem, stream, args...); });
   if (e != cudaSuccess) return fail(FCSA_ERR_CUDA, "%s kernel launch: %s", what, cudaGetErrorString(e));
   g_launches.fetch_add(1);
   return FCSA_OK;
@@ -230,38 +237,73 @@ fcsa::RowArgs row_args(int32_t B, int32_t D, int32_t G, const float* mul = nullp
   return a;
 }
 
+// The fused l2norm n of a checked problem over rows_batch x rows_n query rows (packed sequences: 1 x total_q): its
+// groups and rnorms.  The forward's pre-pass (prepass) also checks its inputs q, k and the q^, k^ it writes.
+int check_l2norm(const fcsa_problem* p, const fcsa_l2norm* n, int32_t rows_batch, int32_t rows_n, bool prepass = false,
+                 const fcsa_tensor* q = nullptr, const fcsa_tensor* k = nullptr) {
+  int r;
+  if ((r = check_rows(false, p->dtype, rows_batch, p->heads, rows_n, p->head_dim, n->groups))) return r;
+  if (prepass && ((r = check_tensor(q, "q")) || (r = check_tensor(k, "k")) || (r = check_tensor(&n->q_hat, "q_hat")) ||
+                  (r = check_tensor(&n->k_hat, "k_hat"))))
+    return r;
+  if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
+  return FCSA_OK;
+}
+
+// The q / k l2norm pre-pass of the fused forwards: q^, k^ and their rnorms over B batches of Nq query and Nk key rows
+// (packed sequences: one batch of total_q / total_k)
+int l2norm_qk(const fcsa_problem* p, const fcsa_l2norm* n, const fcsa_tensor* q, const fcsa_tensor* k, int32_t B,
+              int32_t Nq, int32_t Nk, cudaStream_t s) {
+  int r;
+  if ((r = check_l2norm(p, n, B, Nq, true, q, k))) return r;
+  fcsa::RowArgs a = row_args(B, p->head_dim, n->groups);
+  a.t[0] = {p->heads, Nq, *q, n->q_hat, {}, n->q_rnorm};
+  a.t[1] = {p->kv_heads, Nk, *k, n->k_hat, {}, n->k_rnorm};
+  return launched(timed(g_ev[2], s, [&] { return fcsa::launch_row_fwd(a, p->dtype == FCSA_BF16, false, s); }),
+                  "l2norm (q, k) launch");
+}
+
 // ---- key/value-cache decode --------------------------------------------------------------------
-// The problem of a decode call: seq_q = new queries, seq_k = cache capacity; no key mask, 16-bit output.
-int check_decode_problem(const fcsa_problem* p, int32_t n_new) {
+// A decode call (fcsa_decode, fcsa_decode_varlen, fcsa_decode_rolling): seq_q = new queries (packed: the longest
+// sequence's), seq_k = cache capacity.
+struct DecodeCall {
+  const char* who;        // the route's message prefix
+  bool packed;            // total_q new rows, sequence b owning [cu[b], cu[b + 1]); dense: batch x seq_q
+  const int32_t* cu;
+  int32_t total_q;
+  int32_t n_new;          // fcsa_decode: rows appended per sequence; the other routes append when k_new, v_new are set
+  bool ring;              // rolling caches of seq_k rows
+};
+
+// The checks of decode call c, in the order the routes report them.  A workspace-size query (query = true) has no
+// cu_seqlens_q or k_new / v_new to check.
+int check_decode(const fcsa_problem* p, const DecodeCall& c, bool query, const fcsa_tensor* k_new = nullptr,
+                 const fcsa_tensor* v_new = nullptr) {
+  if (c.packed && p && p->seq_q < 0)
+    return fail(FCSA_ERR_INVALID, "decode varlen: max_seqlen_q (seq_q) %d < 0", p->seq_q);
   int r;
   if ((r = check_problem(p))) return r;
   if (p->key_mask) return fail(FCSA_ERR_UNSUPPORTED, "decode: no key mask (cache_seqlens gives the valid rows)");
   if (p->out_f32) return fail(FCSA_ERR_UNSUPPORTED, "decode: out_f32 is not implemented");
-  if (n_new < 0) return fail(FCSA_ERR_INVALID, "decode: n_new %d < 0", n_new);
+  if (c.n_new < 0) return fail(FCSA_ERR_INVALID, "decode: n_new %d < 0", c.n_new);
   if ((long long)(p->heads / p->kv_heads) * p->seq_q > 0x7FFFFFFFLL - 64)
     return fail(FCSA_ERR_INVALID, "decode: heads per kv head x seq_q too large");
-  return FCSA_OK;
-}
-
-// The problem of a packed decode call: check_decode_problem's with seq_q = max_seqlen_q, and total_q packed rows
-int check_decode_varlen(const fcsa_problem* p, int32_t total_q) {
-  if (p && p->seq_q < 0) return fail(FCSA_ERR_INVALID, "decode varlen: max_seqlen_q (seq_q) %d < 0", p->seq_q);
-  int r;
-  if ((r = check_decode_problem(p, 0))) return r;
-  if (total_q < 0) return fail(FCSA_ERR_INVALID, "decode varlen: total_q %d < 0", total_q);
-  return FCSA_OK;
-}
-
-// A rolling cache (fcsa_decode_rolling) of C = seq_k rows for seq_q new queries (packed: the longest): it needs a
-// window, whole 128-row tiles (a tile never straddles the wrap), and C >= W + seq_q - 1, so that the keys a call sees,
-// [T_b - seq_q - W + 1, T_b), are not overwritten by its own append.
-int check_decode_ring(const fcsa_problem* p) {
-  if (p->window <= 0) return fail(FCSA_ERR_INVALID, "decode rolling: a rolling cache needs a window");
-  if (p->seq_k % 128 != 0)
+  if (c.packed && c.total_q < 0) return fail(FCSA_ERR_INVALID, "decode varlen: total_q %d < 0", c.total_q);
+  // A rolling cache of C = seq_k rows needs a window, whole 128-row tiles (a tile never straddles the wrap), and
+  // C >= W + seq_q - 1, so that the keys a call sees, [T_b - seq_q - W + 1, T_b), are not overwritten by its own
+  // append.
+  if (c.ring && p->window <= 0) return fail(FCSA_ERR_INVALID, "decode rolling: a rolling cache needs a window");
+  if (c.ring && p->seq_k % 128 != 0)
     return fail(FCSA_ERR_INVALID, "decode rolling: cache rows %d must be a multiple of 128", p->seq_k);
-  if ((long long)p->seq_k < (long long)p->window + p->seq_q - 1)
+  if (c.ring && (long long)p->seq_k < (long long)p->window + p->seq_q - 1)
     return fail(FCSA_ERR_INVALID, "decode rolling: cache rows %d < window %d + new queries %d - 1", p->seq_k,
                 p->window, p->seq_q);
+  if (query) return FCSA_OK;
+  if (c.packed && !c.cu) return fail(FCSA_ERR_INVALID, "%snull cu_seqlens_q", c.who);
+  if (reinterpret_cast<uintptr_t>(c.cu) & 3)
+    return fail(FCSA_ERR_INVALID, "%scu_seqlens_q must be a 4-byte aligned int32 array", c.who);
+  if ((c.packed || c.ring) && (k_new == nullptr) != (v_new == nullptr))
+    return fail(FCSA_ERR_INVALID, "%spass both k_new and v_new, or neither", c.who);
   return FCSA_OK;
 }
 
@@ -285,15 +327,28 @@ int decode_shape(const fcsa_problem* p, DecodeShape* s) {
 
 size_t align16(size_t n) { return (n + 15) & ~size_t(15); }
 
-// q^ of `rows` query rows (batch x seq_q, or the packed total_q)
-size_t decode_qhat_bytes(const fcsa_problem* p, size_t rows) { return align16(rows * p->heads * p->head_dim * 2); }
+// The scratch of decode call c: q^ of its query rows, then the partials of its splits
+size_t decode_qhat_bytes(const fcsa_problem* p, const DecodeCall& c) {
+  const size_t rows = c.packed ? (size_t)c.total_q : (size_t)p->batch * p->seq_q;
+  return align16(rows * p->heads * p->head_dim * 2);
+}
 
-// cu, total_q: packed new tokens (DecodeArgs::cu_q), nullptr = dense; n_new is then 1 (appended) or 0.  ring: the
-// caches are rolling caches of seq_k rows (checked by check_decode_ring)
+size_t decode_bytes(const fcsa_problem* p, const DecodeCall& c, const DecodeShape& sh) {
+  return decode_qhat_bytes(p, c) + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
+}
+
+// The workspace-size query of decode call c: 0 for a refused problem
+size_t decode_workspace_bytes(const fcsa_problem* p, const DecodeCall& c) {
+  DecodeShape sh;
+  if (check_decode(p, c, true) || decode_shape(p, &sh)) return 0;
+  return decode_bytes(p, c, sh);
+}
+
+// n_new: rows appended per sequence (packed: 1 when appending, else 0)
 template <typename T, int D>
-int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tensor* q, const fcsa_tensor* kc,
-                  const fcsa_tensor* vc, const int32_t* seqlens, int32_t n_new, const fcsa_tensor* o, float* part,
-                  const int32_t* cu, int32_t total_q, bool ring, cudaStream_t stream) {
+int launch_decode(const fcsa_problem* p, const DecodeCall& c, const DecodeShape& sh, const fcsa_tensor* q,
+                  const fcsa_tensor* kc, const fcsa_tensor* vc, const int32_t* seqlens, int32_t n_new,
+                  const fcsa_tensor* o, float* part, cudaStream_t stream) {
   using Cfg = fcsa::DecodeCfg<D>;
   CUtensorMap tk, tv;
   int r;
@@ -309,13 +364,13 @@ int launch_decode(const fcsa_problem* p, const DecodeShape& sh, const fcsa_tenso
   const float log2e = 1.4426950408889634f;
   a.c1 = p->scale * log2e;
   a.c2 = p->shift * log2e;
-  a.ring = ring ? p->seq_k : 0;
+  a.ring = c.ring ? p->seq_k : 0;
   a.seqlens = seqlens;
   a.q = q->ptr; a.q_sb = q->sb; a.q_sh = q->sh; a.q_sn = q->sn;
   a.o = o->ptr; a.o_sb = o->sb; a.o_sh = o->sh; a.o_sn = o->sn;
   a.part = part;
-  a.cu_q = cu; a.total_q = total_q;
-  if (cu) a.q_sb = a.o_sb = 0;
+  a.cu_q = c.cu; a.total_q = c.total_q;
+  if (c.cu) a.q_sb = a.o_sb = 0;
   const long long grid = sh.items * sh.n_split;
   if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "decode: problem too large for one launch");
   const auto launch = [&](auto kern) {
@@ -362,15 +417,20 @@ int launch_varlen_tail(const fcsa_problem* p, fcsa::TailArgs a, int n, cudaStrea
 }
 
 // ---- backward ------------------------------------------------------------------------------------
-// The backward's workspaces: dense, or packed sequences (vl)
-fcsa::BwdWorkspace bwd_layout(const fcsa_problem* p, const fcsa_varlen* vl) {
-  if (vl)
-    return fcsa::bwd_varlen_workspace_layout(p->batch, p->heads, p->kv_heads, vl->total_q, vl->total_k, p->head_dim);
-  return fcsa::bwd_workspace_layout(p->batch, p->heads, p->kv_heads, p->seq_q, p->seq_k, p->head_dim);
-}
+// The backward's workspace layout, dense or packed sequences (vl), and the scratch and zeroed bytes its route needs.
+// The deterministic route takes the stats alone as scratch (no dq accumulator, and no dk / dv accumulators:
+// split = 1) and no zeroed workspace.
+struct BwdNeed {
+  fcsa::BwdWorkspace w;
+  size_t scratch, zeroed;
+};
 
-// The deterministic backward's scratch: the stats alone (no dq accumulator, and no dk / dv accumulators: split = 1)
-size_t bwd_deterministic_bytes(const fcsa::BwdWorkspace& w) { return w.dkv_off; }
+BwdNeed bwd_need(const fcsa_problem* p, const fcsa_varlen* vl, bool deterministic) {
+  const fcsa::BwdWorkspace w =
+      vl ? fcsa::bwd_varlen_workspace_layout(p->batch, p->heads, p->kv_heads, vl->total_q, vl->total_k, p->head_dim)
+         : fcsa::bwd_workspace_layout(p->batch, p->heads, p->kv_heads, p->seq_q, p->seq_k, p->head_dim);
+  return {w, deterministic ? w.dkv_off : w.total, deterministic ? 0 : w.ztotal};
+}
 
 // The backward's arguments, filled from the problem and the caller's tensors by backward_impl
 struct BwdHostArgs {
@@ -441,7 +501,7 @@ int launch_dq(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, const float* st
 
 // The backward's launches: preprocess, main kernel, dq finish, and for split groups the dk / dv finish (and the l2norm
 // backward of dk).  Deterministic: preprocess, the dK / dV kernel with split = 1, the dQ kernel.  w: the workspaces'
-// layout (bwd_layout).
+// layout (bwd_need).
 template <typename T, int D, bool BIAS = false, bool VARLEN = false>
 int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream_t stream) {
   using namespace fcsa;
@@ -489,9 +549,9 @@ int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream
     pa.bpb = (padded + rows_per_block - 1) / rows_per_block;
     const long long grid = (long long)pa.bpb * h.B * h.H;
     if (grid > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
-    if (g_ev[3][0]) cudaEventRecord(g_ev[3][0], stream);
-    e = launch_pdl(bwd_prep_kernel<T, D / 8, VARLEN>, dim3((unsigned)grid), dim3(256), 0, stream, pa);
-    if (g_ev[3][1]) cudaEventRecord(g_ev[3][1], stream);
+    e = timed(g_ev[3], stream, [&] {
+      return launch_pdl(bwd_prep_kernel<T, D / 8, VARLEN>, dim3((unsigned)grid), dim3(256), 0, stream, pa);
+    });
     if ((r = launched(e, "backward preprocess launch"))) return r;
   }
   // 2. main
@@ -575,9 +635,9 @@ int run_backward_t(const BwdHostArgs& h, const fcsa::BwdWorkspace& w, cudaStream
     const long long threads = (long long)h.B * h.H * (VARLEN ? fa.padded : h.Nq) * (D / 8);
     const long long blocks = VARLEN ? (threads + 255) / 256 : (threads + 511) / 512;   // dense: two rows per thread
     if (blocks > 0x7FFFFFFFLL) return fail(FCSA_ERR_INVALID, "problem too large for one launch");
-    if (g_ev[4][0]) cudaEventRecord(g_ev[4][0], stream);
-    e = launch_pdl(bwd_dq_finish_kernel<T, D, VARLEN>, dim3((unsigned)blocks), dim3(256), 0, stream, fa);
-    if (g_ev[4][1]) cudaEventRecord(g_ev[4][1], stream);
+    e = timed(g_ev[4], stream, [&] {
+      return launch_pdl(bwd_dq_finish_kernel<T, D, VARLEN>, dim3((unsigned)blocks), dim3(256), 0, stream, fa);
+    });
     if ((r = launched(e, "dq finish launch"))) return r;
     if (to_acc) {
       for (int which = 0; which < 2; ++which) {
@@ -651,13 +711,11 @@ int fcsa_forward_bias(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_te
 }
 
 size_t fcsa_backward_workspace_bytes(const fcsa_problem* p) {
-  if (check_problem(p)) return 0;
-  return fcsa::bwd_workspace_bytes(p->batch, p->heads, p->kv_heads, p->seq_q, p->seq_k, p->head_dim);
+  return check_problem(p) ? 0 : bwd_need(p, nullptr, false).scratch;
 }
 
 size_t fcsa_backward_zeroed_bytes(const fcsa_problem* p) {
-  if (check_problem(p)) return 0;
-  return fcsa::bwd_zeroed_workspace_bytes(p->batch, p->heads, p->kv_heads, p->seq_q, p->seq_k, p->head_dim);
+  return check_problem(p) ? 0 : bwd_need(p, nullptr, false).zeroed;
 }
 
 int fcsa_zeroed_init(void* zeroed, size_t bytes, void* stream) {
@@ -669,7 +727,8 @@ int fcsa_zeroed_init(void* zeroed, size_t bytes, void* stream) {
 
 // Every backward entry point: dense or packed sequences (vl), with the fused l2norm backward over `groups` when
 // q_rnorm / k_rnorm are set (q, k are then the normalised tensors), or with a bias.  deterministic: the route without
-// atomics, which needs the stats alone as scratch and no zeroed workspace (zeroed is ignored).
+// atomics, which needs the stats alone as scratch and no zeroed workspace (zeroed is ignored).  Packed sequences end
+// with zero gradients in the rows outside every sequence.
 static int backward_impl(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_tensor* q, const fcsa_tensor* k,
                          const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o,
                          const float* inv_l, const fcsa_tensor* dq, const fcsa_tensor* dk,
@@ -686,14 +745,13 @@ static int backward_impl(const fcsa_problem* p, const fcsa_varlen* vl, const fcs
       (r = check_tensor(dk, "dk")) || (r = check_tensor(dv, "dv")))
     return r;
   if (!inv_l) return fail(FCSA_ERR_INVALID, "inv_l: null");
-  const fcsa::BwdWorkspace w = bwd_layout(p, vl);
-  const size_t need = deterministic ? bwd_deterministic_bytes(w) : w.total;
-  if (!workspace || workspace_bytes < need)
-    return fail(FCSA_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need, workspace_bytes);
+  const BwdNeed need = bwd_need(p, vl, deterministic);
+  if (!workspace || workspace_bytes < need.scratch)
+    return fail(FCSA_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need.scratch, workspace_bytes);
   if (!aligned16(workspace)) return fail(FCSA_ERR_INVALID, "workspace not 16-byte aligned");
   if (!deterministic) {
-    if (!zeroed || zeroed_bytes < w.ztotal)
-      return fail(FCSA_ERR_WORKSPACE, "zeroed workspace too small: need %zu bytes, got %zu", w.ztotal, zeroed_bytes);
+    if (!zeroed || zeroed_bytes < need.zeroed)
+      return fail(FCSA_ERR_WORKSPACE, "zeroed workspace too small: need %zu bytes, got %zu", need.zeroed, zeroed_bytes);
     if (!aligned16(zeroed)) return fail(FCSA_ERR_INVALID, "zeroed workspace not 16-byte aligned");
   }
   if (p->out_f32 && (q_rnorm || k_rnorm))
@@ -723,13 +781,38 @@ static int backward_impl(const fcsa_problem* p, const fcsa_varlen* vl, const fcs
     h.total_q = vl->total_q; h.total_k = vl->total_k;
   }
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  return dispatch(p, [&](auto t, auto d) {
+  r = dispatch(p, [&](auto t, auto d) {
     using T = typename decltype(t)::type;
     constexpr int D = decltype(d)::value;
-    if (vl) return run_backward_t<T, D, false, true>(h, w, s);   // (packed sequences take no bias)
-    if (bias) return run_backward_t<T, D, true>(h, w, s);
-    return run_backward_t<T, D>(h, w, s);
+    if (vl) return run_backward_t<T, D, false, true>(h, need.w, s);   // (packed sequences take no bias)
+    if (bias) return run_backward_t<T, D, true>(h, need.w, s);
+    return run_backward_t<T, D>(h, need.w, s);
   });
+  if (r || !vl) return r;
+  fcsa::TailArgs ta = {};
+  ta.t[0] = {dq->ptr, dq->sh, dq->sn, p->heads, vl->total_q, vl->cu_seqlens_q};
+  ta.t[1] = {dk->ptr, dk->sh, dk->sn, p->kv_heads, vl->total_k, vl->cu_seqlens_k};
+  ta.t[2] = {dv->ptr, dv->sh, dv->sn, p->kv_heads, vl->total_k, vl->cu_seqlens_k};
+  return launch_varlen_tail(p, ta, 3, s);
+}
+
+// The backward entry points that take the fused l2norm's outputs n (q^, k^ and their rnorms): dense, or packed
+// sequences (the varlen entry points, whose vl must be set).  groups = 0 is the plain backward of q^, k^, except in
+// fcsa_backward_fused.
+static int backward_l2norm(const fcsa_problem* p, bool packed, const fcsa_varlen* vl, const fcsa_l2norm* n,
+                           const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
+                           const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv, void* workspace,
+                           size_t workspace_bytes, void* zeroed, size_t zeroed_bytes, void* stream,
+                           bool deterministic) {
+  int r;
+  if (packed && (r = check_varlen(p, vl))) return r;
+  if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
+  if (!packed && (r = check_problem(p))) return r;
+  const bool fused = n->groups != 0 || (!vl && !deterministic);
+  if (fused && (r = check_l2norm(p, n, vl ? 1 : p->batch, vl ? vl->total_q : p->seq_q))) return r;
+  return backward_impl(p, vl, &n->q_hat, &n->k_hat, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed,
+                       zeroed_bytes, stream, fused ? n->q_rnorm : nullptr, fused ? n->k_rnorm : nullptr,
+                       fused ? n->groups : 1, deterministic);
 }
 
 int fcsa_backward(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k,
@@ -757,19 +840,7 @@ int fcsa_forward_fused(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_t
   int r;
   if ((r = check_problem(p))) return r;
   if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
-  if ((r = check_rows(false, p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, n->groups))) return r;
-  if ((r = check_tensor(q, "q")) || (r = check_tensor(k, "k")) || (r = check_tensor(&n->q_hat, "q_hat")) ||
-      (r = check_tensor(&n->k_hat, "k_hat")))
-    return r;
-  if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
-  fcsa::RowArgs a = row_args(p->batch, p->head_dim, n->groups);
-  a.t[0] = {p->heads, p->seq_q, *q, n->q_hat, {}, n->q_rnorm};
-  a.t[1] = {p->kv_heads, p->seq_k, *k, n->k_hat, {}, n->k_rnorm};
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  if (g_ev[2][0]) cudaEventRecord(g_ev[2][0], s);
-  const cudaError_t e = fcsa::launch_row_fwd(a, p->dtype == FCSA_BF16, false, s);
-  if (g_ev[2][1]) cudaEventRecord(g_ev[2][1], s);
-  if ((r = launched(e, "l2norm (q, k) launch"))) return r;
+  if ((r = l2norm_qk(p, n, q, k, p->batch, p->seq_q, p->seq_k, reinterpret_cast<cudaStream_t>(stream)))) return r;
   return fcsa_forward(p, &n->q_hat, &n->k_hat, v, o, inv_l, stream);
 }
 
@@ -778,35 +849,20 @@ int fcsa_backward_fused(const fcsa_problem* p, const fcsa_l2norm* n, const fcsa_
                         const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv,
                         void* workspace, size_t workspace_bytes, void* zeroed, size_t zeroed_bytes,
                         void* stream) {
-  if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
-  int r;
-  if ((r = check_problem(p))) return r;
-  if ((r = check_rows(false, p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, n->groups))) return r;
-  if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
-  return backward_impl(p, nullptr, &n->q_hat, &n->k_hat, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes,
-                       zeroed, zeroed_bytes, stream, n->q_rnorm, n->k_rnorm, n->groups, false);
+  return backward_l2norm(p, false, nullptr, n, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed,
+                         zeroed_bytes, stream, false);
 }
 
 size_t fcsa_backward_fused_deterministic_workspace_bytes(const fcsa_problem* p) {
-  if (check_problem(p)) return 0;
-  return bwd_deterministic_bytes(bwd_layout(p, nullptr));
+  return check_problem(p) ? 0 : bwd_need(p, nullptr, true).scratch;
 }
 
 int fcsa_backward_fused_deterministic(const fcsa_problem* p, const fcsa_l2norm* n, const fcsa_tensor* v,
                                       const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
                                       const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv,
                                       void* workspace, size_t workspace_bytes, void* stream) {
-  if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
-  int r;
-  if ((r = check_problem(p))) return r;
-  const bool fused = n->groups != 0;
-  if (fused) {
-    if ((r = check_rows(false, p->dtype, p->batch, p->heads, p->seq_q, p->head_dim, n->groups))) return r;
-    if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
-  }
-  return backward_impl(p, nullptr, &n->q_hat, &n->k_hat, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes,
-                       nullptr, 0, stream, fused ? n->q_rnorm : nullptr, fused ? n->k_rnorm : nullptr,
-                       fused ? n->groups : 1, true);
+  return backward_l2norm(p, false, nullptr, n, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, nullptr, 0,
+                         stream, true);
 }
 
 int fcsa_f32_cast(int32_t dtype, int32_t batch, int32_t heads, int32_t rows, int32_t head_dim, int32_t groups,
@@ -867,28 +923,28 @@ int fcsa_l2norm_backward(int32_t dtype, int32_t batch, int32_t heads, int32_t ro
                   "l2norm backward launch");
 }
 
-// fcsa_decode, fcsa_decode_varlen and fcsa_decode_rolling: dense, or packed new tokens (cu != nullptr: q, o, k_new,
-// v_new are total_q rows, sequence b owning [cu[b], cu[b + 1]); appending when k_new and v_new are set, n_new unused),
-// into full-length or (ring) rolling caches
-static int decode_impl(const fcsa_problem* p, const int32_t* cu, int32_t total_q, const fcsa_tensor* q,
-                       const fcsa_tensor* k_cache, const fcsa_tensor* v_cache, const int32_t* cache_seqlens,
-                       const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t n_new, int32_t groups,
-                       const fcsa_tensor* o, void* workspace, size_t workspace_bytes, void* stream, bool ring = false) {
+// fcsa_decode, fcsa_decode_varlen and fcsa_decode_rolling: decode call c (packed: q, o, k_new, v_new are total_q rows)
+static int decode_impl(const fcsa_problem* p, const DecodeCall& c, const fcsa_tensor* q, const fcsa_tensor* k_cache,
+                       const fcsa_tensor* v_cache, const int32_t* cache_seqlens, const fcsa_tensor* k_new,
+                       const fcsa_tensor* v_new, int32_t groups, const fcsa_tensor* o, void* workspace,
+                       size_t workspace_bytes, void* stream) {
   int r;
-  const bool append = cu ? (k_new != nullptr || v_new != nullptr) : n_new > 0;
+  if ((r = check_decode(p, c, false, k_new, v_new))) return r;
+  const bool append = c.packed || c.ring ? k_new != nullptr : c.n_new > 0;
+  // rows appended per sequence (packed: 1, each sequence appending its own rows); a dense rolling call one per query
+  const int32_t n_new = !append ? 0 : c.packed ? 1 : c.ring ? p->seq_q : c.n_new;
   if ((r = check_tensor(q, "q")) || (r = check_tensor(k_cache, "k_cache")) || (r = check_tensor(v_cache, "v_cache")) ||
       (r = check_tensor(o, "o")))
     return r;
   if (append && ((r = check_tensor(k_new, "k")) || (r = check_tensor(v_new, "v")))) return r;
-  if (cu && total_q == 0) return FCSA_OK;
+  if (c.packed && c.total_q == 0) return FCSA_OK;
   // the row pass's shape: the batch's rows, or the packed rows as one batch
-  const int32_t rB = cu ? 1 : p->batch, rN = cu ? total_q : p->seq_q;
+  const int32_t rB = c.packed ? 1 : p->batch, rN = c.packed ? c.total_q : p->seq_q;
   if (groups != 0 && (r = check_rows(false, p->dtype, rB, p->heads, rN, p->head_dim, groups))) return r;
   if (!cache_seqlens) return fail(FCSA_ERR_INVALID, "cache_seqlens: null");
   DecodeShape sh;
   if ((r = decode_shape(p, &sh))) return r;
-  const size_t qbytes = decode_qhat_bytes(p, (size_t)rB * rN);
-  const size_t need = qbytes + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
+  const size_t need = decode_bytes(p, c, sh);
   if (!workspace || workspace_bytes < need)
     return fail(FCSA_ERR_WORKSPACE, "workspace too small: need %zu bytes, got %zu", need, workspace_bytes);
   if (!aligned16(workspace)) return fail(FCSA_ERR_INVALID, "workspace not 16-byte aligned");
@@ -900,95 +956,65 @@ static int decode_impl(const fcsa_problem* p, const int32_t* cu, int32_t total_q
   const int64_t H = p->heads, N = rN, D = p->head_dim;
   const fcsa_tensor qhat = {workspace, H * N * D, N * D, D};
   fcsa::RowArgs a = row_args(rB, p->head_dim, groups);
-  const int32_t n_app = cu ? total_q : n_new;
+  const int32_t n_app = c.packed ? c.total_q : n_new;
   int n = 0;
   if (groups > 0) a.t[n++] = {p->heads, rN, *q, qhat, {}, nullptr, nullptr, rN, 0};
   if (append) {
-    const uint8_t k_raw = groups == 0 ? 1 : 0, rolling = ring ? 1 : 0;
-    a.t[n++] = {p->kv_heads, n_app, *k_new, *k_cache, {}, nullptr, cache_seqlens, p->seq_k, k_raw, rolling, cu,
+    const uint8_t k_raw = groups == 0 ? 1 : 0, rolling = c.ring ? 1 : 0;
+    a.t[n++] = {p->kv_heads, n_app, *k_new, *k_cache, {}, nullptr, cache_seqlens, p->seq_k, k_raw, rolling, c.cu,
                 p->batch, p->seq_q};
-    a.t[n++] = {p->kv_heads, n_app, *v_new, *v_cache, {}, nullptr, cache_seqlens, p->seq_k, 1, rolling, cu, p->batch,
-                p->seq_q};
+    a.t[n++] = {p->kv_heads, n_app, *v_new, *v_cache, {}, nullptr, cache_seqlens, p->seq_k, 1, rolling, c.cu,
+                p->batch, p->seq_q};
   }
   if (n > 0 && (r = launched(fcsa::launch_row_append(a, n, p->dtype == FCSA_BF16, s), "append pass launch")))
     return r;
 
   const fcsa_tensor* qa = groups > 0 ? &qhat : q;
-  float* part = reinterpret_cast<float*>(static_cast<char*>(workspace) + qbytes);
+  float* part = reinterpret_cast<float*>(static_cast<char*>(workspace) + decode_qhat_bytes(p, c));
   r = dispatch(p, [&](auto t, auto d) {
-    return launch_decode<typename decltype(t)::type, decltype(d)::value>(
-        p, sh, qa, k_cache, v_cache, cache_seqlens, cu ? (append ? 1 : 0) : n_new, o, part, cu, total_q, ring, s);
+    return launch_decode<typename decltype(t)::type, decltype(d)::value>(p, c, sh, qa, k_cache, v_cache, cache_seqlens,
+                                                                         n_new, o, part, s);
   });
-  if (r || !cu) return r;
+  if (r || !c.packed) return r;
   // o = 0 in the rows outside every sequence
   fcsa::TailArgs ta = {};
-  ta.t[0] = {o->ptr, o->sh, o->sn, p->heads, total_q, cu};
+  ta.t[0] = {o->ptr, o->sh, o->sn, p->heads, c.total_q, c.cu};
   return launch_varlen_tail(p, ta, 1, s);
 }
 
 size_t fcsa_decode_workspace_bytes(const fcsa_problem* p, int32_t n_new) {
-  DecodeShape sh;
-  if (check_decode_problem(p, n_new) || decode_shape(p, &sh)) return 0;
-  return decode_qhat_bytes(p, (size_t)p->batch * p->seq_q) + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
+  return decode_workspace_bytes(p, {"decode: ", false, nullptr, 0, n_new, false});
 }
 
 int fcsa_decode(const fcsa_problem* p, const fcsa_tensor* q, const fcsa_tensor* k_cache, const fcsa_tensor* v_cache,
                 const int32_t* cache_seqlens, const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t n_new,
                 int32_t groups, const fcsa_tensor* o, void* workspace, size_t workspace_bytes, void* stream) {
-  int r;
-  if ((r = check_decode_problem(p, n_new))) return r;
-  return decode_impl(p, nullptr, 0, q, k_cache, v_cache, cache_seqlens, k_new, v_new, n_new, groups, o, workspace,
-                     workspace_bytes, stream);
+  return decode_impl(p, {"decode: ", false, nullptr, 0, n_new, false}, q, k_cache, v_cache, cache_seqlens, k_new, v_new,
+                     groups, o, workspace, workspace_bytes, stream);
 }
 
 size_t fcsa_decode_varlen_workspace_bytes(const fcsa_problem* p, int32_t total_q) {
-  DecodeShape sh;
-  if (check_decode_varlen(p, total_q) || decode_shape(p, &sh)) return 0;
-  return decode_qhat_bytes(p, (size_t)total_q) + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
+  return decode_workspace_bytes(p, {"decode varlen: ", true, nullptr, total_q, 0, false});
 }
 
 int fcsa_decode_varlen(const fcsa_problem* p, const int32_t* cu_seqlens_q, int32_t total_q, const fcsa_tensor* q,
                        const fcsa_tensor* k_cache, const fcsa_tensor* v_cache, const int32_t* cache_seqlens,
                        const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t groups, const fcsa_tensor* o,
                        void* workspace, size_t workspace_bytes, void* stream) {
-  int r;
-  if ((r = check_decode_varlen(p, total_q))) return r;
-  if (!cu_seqlens_q) return fail(FCSA_ERR_INVALID, "decode varlen: null cu_seqlens_q");
-  if (reinterpret_cast<uintptr_t>(cu_seqlens_q) & 3)
-    return fail(FCSA_ERR_INVALID, "decode varlen: cu_seqlens_q must be a 4-byte aligned int32 array");
-  if ((k_new == nullptr) != (v_new == nullptr))
-    return fail(FCSA_ERR_INVALID, "decode varlen: pass both k_new and v_new, or neither");
-  return decode_impl(p, cu_seqlens_q, total_q, q, k_cache, v_cache, cache_seqlens, k_new, v_new, 0, groups, o,
-                     workspace, workspace_bytes, stream);
-}
-
-// The problem of a rolling-cache call: check_decode_problem's (dense) or check_decode_varlen's (packed), then the ring's
-static int check_decode_rolling(const fcsa_problem* p, const int32_t* cu, int32_t total_q) {
-  int r;
-  if ((r = cu ? check_decode_varlen(p, total_q) : check_decode_problem(p, 0))) return r;
-  return check_decode_ring(p);
+  return decode_impl(p, {"decode varlen: ", true, cu_seqlens_q, total_q, 0, false}, q, k_cache, v_cache, cache_seqlens,
+                     k_new, v_new, groups, o, workspace, workspace_bytes, stream);
 }
 
 size_t fcsa_decode_rolling_workspace_bytes(const fcsa_problem* p, const int32_t* cu_seqlens_q, int32_t total_q) {
-  DecodeShape sh;
-  if (check_decode_rolling(p, cu_seqlens_q, total_q) || decode_shape(p, &sh)) return 0;
-  const size_t rows = cu_seqlens_q ? (size_t)total_q : (size_t)p->batch * p->seq_q;
-  return decode_qhat_bytes(p, rows) + fcsa::decode_partial_bytes(sh.items, sh.n_split, p->head_dim);
+  return decode_workspace_bytes(p, {"decode rolling: ", cu_seqlens_q != nullptr, cu_seqlens_q, total_q, 0, true});
 }
 
 int fcsa_decode_rolling(const fcsa_problem* p, const int32_t* cu_seqlens_q, int32_t total_q, const fcsa_tensor* q,
                         const fcsa_tensor* k_cache, const fcsa_tensor* v_cache, const int32_t* cache_seqlens,
                         const fcsa_tensor* k_new, const fcsa_tensor* v_new, int32_t groups, const fcsa_tensor* o,
                         void* workspace, size_t workspace_bytes, void* stream) {
-  int r;
-  if ((r = check_decode_rolling(p, cu_seqlens_q, total_q))) return r;
-  if (reinterpret_cast<uintptr_t>(cu_seqlens_q) & 3)
-    return fail(FCSA_ERR_INVALID, "decode rolling: cu_seqlens_q must be a 4-byte aligned int32 array");
-  if ((k_new == nullptr) != (v_new == nullptr))
-    return fail(FCSA_ERR_INVALID, "decode rolling: pass both k_new and v_new, or neither");
-  const int32_t n_new = !cu_seqlens_q && k_new ? p->seq_q : 0;
-  return decode_impl(p, cu_seqlens_q, total_q, q, k_cache, v_cache, cache_seqlens, k_new, v_new, n_new, groups, o,
-                     workspace, workspace_bytes, stream, true);
+  return decode_impl(p, {"decode rolling: ", cu_seqlens_q != nullptr, cu_seqlens_q, total_q, 0, true}, q, k_cache,
+                     v_cache, cache_seqlens, k_new, v_new, groups, o, workspace, workspace_bytes, stream);
 }
 
 int fcsa_forward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_tensor* q, const fcsa_tensor* k,
@@ -1001,22 +1027,10 @@ int fcsa_forward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, cons
       (r = check_tensor(o, "o")))
     return r;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  const fcsa_tensor *qa = q, *ka = k;
-  if (n->groups != 0) {
-    // the row pass runs over the packed rows as one batch: rnorm is [heads][total][groups]
-    if ((r = check_rows(false, p->dtype, 1, p->heads, vl->total_q, p->head_dim, n->groups))) return r;
-    if ((r = check_tensor(&n->q_hat, "q_hat")) || (r = check_tensor(&n->k_hat, "k_hat"))) return r;
-    if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
-    fcsa::RowArgs a = row_args(1, p->head_dim, n->groups);
-    a.t[0] = {p->heads, vl->total_q, *q, n->q_hat, {}, n->q_rnorm};
-    a.t[1] = {p->kv_heads, vl->total_k, *k, n->k_hat, {}, n->k_rnorm};
-    if (g_ev[2][0]) cudaEventRecord(g_ev[2][0], s);
-    const cudaError_t e = fcsa::launch_row_fwd(a, p->dtype == FCSA_BF16, false, s);
-    if (g_ev[2][1]) cudaEventRecord(g_ev[2][1], s);
-    if ((r = launched(e, "l2norm (q, k) launch"))) return r;
-    qa = &n->q_hat;
-    ka = &n->k_hat;
-  }
+  // the row pass runs over the packed rows as one batch: rnorm is [heads][total][groups]
+  const bool fused = n->groups != 0;
+  if (fused && (r = l2norm_qk(p, n, q, k, 1, vl->total_q, vl->total_k, s))) return r;
+  const fcsa_tensor *qa = fused ? &n->q_hat : q, *ka = fused ? &n->k_hat : k;
   r = dispatch(p, [&](auto t, auto d) {
     return launch_forward<typename decltype(t)::type, decltype(d)::value, false, true>(p, qa, ka, v, o, inv_l, s,
                                                                                        nullptr, vl);
@@ -1029,52 +1043,23 @@ int fcsa_forward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, cons
 }
 
 size_t fcsa_backward_fused_varlen_workspace_bytes(const fcsa_problem* p, const fcsa_varlen* vl) {
-  if (check_varlen(p, vl)) return 0;
-  return bwd_layout(p, vl).total;
+  return check_varlen(p, vl) ? 0 : bwd_need(p, vl, false).scratch;
 }
 
 size_t fcsa_backward_fused_varlen_zeroed_bytes(const fcsa_problem* p, const fcsa_varlen* vl) {
-  if (check_varlen(p, vl)) return 0;
-  return bwd_layout(p, vl).ztotal;
-}
-
-// fcsa_backward_fused_varlen and its deterministic twin (zeroed unused)
-static int backward_varlen_impl(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_l2norm* n,
-                                const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
-                                const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv, void* workspace,
-                                size_t workspace_bytes, void* zeroed, size_t zeroed_bytes, void* stream,
-                                bool deterministic) {
-  int r;
-  if ((r = check_varlen(p, vl))) return r;
-  if (!n) return fail(FCSA_ERR_INVALID, "null fcsa_l2norm");
-  const bool fused = n->groups != 0;
-  if (fused) {
-    if ((r = check_rows(false, p->dtype, 1, p->heads, vl->total_q, p->head_dim, n->groups))) return r;
-    if (!n->q_rnorm || !n->k_rnorm) return fail(FCSA_ERR_INVALID, "q_rnorm / k_rnorm: null");
-  }
-  if ((r = backward_impl(p, vl, &n->q_hat, &n->k_hat, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed,
-                         zeroed_bytes, stream, fused ? n->q_rnorm : nullptr, fused ? n->k_rnorm : nullptr,
-                         fused ? n->groups : 1, deterministic)))
-    return r;
-  // zero gradients in the rows outside every sequence
-  fcsa::TailArgs ta = {};
-  ta.t[0] = {dq->ptr, dq->sh, dq->sn, p->heads, vl->total_q, vl->cu_seqlens_q};
-  ta.t[1] = {dk->ptr, dk->sh, dk->sn, p->kv_heads, vl->total_k, vl->cu_seqlens_k};
-  ta.t[2] = {dv->ptr, dv->sh, dv->sn, p->kv_heads, vl->total_k, vl->cu_seqlens_k};
-  return launch_varlen_tail(p, ta, 3, reinterpret_cast<cudaStream_t>(stream));
+  return check_varlen(p, vl) ? 0 : bwd_need(p, vl, false).zeroed;
 }
 
 int fcsa_backward_fused_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_l2norm* n,
                                const fcsa_tensor* v, const fcsa_tensor* o, const fcsa_tensor* d_o, const float* inv_l,
                                const fcsa_tensor* dq, const fcsa_tensor* dk, const fcsa_tensor* dv, void* workspace,
                                size_t workspace_bytes, void* zeroed, size_t zeroed_bytes, void* stream) {
-  return backward_varlen_impl(p, vl, n, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed, zeroed_bytes,
-                              stream, false);
+  return backward_l2norm(p, true, vl, n, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, zeroed,
+                         zeroed_bytes, stream, false);
 }
 
 size_t fcsa_backward_fused_deterministic_varlen_workspace_bytes(const fcsa_problem* p, const fcsa_varlen* vl) {
-  if (check_varlen(p, vl)) return 0;
-  return bwd_deterministic_bytes(bwd_layout(p, vl));
+  return check_varlen(p, vl) ? 0 : bwd_need(p, vl, true).scratch;
 }
 
 int fcsa_backward_fused_deterministic_varlen(const fcsa_problem* p, const fcsa_varlen* vl, const fcsa_l2norm* n,
@@ -1082,8 +1067,8 @@ int fcsa_backward_fused_deterministic_varlen(const fcsa_problem* p, const fcsa_v
                                              const float* inv_l, const fcsa_tensor* dq, const fcsa_tensor* dk,
                                              const fcsa_tensor* dv, void* workspace, size_t workspace_bytes,
                                              void* stream) {
-  return backward_varlen_impl(p, vl, n, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, nullptr, 0, stream,
-                              true);
+  return backward_l2norm(p, true, vl, n, v, o, d_o, inv_l, dq, dk, dv, workspace, workspace_bytes, nullptr, 0, stream,
+                         true);
 }
 
 }  // extern "C"

@@ -213,8 +213,30 @@ Workspaces workspaces_of_size(size_t need_s, size_t need_z, const Tensor& like, 
   return w;
 }
 
-Workspaces backward_workspaces(const fcsa_problem& p, const Tensor& like, cudaStream_t stream) {
+// The workspaces of a backward route, dense or packed sequences (vl): the deterministic one takes scratch only, the
+// default one scratch and zeroed.
+Workspaces backward_workspaces(const fcsa_problem& p, const fcsa_varlen* vl, bool deterministic, const Tensor& like,
+                               cudaStream_t stream) {
+  if (deterministic)
+    return workspaces_of_size(vl ? fcsa_backward_fused_deterministic_varlen_workspace_bytes(&p, vl)
+                                 : fcsa_backward_fused_deterministic_workspace_bytes(&p),
+                              0, like, stream, false);
+  if (vl)
+    return workspaces_of_size(fcsa_backward_fused_varlen_workspace_bytes(&p, vl),
+                              fcsa_backward_fused_varlen_zeroed_bytes(&p, vl), like, stream);
   return workspaces_of_size(fcsa_backward_workspace_bytes(&p), fcsa_backward_zeroed_bytes(&p), like, stream);
+}
+
+// The fcsa_l2norm of q^, k^ (view: their ABI addressing) and their rnorms; undefined tensors are passed as null
+fcsa_l2norm l2norm_of(const Tensor& q_hat, const Tensor& k_hat, const Tensor& q_rnorm, const Tensor& k_rnorm,
+                      int64_t groups, fcsa_tensor (*view)(const Tensor&)) {
+  fcsa_l2norm n;
+  n.groups = (int32_t)groups;
+  n.q_hat = q_hat.defined() ? view(q_hat) : fcsa_tensor{nullptr, 0, 0, 0};
+  n.k_hat = k_hat.defined() ? view(k_hat) : fcsa_tensor{nullptr, 0, 0, 0};
+  n.q_rnorm = q_rnorm.defined() ? q_rnorm.data_ptr<float>() : nullptr;
+  n.k_rnorm = k_rnorm.defined() ? k_rnorm.data_ptr<float>() : nullptr;
+  return n;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -330,10 +352,7 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> forward_ex(
     kn = at::empty(k.sizes(), k.options());
     rq = at::empty({sh.B, sh.H, sh.Nq, l2norm_groups}, q.options().dtype(at::kFloat));
     rk = at::empty({sh.B, sh.kv_heads, sh.Nk, l2norm_groups}, q.options().dtype(at::kFloat));
-    fcsa_l2norm n;
-    n.groups = (int32_t)l2norm_groups;
-    n.q_hat = view4(qn); n.k_hat = view4(kn);
-    n.q_rnorm = rq.data_ptr<float>(); n.k_rnorm = rk.data_ptr<float>();
+    const fcsa_l2norm n = l2norm_of(qn, kn, rq, rk, l2norm_groups, view4);
     FCSA_CHECK(fcsa_forward_fused(&p, &tq, &tk, &tv, &n, &to, inv_l_ptr, stream));
   } else if (has_bias) {
     const fcsa_bias b = bias_struct(*bias_prepared, bias_batch_dim, bias_amax);
@@ -379,32 +398,22 @@ std::tuple<Tensor, Tensor, Tensor, Tensor> backward_ex(
   const bool has_bias = bias_prepared.has_value() && bias_prepared->defined();
   const bool fused = q_rnorm.has_value() && q_rnorm->defined();
   Tensor db;
+  TORCH_CHECK(!deterministic || !has_bias, "backward_ex: the deterministic backward takes no attn_bias");
+  const Workspaces ws = backward_workspaces(p, nullptr, deterministic, q, stream);
+  void* wsp = ws.scratch.data_ptr();
+  const size_t wsn = (size_t)ws.scratch.numel();
+  TORCH_CHECK(!fused || (!has_bias && k_rnorm.has_value() && k_rnorm->defined() && groups > 0),
+              "backward_ex: bad fused-l2norm arguments");
+  const fcsa_l2norm n =
+      l2norm_of(q, k, fused ? *q_rnorm : Tensor(), fused ? *k_rnorm : Tensor(), fused ? groups : 0, view4);
   if (deterministic) {
-    TORCH_CHECK(!has_bias, "backward_ex: the deterministic backward takes no attn_bias");
-    const Tensor scratch =
-        workspaces_of_size(fcsa_backward_fused_deterministic_workspace_bytes(&p), 0, q, stream, false).scratch;
-    fcsa_l2norm n;
-    n.groups = fused ? (int32_t)groups : 0;
-    n.q_hat = tq; n.k_hat = tk;
-    n.q_rnorm = n.k_rnorm = nullptr;
-    if (fused) {
-      TORCH_CHECK(k_rnorm.has_value() && k_rnorm->defined() && groups > 0, "backward_ex: bad fused-l2norm arguments");
-      n.q_rnorm = q_rnorm->data_ptr<float>(); n.k_rnorm = k_rnorm->data_ptr<float>();
-    }
-    FCSA_CHECK(fcsa_backward_fused_deterministic(&p, &n, &tv, &to, &tdo, inv_l.data_ptr<float>(), &tdq, &tdk, &tdv,
-                                                 scratch.data_ptr(), (size_t)scratch.numel(), stream));
+    FCSA_CHECK(fcsa_backward_fused_deterministic(&p, &n, &tv, &to, &tdo, inv_l.data_ptr<float>(), &tdq, &tdk, &tdv, wsp,
+                                                 wsn, stream));
     return {dq, dk, dv, db};
   }
-  const Workspaces ws = backward_workspaces(p, q, stream);
-  void* wsp = ws.scratch.data_ptr();
   void* zsp = ws.zeroed.data_ptr();
-  const size_t wsn = (size_t)ws.scratch.numel(), zsn = (size_t)ws.zeroed.numel();
+  const size_t zsn = (size_t)ws.zeroed.numel();
   if (fused) {
-    TORCH_CHECK(!has_bias && k_rnorm.has_value() && k_rnorm->defined() && groups > 0, "backward_ex: bad fused-l2norm arguments");
-    fcsa_l2norm n;
-    n.groups = (int32_t)groups;
-    n.q_hat = tq; n.k_hat = tk;
-    n.q_rnorm = q_rnorm->data_ptr<float>(); n.k_rnorm = k_rnorm->data_ptr<float>();
     FCSA_CHECK(fcsa_backward_fused(&p, &n, &tv, &to, &tdo, inv_l.data_ptr<float>(), &tdq, &tdk, &tdv, wsp, wsn, zsp,
                                    zsn, stream));
   } else if (has_bias) {
@@ -520,71 +529,75 @@ std::tuple<Tensor, Tensor> decode_checks(const Tensor& q_in, const Tensor& k_cac
   return {k, v};
 }
 
-Tensor decode(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
-              const optional<Tensor>& k_in, const optional<Tensor>& v_in, double scale, double shift, bool causal,
-              int64_t groups, int64_t window, bool rolling) {
+// decode (cu_q = nullptr) and decode_varlen (cu_q, max_q: packed new tokens)
+Tensor decode_any(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
+                  const Tensor* cu_q, int64_t max_q, const optional<Tensor>& k_in, const optional<Tensor>& v_in,
+                  double scale, double shift, bool causal, int64_t groups, int64_t window, bool rolling) {
+  const bool packed = cu_q != nullptr;
   Tensor k, v;
-  std::tie(k, v) = decode_checks(q_in, k_cache, v_cache, cache_seqlens, k_in, v_in, false);
-  const int64_t B = q_in.size(0), H = q_in.size(1), Nq = q_in.size(2), D = q_in.size(3);
-  const int64_t Hk = k_cache.size(1), cap = k_cache.size(2);
-  const int64_t n_new = k.defined() ? k.size(2) : 0;
-  TORCH_CHECK(!rolling || !k.defined() || n_new == Nq, "decode: a rolling cache appends one k, v row per query (",
-              Nq, "), got ", n_new);
+  std::tie(k, v) = decode_checks(q_in, k_cache, v_cache, cache_seqlens, k_in, v_in, packed);
+  const int64_t B = k_cache.size(0), H = q_in.size(1), D = q_in.size(-1), Hk = k_cache.size(1), cap = k_cache.size(2);
+  const int64_t Nq = packed ? max_q : q_in.size(2), Tq = q_in.size(0);
+  const int64_t n_new = !packed && k.defined() ? k.size(2) : 0;
+  if (packed) {
+    TORCH_CHECK(cu_q->is_cuda() && cu_q->get_device() == q_in.get_device() && cu_q->scalar_type() == at::kInt &&
+                    cu_q->dim() == 1 && cu_q->size(0) == B + 1,
+                "decode_varlen: cu_seqlens_q must be an int32 tensor of shape (", B + 1, ",) on q's device");
+    TORCH_CHECK(cu_q->is_contiguous(),
+                "decode_varlen: cu_seqlens_q must be contiguous (not a strided or expanded view)");
+    TORCH_CHECK(max_q >= 1 && max_q <= 0x7FFFFFFF, "decode_varlen: max_seqlen_q must be a positive int32 value");
+    TORCH_CHECK(Tq <= 0x7FFFFFFF, "decode_varlen: too many packed rows");
+  } else {
+    TORCH_CHECK(!rolling || !k.defined() || n_new == Nq, "decode: a rolling cache appends one k, v row per query (",
+                Nq, "), got ", n_new);
+  }
   const c10::cuda::CUDAGuard guard(q_in.device());
   const Tensor q = tma_ready(q_in);
   const fcsa_problem p =
       build_problem("decode: ", q, B, H, Hk, Nq, cap, D, scale, shift, causal, c10::nullopt, false, window);
-  Tensor o = at::empty({B, H, Nq, D}, q.options());
+  Tensor o = at::empty(q.sizes(), q.options());
+  if (packed && Tq == 0) return o;
   cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
+  const int32_t* cu = packed ? cu_q->data_ptr<int32_t>() : nullptr;
+  const int32_t total_q = packed ? (int32_t)Tq : 0;
   const Tensor scratch =
-      workspaces_of_size(rolling ? fcsa_decode_rolling_workspace_bytes(&p, nullptr, 0)
-                                 : fcsa_decode_workspace_bytes(&p, (int32_t)n_new),
+      workspaces_of_size(rolling  ? fcsa_decode_rolling_workspace_bytes(&p, cu, total_q)
+                         : packed ? fcsa_decode_varlen_workspace_bytes(&p, total_q)
+                                  : fcsa_decode_workspace_bytes(&p, (int32_t)n_new),
                          0, q, stream, false).scratch;
-  const fcsa_tensor tq = view4(q), tkc = view4(k_cache), tvc = view4(v_cache), to = view4(o);
-  fcsa_tensor tk = {nullptr, 0, 0, 0}, tv = {nullptr, 0, 0, 0};
-  if (k.defined()) { tk = view4(k); tv = view4(v); }
+  const auto view = packed ? view_packed : view4;
+  const fcsa_tensor tq = view(q), tkc = view4(k_cache), tvc = view4(v_cache), to = view(o);
+  fcsa_tensor tk, tv;
+  if (k.defined()) { tk = view(k); tv = view(v); }
+  const fcsa_tensor* pk = k.defined() ? &tk : nullptr;
+  const fcsa_tensor* pv = k.defined() ? &tv : nullptr;
+  const int32_t* seqlens = cache_seqlens.data_ptr<int32_t>();
+  void* ws = scratch.data_ptr();
+  const size_t wsn = (size_t)scratch.numel();
   if (rolling)
-    FCSA_CHECK(fcsa_decode_rolling(&p, nullptr, 0, &tq, &tkc, &tvc, cache_seqlens.data_ptr<int32_t>(),
-                                   k.defined() ? &tk : nullptr, k.defined() ? &tv : nullptr, (int32_t)groups, &to,
-                                   scratch.data_ptr(), (size_t)scratch.numel(), stream));
+    FCSA_CHECK(fcsa_decode_rolling(&p, cu, total_q, &tq, &tkc, &tvc, seqlens, pk, pv, (int32_t)groups, &to, ws, wsn,
+                                   stream));
+  else if (packed)
+    FCSA_CHECK(fcsa_decode_varlen(&p, cu, total_q, &tq, &tkc, &tvc, seqlens, pk, pv, (int32_t)groups, &to, ws, wsn,
+                                  stream));
   else
-    FCSA_CHECK(fcsa_decode(&p, &tq, &tkc, &tvc, cache_seqlens.data_ptr<int32_t>(), &tk, &tv, (int32_t)n_new,
-                           (int32_t)groups, &to, scratch.data_ptr(), (size_t)scratch.numel(), stream));
+    FCSA_CHECK(
+        fcsa_decode(&p, &tq, &tkc, &tvc, seqlens, pk, pv, (int32_t)n_new, (int32_t)groups, &to, ws, wsn, stream));
   return o;
 }
 
-Tensor decode_varlen(const Tensor& q_in, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
-                     const Tensor& cu_q, int64_t max_q, const optional<Tensor>& k_in, const optional<Tensor>& v_in,
+Tensor decode(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
+              const optional<Tensor>& k, const optional<Tensor>& v, double scale, double shift, bool causal,
+              int64_t groups, int64_t window, bool rolling) {
+  return decode_any(q, k_cache, v_cache, cache_seqlens, nullptr, 0, k, v, scale, shift, causal, groups, window,
+                    rolling);
+}
+
+Tensor decode_varlen(const Tensor& q, const Tensor& k_cache, const Tensor& v_cache, const Tensor& cache_seqlens,
+                     const Tensor& cu_q, int64_t max_q, const optional<Tensor>& k, const optional<Tensor>& v,
                      double scale, double shift, bool causal, int64_t groups, int64_t window, bool rolling) {
-  Tensor k, v;
-  std::tie(k, v) = decode_checks(q_in, k_cache, v_cache, cache_seqlens, k_in, v_in, true);
-  const int64_t B = k_cache.size(0), H = q_in.size(1), Tq = q_in.size(0), D = q_in.size(2);
-  const int64_t Hk = k_cache.size(1), cap = k_cache.size(2);
-  TORCH_CHECK(cu_q.is_cuda() && cu_q.get_device() == q_in.get_device() && cu_q.scalar_type() == at::kInt &&
-                  cu_q.dim() == 1 && cu_q.size(0) == B + 1,
-              "decode_varlen: cu_seqlens_q must be an int32 tensor of shape (", B + 1, ",) on q's device");
-  TORCH_CHECK(cu_q.is_contiguous(), "decode_varlen: cu_seqlens_q must be contiguous (not a strided or expanded view)");
-  TORCH_CHECK(max_q >= 1 && max_q <= 0x7FFFFFFF, "decode_varlen: max_seqlen_q must be a positive int32 value");
-  TORCH_CHECK(Tq <= 0x7FFFFFFF, "decode_varlen: too many packed rows");
-  const c10::cuda::CUDAGuard guard(q_in.device());
-  const Tensor q = tma_ready(q_in);
-  const fcsa_problem p =
-      build_problem("decode: ", q, B, H, Hk, max_q, cap, D, scale, shift, causal, c10::nullopt, false, window);
-  Tensor o = at::empty({Tq, H, D}, q.options());
-  if (Tq == 0) return o;
-  cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
-  const int32_t* cu = cu_q.data_ptr<int32_t>();
-  const Tensor scratch =
-      workspaces_of_size(rolling ? fcsa_decode_rolling_workspace_bytes(&p, cu, (int32_t)Tq)
-                                 : fcsa_decode_varlen_workspace_bytes(&p, (int32_t)Tq),
-                         0, q, stream, false).scratch;
-  const fcsa_tensor tq = view_packed(q), tkc = view4(k_cache), tvc = view4(v_cache), to = view_packed(o);
-  fcsa_tensor tk, tv;
-  if (k.defined()) { tk = view_packed(k); tv = view_packed(v); }
-  const auto run = rolling ? fcsa_decode_rolling : fcsa_decode_varlen;
-  FCSA_CHECK(run(&p, cu, (int32_t)Tq, &tq, &tkc, &tvc, cache_seqlens.data_ptr<int32_t>(), k.defined() ? &tk : nullptr,
-                 k.defined() ? &tv : nullptr, (int32_t)groups, &to, scratch.data_ptr(), (size_t)scratch.numel(), stream));
-  return o;
+  return decode_any(q, k_cache, v_cache, cache_seqlens, &cu_q, max_q, k, v, scale, shift, causal, groups, window,
+                    rolling);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -640,18 +653,13 @@ std::tuple<Tensor, Tensor, Tensor, Tensor, Tensor, Tensor> forward_varlen(
   Tensor inv_l;
   if (need_inv_l) inv_l = at::empty({H, Tq}, q.options().dtype(at::kFloat));
   Tensor qn, kn, rq, rk;
-  fcsa_l2norm n;
-  n.groups = (int32_t)groups;
-  n.q_hat = n.k_hat = fcsa_tensor{nullptr, 0, 0, 0};
-  n.q_rnorm = n.k_rnorm = nullptr;
   if (groups > 0) {
     qn = at::empty(q.sizes(), q.options());
     kn = at::empty(k.sizes(), k.options());
     rq = at::empty({H, Tq, groups}, q.options().dtype(at::kFloat));
     rk = at::empty({Hk, Tk, groups}, q.options().dtype(at::kFloat));
-    n.q_hat = view_packed(qn); n.k_hat = view_packed(kn);
-    n.q_rnorm = rq.data_ptr<float>(); n.k_rnorm = rk.data_ptr<float>();
   }
+  const fcsa_l2norm n = l2norm_of(qn, kn, rq, rk, groups, view_packed);
   const fcsa_tensor tq = view_packed(q), tk = view_packed(k), tv = view_packed(v), to = view_packed(o);
   FCSA_CHECK(fcsa_forward_fused_varlen(&vr.p, &vr.vl, &tq, &tk, &tv, &n, &to, need_inv_l ? inv_l.data_ptr<float>() : nullptr,
                                        at::cuda::getCurrentCUDAStream().stream()));
@@ -678,30 +686,21 @@ std::tuple<Tensor, Tensor, Tensor> backward_varlen(
   Tensor dk = at::empty(k.sizes(), k.options());
   Tensor dv = at::empty(v.sizes(), v.options());
   cudaStream_t stream = at::cuda::getCurrentCUDAStream().stream();
-  fcsa_l2norm n;
-  n.groups = (int32_t)groups;
-  n.q_hat = view_packed(q); n.k_hat = view_packed(k);
-  n.q_rnorm = n.k_rnorm = nullptr;
-  if (groups > 0) {
-    TORCH_CHECK(q_rnorm.has_value() && q_rnorm->defined() && k_rnorm.has_value() && k_rnorm->defined(),
-                "backward_varlen: q_rnorm and k_rnorm are needed with groups > 0");
-    n.q_rnorm = q_rnorm->data_ptr<float>(); n.k_rnorm = k_rnorm->data_ptr<float>();
-  }
+  TORCH_CHECK(groups <= 0 || (q_rnorm.has_value() && q_rnorm->defined() && k_rnorm.has_value() && k_rnorm->defined()),
+              "backward_varlen: q_rnorm and k_rnorm are needed with groups > 0");
+  const fcsa_l2norm n = l2norm_of(q, k, groups > 0 ? *q_rnorm : Tensor(), groups > 0 ? *k_rnorm : Tensor(), groups,
+                                  view_packed);
   const fcsa_tensor tv = view_packed(v), to = view_packed(o), tdo = view_packed(d_o), tdq = view_packed(dq),
                     tdk = view_packed(dk), tdv = view_packed(dv);
-  if (deterministic) {
-    const Tensor scratch = workspaces_of_size(fcsa_backward_fused_deterministic_varlen_workspace_bytes(&vr.p, &vr.vl), 0,
-                                              q, stream, false).scratch;
+  const Workspaces ws = backward_workspaces(vr.p, &vr.vl, deterministic, q, stream);
+  if (deterministic)
     FCSA_CHECK(fcsa_backward_fused_deterministic_varlen(&vr.p, &vr.vl, &n, &tv, &to, &tdo, inv_l.data_ptr<float>(),
-                                                        &tdq, &tdk, &tdv, scratch.data_ptr(),
-                                                        (size_t)scratch.numel(), stream));
-    return {dq, dk, dv};
-  }
-  const Workspaces ws = workspaces_of_size(fcsa_backward_fused_varlen_workspace_bytes(&vr.p, &vr.vl),
-                                           fcsa_backward_fused_varlen_zeroed_bytes(&vr.p, &vr.vl), q, stream);
-  FCSA_CHECK(fcsa_backward_fused_varlen(&vr.p, &vr.vl, &n, &tv, &to, &tdo, inv_l.data_ptr<float>(), &tdq, &tdk, &tdv,
-                                        ws.scratch.data_ptr(), (size_t)ws.scratch.numel(), ws.zeroed.data_ptr(),
-                                        (size_t)ws.zeroed.numel(), stream));
+                                                        &tdq, &tdk, &tdv, ws.scratch.data_ptr(),
+                                                        (size_t)ws.scratch.numel(), stream));
+  else
+    FCSA_CHECK(fcsa_backward_fused_varlen(&vr.p, &vr.vl, &n, &tv, &to, &tdo, inv_l.data_ptr<float>(), &tdq, &tdk, &tdv,
+                                          ws.scratch.data_ptr(), (size_t)ws.scratch.numel(), ws.zeroed.data_ptr(),
+                                          (size_t)ws.zeroed.numel(), stream));
   return {dq, dk, dv};
 }
 
